@@ -220,6 +220,10 @@ GrB_Info B200_device_synchronize(void);
 int B200_have_device(void);
 /* statistics of the last hot-path call: kernel launch count (cumulative) */
 uint64_t B200_kernel_launches(void);
+/* allocation test seam: the k-th device allocation from now fails with GrB_OUT_OF_MEMORY before it reaches
+ * the device (k = 0 switches it off); and the number of device blocks allocated and not yet freed */
+void B200_debug_fail_alloc(int64_t k);
+int64_t B200_debug_live_allocs(void);
 /* per-matrix SpGEMM/SpMV work figures of the most recent GrB_mxm (flops = number of
  * multiplies, nnz_out = nvals of the semiring product before accum/mask) */
 GrB_Info B200_last_mxm_stats(uint64_t *flops, uint64_t *nnz_out);

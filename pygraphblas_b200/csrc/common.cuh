@@ -14,6 +14,8 @@
 #include <string>
 #include <vector>
 #include <mutex>
+#include <type_traits>
+#include <utility>
 #include "../../include/b200grb.h"
 
 #define GB_MAGIC 0x42323030  /* "B200" */
@@ -57,37 +59,86 @@ enum UnaryCode : int {
     UOP_COUNT
 };
 
-// Device CSR panel: rows sorted, columns sorted inside each row.
-struct Csr {
-    int64_t nrows = 0, ncols = 0, nnz = 0;
-    int64_t *rowptr = nullptr;     // [nrows+1] 64-bit offsets (canonical)
-    uint32_t *rowptr32 = nullptr;  // [nrows+1] 32-bit shadow, built when nnz < 2^32
-    uint32_t *col = nullptr;       // [nnz]
-    void *val = nullptr;           // [nnz] of the matrix type
-    // SpMV plan: first row of every TILE-sized slice of the nnz range (spmv.cu)
-    uint32_t *tile_row = nullptr;
+// device memory (stream-ordered pool on G.stream)
+GrB_Info dmalloc(void **p, size_t bytes, std::string *err);
+void dfree(void *p);
+template <typename T> static inline GrB_Info dalloc(T **p, size_t count, std::string *err) {
+    return dmalloc((void **)p, count * sizeof(T) + 16, err);   // +16: bulk copies may over-read a tail
+}
+
+// Owner of one dmalloc block, released at scope exit (stream-ordered after the kernels already enqueued).  It converts
+// to the raw pointer, so it can stand wherever a device pointer is read.  DevBuf<void> takes an exact byte count.
+template <typename T> class DevBuf {
+    T *p_ = nullptr;
+public:
+    DevBuf() = default;                 // move-only: declaring the moves deletes the copies
+    DevBuf(DevBuf &&o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+    DevBuf &operator=(DevBuf &&o) noexcept { if (this != &o) { reset(); p_ = o.p_; o.p_ = nullptr; } return *this; }
+    ~DevBuf() { reset(); }
+    GrB_Info alloc(size_t count, std::string *err) {
+        reset();
+        if constexpr (std::is_void<T>::value) return dmalloc(&p_, count, err);
+        else return dalloc(&p_, count, err);
+    }
+    T *get() const { return p_; }
+    operator T *() const { return p_; }
+    template <typename U> explicit operator U *() const { return (U *)p_; }
+    T *release() { T *q = p_; p_ = nullptr; return q; }
+    void reset() { dfree(p_); p_ = nullptr; }
+};
+
+// SpMV tile plan (spmv.cu): first row of every TILE-sized slice of the nnz range
+struct TilePlan {
+    DevBuf<uint32_t> row;            // [ntiles+1]
     int64_t ntiles = 0;
-    int tile_size = 0;
-    // run plan (spmv.cu, dense-u kernel): entries cut into warp-sized runs of 256
-    uint32_t *run_headw = nullptr;   // [ceil(nnz/32)] bit q = entry q starts a row
-    uint16_t *run_lane = nullptr;    // [nruns*32] row starts inside the run before the lane's first entry
-    uint32_t *run_base = nullptr;    // [nruns+1] row starts before the run (= rank of its first row start)
-    int32_t *run_tail_row = nullptr; // [nruns] row still open at the end of the run (its last row start), or -1
-    uint32_t *run_tail_last = nullptr; // [nruns] last run that row reaches
-    uint32_t *nzrow = nullptr;       // [nnzrows] ids of the non-empty rows, ascending
-    uint8_t *pres_tmpl = nullptr;    // [nrows] 1 where the row is non-empty
+    int size = 0;
+};
+// run plan (spmv_run.cu, warp-independent kernels): entries cut into warp-sized runs of 256
+struct RunPlan {
+    DevBuf<uint32_t> headw;          // [ceil(nnz/32)] bit q = entry q starts a row
+    DevBuf<uint16_t> lane;           // [nruns*32] row starts inside the run before the lane's first entry
+    DevBuf<uint32_t> base;           // [nruns+1] row starts before the run (= rank of its first row start)
+    DevBuf<int32_t> tail_row;        // [nruns] row still open at the end of the run (its last row start), or -1
+    DevBuf<uint32_t> tail_last;      // [nruns] last run that row reaches
+    DevBuf<uint32_t> nzrow;          // [nnzrows] ids of the non-empty rows, ascending
+    DevBuf<uint8_t> pres_tmpl;       // [nrows] 1 where the row is non-empty
     int64_t nruns = 0, nnzrows = 0;
-    // hot-column plan (spmv_run.cu): the henc most referenced columns get their rank as id, the others col + henc
-    uint32_t *hperm = nullptr;     // [henc] hot rank -> original column
-    uint32_t *hcol = nullptr;      // [nnz] encoded column ids
-    uint32_t henc = 0;             // ids below this are hot ranks
-    bool hot_planned = false;      // the plan was attempted (hcol stays NULL when the gathers are not concentrated)
-    double hot_cover = 0.0;        // share of the entries whose column is among the henc most referenced
     // per-call scratch of the run kernels, kept with the plan (no allocation on the call path)
-    void *ws_head = nullptr, *ws_tail = nullptr;   // [nruns] x 8 bytes: partials of the rows a run starts / ends inside
-    uint8_t *ws_head_has = nullptr, *ws_tail_has = nullptr;
-    void *ws_uhot = nullptr;       // [henc] x 8 bytes: u at the hot columns
+    DevBuf<void> ws_head, ws_tail;   // [nruns] x 8 bytes: partials of the rows a run starts / ends inside
+    DevBuf<uint8_t> ws_head_has, ws_tail_has;
+};
+// hot-column plan (spmv_run.cu): the henc most referenced columns get their rank as id, the others col + henc
+struct HotPlan {
+    DevBuf<uint32_t> perm;           // [henc] hot rank -> original column
+    DevBuf<uint32_t> col;            // [nnz] encoded column ids
+    DevBuf<void> ws_uhot;            // [henc] x 8 bytes: u at the hot columns
+    uint32_t henc = 0;               // ids below this are hot ranks
+    bool planned = false;            // the plan was attempted (col stays NULL when the gathers are not concentrated)
+    double cover = 0.0;              // share of the entries whose column is among the henc most referenced
+};
+
+// Device CSR panel: rows sorted, columns sorted inside each row.  Owns its arrays and cached plans.
+struct CsrFields {
+    int64_t nrows = 0, ncols = 0, nnz = 0;
+    DevBuf<int64_t> rowptr;          // [nrows+1] 64-bit offsets (canonical)
+    DevBuf<uint32_t> rowptr32;       // [nrows+1] 32-bit shadow, built when nnz < 2^32
+    DevBuf<uint32_t> col;            // [nnz]
+    DevBuf<void> val;                // [nnz] of the matrix type
+    // cached SpMV plans, each either complete or absent
+    TilePlan tile;
+    RunPlan run;
+    HotPlan hot;
     bool valid = false;
+};
+// A move is the member-wise move of every field, then a reset of the source: a moved-from Csr is empty, not
+// "valid with null arrays", whatever fields are added later.
+struct Csr : CsrFields {
+    Csr() = default;
+    Csr(Csr &&o) noexcept : CsrFields(std::move(o)) { o.clear(); }
+    Csr &operator=(Csr &&o) noexcept { if (this != &o) { CsrFields::operator=(std::move(o)); o.clear(); } return *this; }
+    void clear() { static_cast<CsrFields &>(*this) = CsrFields(); }
+    // the cached SpMV plans and scratch (dropped whenever the structure changes)
+    void drop_plans() { tile = TilePlan(); run = RunPlan(); hot = HotPlan(); }
 };
 
 // per-object storage hints of SuiteSparse's GxB_*_Option_set/get: recorded and reported back, without effect on the HBM
@@ -181,14 +232,6 @@ struct GbBurble {
     ~GbBurble();
 };
 
-// device memory (stream-ordered pool on G.stream)
-GrB_Info dmalloc(void **p, size_t bytes, std::string *err);
-void dfree(void *p);
-template <typename T> static inline GrB_Info dalloc(T **p, size_t count, std::string *err) {
-    return dmalloc((void **)p, count * sizeof(T) + 16, err);   // +16: bulk copies may over-read a tail
-}
-void csr_free(Csr &c);
-void csr_drop_plans(Csr &c);
 // Persistent scratch of the compute calls: slot k keeps its buffer between calls and only grows (calls are serialised on one
 // stream, so a slot is never in use twice).  Large transient cudaMallocAsync / cudaFreeAsync pairs were measured to cost
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
@@ -205,7 +248,7 @@ GrB_Info matrix_ensure_host(GrB_Matrix A);
 GrB_Info matrix_ensure_device(GrB_Matrix A);
 GrB_Info matrix_ensure_transpose(GrB_Matrix A);     // builds A->devT on the device
 void matrix_invalidate_device(GrB_Matrix A);
-void matrix_adopt_device(GrB_Matrix A, Csr &c);     // A takes ownership of c, host form dropped
+void matrix_adopt_device(GrB_Matrix A, Csr &&c);    // A takes ownership of c, host form dropped
 GrB_Info vector_ensure_host(GrB_Vector v);
 GrB_Info vector_ensure_device(GrB_Vector v);
 void vector_invalidate_device(GrB_Vector v);
@@ -224,24 +267,25 @@ GrB_Info hyper_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
                    const GrB_Descriptor desc);
 DescFlags desc_flags(const GrB_Descriptor d);
 
-// w<mask> = accum(w, T) on the device (vector_ops.cu).  T = (tval, tpres) of type ttc over w->n positions
-// (tpres NULL: every position present; t_scalar: tval is ONE value standing for all positions).  region
-// (NULL = everything) limits the write to the positions it flags, GrB_assign style.  own_t: T's buffers are
-// released here.
 struct Sc;
 // C<Mask> = accum(C, T) for a CSR T of type ttc (spgemm.cu); consumes T
 GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f,
-                          Csr &T, int ttc, bool t_already_masked, std::string *err);
+                          Csr &&T, int ttc, bool t_already_masked, std::string *err);
 // fold of n values (presence bytes optional) with a builtin monoid operator on the device (vector_ops.cu)
 GrB_Info dev_reduce_values(const void *val, const uint8_t *pres, int vtc, int64_t n, int op, int mtc, Sc *out, bool *has, std::string *err);
+// w<mask> = accum(w, T) on the device (vector_ops.cu).  T = (tval, tpres) of type ttc over w->n positions
+// (tpres NULL: every position present; t_scalar: tval is ONE value standing for all positions).  region
+// (NULL = everything) limits the write to the positions it flags, GrB_assign style.  own_val / own_pres hold
+// T's buffers when the caller hands them over (w may then adopt them); empty when T is borrowed.
 GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const DescFlags &f,
-                      void *tval, uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region, bool own_t);
+                      const void *tval, const uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region,
+                      DevBuf<void> &&own_val = DevBuf<void>(), DevBuf<uint8_t> &&own_pres = DevBuf<uint8_t>());
 
 // kernels (device_ops.cu / spmv.cu / spgemm.cu)
 GrB_Info dev_build_rowptr32(Csr &c, std::string *err);
 GrB_Info dev_exclusive_scan(int64_t *data, int64_t n, std::string *err);
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err);
-GrB_Info dev_cast_values(void **out, int to_code, const void *in, int from_code, int64_t n, std::string *err);
+GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int from_code, int64_t n, std::string *err);
 GrB_Info dev_count_present(const uint8_t *pres, int64_t n, int64_t *count, std::string *err);
 
 // ---------------------------------------------------------------- scalar carrier

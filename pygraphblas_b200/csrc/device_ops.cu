@@ -65,12 +65,11 @@ GrB_Info dev_exclusive_scan(int64_t *data, int64_t n, std::string *err) {
         scan_block_apply<<<1, SCAN_THREADS, 0, G.stream>>>(data, n, nullptr); GB_LAUNCHED();
         return GrB_SUCCESS;
     }
-    int64_t *totals = nullptr;
-    GB_TRY(dalloc(&totals, (size_t)nb, err));
+    DevBuf<int64_t> totals;
+    GB_TRY(totals.alloc((size_t)nb, err));
     scan_block_totals<<<(unsigned)nb, SCAN_THREADS, 0, G.stream>>>(data, n, totals); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(totals, nb, err));
     scan_block_apply<<<(unsigned)nb, SCAN_THREADS, 0, G.stream>>>(data, n, totals); GB_LAUNCHED();
-    dfree(totals);
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
@@ -81,14 +80,16 @@ __global__ void narrow_rowptr_kernel(const int64_t *rp, uint32_t *rp32, int64_t 
         rp32[i] = (uint32_t)rp[i];
 }
 GrB_Info dev_build_rowptr32(Csr &c, std::string *err) {
-    dfree(c.rowptr32); c.rowptr32 = nullptr;
-    csr_drop_plans(c);
+    c.rowptr32.reset();
+    c.drop_plans();
     if (c.nnz >= ((int64_t)1 << 32)) return GrB_SUCCESS;
-    GB_TRY(dalloc(&c.rowptr32, (size_t)c.nrows + 1, err));
+    DevBuf<uint32_t> rp32;
+    GB_TRY(rp32.alloc((size_t)c.nrows + 1, err));
     const int64_t n = c.nrows + 1;
     const int blocks = (int)std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 8);
-    narrow_rowptr_kernel<<<blocks, 256, 0, G.stream>>>(c.rowptr, c.rowptr32, n); GB_LAUNCHED();
+    narrow_rowptr_kernel<<<blocks, 256, 0, G.stream>>>(c.rowptr, rp32, n); GB_LAUNCHED();
     CU_TRY(cudaGetLastError(), err);
+    c.rowptr32 = std::move(rp32);
     return GrB_SUCCESS;
 }
 
@@ -132,25 +133,24 @@ static inline int grid_for(int64_t n, int threads = 256) {
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err) {
     if (a.nnz >= ((int64_t)1 << 32)) return gb_fail(GrB_INVALID_VALUE, err, "transpose: nnz >= 2^32 not supported");
     t = Csr(); t.nrows = a.ncols; t.ncols = a.nrows; t.nnz = a.nnz;
-    GB_TRY(dalloc(&t.rowptr, (size_t)t.nrows + 1, err));
-    GB_TRY(dalloc(&t.col, (size_t)t.nnz, err));
-    GB_TRY(dmalloc(&t.val, (size_t)t.nnz * vsize + 16, err));
+    GB_TRY(t.rowptr.alloc((size_t)t.nrows + 1, err));
+    GB_TRY(t.col.alloc((size_t)t.nnz, err));
+    GB_TRY(t.val.alloc((size_t)t.nnz * vsize + 16, err));
     CU_TRY(cudaMemsetAsync(t.rowptr, 0, ((size_t)t.nrows + 1) * 8, G.stream), err);
     if (a.nnz > 0) {
-        uint32_t *rowid = nullptr, *perm_in = nullptr, *perm_out = nullptr, *keys_out = nullptr;
-        GB_TRY(dalloc(&rowid, (size_t)a.nnz, err)); GB_TRY(dalloc(&perm_in, (size_t)a.nnz, err));
-        GB_TRY(dalloc(&perm_out, (size_t)a.nnz, err)); GB_TRY(dalloc(&keys_out, (size_t)a.nnz, err));
+        DevBuf<uint32_t> rowid, perm_in, perm_out, keys_out;
+        GB_TRY(rowid.alloc((size_t)a.nnz, err)); GB_TRY(perm_in.alloc((size_t)a.nnz, err));
+        GB_TRY(perm_out.alloc((size_t)a.nnz, err)); GB_TRY(keys_out.alloc((size_t)a.nnz, err));
         expand_rows_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a.rowptr, a.nrows, rowid); GB_LAUNCHED();
         count_cols_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a.col, a.nnz, t.rowptr); GB_LAUNCHED();
         iota_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(perm_in, a.nnz); GB_LAUNCHED();
         int end_bit = 1; while (end_bit < 32 && ((int64_t)1 << end_bit) < a.ncols) ++end_bit;
         size_t tmp_bytes = 0;
-        CU_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, a.col, keys_out, perm_in, perm_out, (int64_t)a.nnz, 0, end_bit, G.stream), err);
-        void *tmp = nullptr; GB_TRY(dmalloc(&tmp, tmp_bytes, err));
-        CU_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, a.col, keys_out, perm_in, perm_out, (int64_t)a.nnz, 0, end_bit, G.stream), err);
+        CU_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, a.col.get(), keys_out.get(), perm_in.get(), perm_out.get(), (int64_t)a.nnz, 0, end_bit, G.stream), err);
+        DevBuf<void> tmp; GB_TRY(tmp.alloc(tmp_bytes, err));
+        CU_TRY(cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, a.col.get(), keys_out.get(), perm_in.get(), perm_out.get(), (int64_t)a.nnz, 0, end_bit, G.stream), err);
         G.launches += 8;
         permute_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(perm_out, rowid, (const uint8_t *)a.val, (int)vsize, a.nnz, t.col, (uint8_t *)t.val); GB_LAUNCHED();
-        dfree(tmp); dfree(rowid); dfree(perm_in); dfree(perm_out); dfree(keys_out);
     }
     GB_TRY(dev_exclusive_scan(t.rowptr, t.nrows + 1, err));
     GB_TRY(dev_build_rowptr32(t, err));
@@ -163,9 +163,9 @@ __global__ void cast_kernel(void *out, int to, const void *in, int from, int64_t
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
         sc_store(to, out, (size_t)k, sc_cast(sc_load(from, in, (size_t)k), from, to));
 }
-GrB_Info dev_cast_values(void **out, int to_code, const void *in, int from_code, int64_t n, std::string *err) {
-    GB_TRY(dmalloc(out, (size_t)n * tc_size(to_code) + 16, err));
-    if (n > 0) { cast_kernel<<<grid_for(n), 256, 0, G.stream>>>(*out, to_code, in, from_code, n); GB_LAUNCHED(); }
+GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int from_code, int64_t n, std::string *err) {
+    GB_TRY(out.alloc((size_t)n * tc_size(to_code) + 16, err));
+    if (n > 0) { cast_kernel<<<grid_for(n), 256, 0, G.stream>>>(out, to_code, in, from_code, n); GB_LAUNCHED(); }
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
@@ -178,14 +178,13 @@ __global__ void count_present_kernel(const uint8_t *pres, int64_t n, unsigned lo
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
 GrB_Info dev_count_present(const uint8_t *pres, int64_t n, int64_t *count, std::string *err) {
-    unsigned long long *d = nullptr;
-    GB_TRY(dalloc(&d, 1, err));
+    DevBuf<unsigned long long> d;
+    GB_TRY(d.alloc(1, err));
     CU_TRY(cudaMemsetAsync(d, 0, 8, G.stream), err);
     count_present_kernel<<<grid_for(n), 256, 0, G.stream>>>(pres, n, d); GB_LAUNCHED();
     unsigned long long h = 0;
     CU_TRY(cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
-    dfree(d);
     *count = (int64_t)h;
     return GrB_SUCCESS;
 }

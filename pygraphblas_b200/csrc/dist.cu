@@ -236,15 +236,15 @@ extern "C" GrB_Info B200_Comm_allgather(B200_Comm c, const GrB_Vector slice, GrB
                                                             (unsigned long long)row0, (unsigned long long)slice->n);
     GbBurble burble("B200_Comm_allgather");
     GB_TRY(vector_ensure_device(slice));
-    const uint8_t *pres = slice->dpres; uint8_t *ones = nullptr;
+    const uint8_t *pres = slice->dpres; DevBuf<uint8_t> ones;
     if (!pres) {                                                           // a full slice: its presence is all ones
-        GB_TRY(dalloc(&ones, (size_t)slice->n + 16, &c->err));
+        GB_TRY(ones.alloc((size_t)slice->n + 16, &c->err));
         fill_bytes_kernel<<<cgrid(slice->n), 256, 0, G.stream>>>(ones, (int64_t)slice->n + 16, 1); GB_LAUNCHED();
         pres = ones;
     }
     const int which = (int)((c->step + 1) & 1);
     GrB_Info r = comm_push_and_wait(c, slice->dval, pres, row0, slice->n, which);
-    dfree(ones);
+    ones.reset();
     burble.note("peer push (NVLink stores) + flag wait", (double)slice->n * (c->esize + 1) * (c->world - 1));
     return r;
 }
@@ -274,9 +274,9 @@ extern "C" GrB_Info B200_Comm_allreduce(B200_Comm c, const GrB_Vector partial, G
     const uint64_t per = ((c->n + (uint64_t)c->world - 1) / c->world + 15) & ~(uint64_t)15;
     const uint64_t e0 = std::min<uint64_t>(c->n, per * (uint64_t)c->rank), e1 = std::min<uint64_t>(c->n, e0 + per);
     const int64_t cnt = (int64_t)(e1 - e0);
-    void *oval = nullptr; uint8_t *opres = nullptr;
-    GB_TRY(dmalloc(&oval, (size_t)cnt * c->esize + 32, &c->err));
-    GB_TRY(dalloc(&opres, (size_t)cnt + 16, &c->err));
+    DevBuf<void> oval; DevBuf<uint8_t> opres;
+    GB_TRY(oval.alloc((size_t)cnt * c->esize + 32, &c->err));
+    GB_TRY(opres.alloc((size_t)cnt + 16, &c->err));
     PeerPtrs part{}; for (int p = 0; p < c->world; ++p) part.p[p] = comm_buf(c, c->peer[p], 2);
     if (cnt > 0) switch (tc) {
         case TC_BOOL: launch_fold<bool>(c, part, (int64_t)e0, cnt, op, oval, opres); break;
@@ -293,7 +293,7 @@ extern "C" GrB_Info B200_Comm_allreduce(B200_Comm c, const GrB_Vector partial, G
     }
     const int which = (int)(step & 1);
     GrB_Info r = comm_push_and_wait(c, oval, opres, e0, (uint64_t)cnt, which);
-    dfree(oval); dfree(opres);
+    oval.reset(); opres.reset();
     burble.note("peer fold (NVLink loads, rank order) + peer push + flag waits", (double)c->n * (c->esize + 1) * 2.0 * (c->world - 1) / c->world);
     return r;
 }

@@ -35,9 +35,9 @@ static GrB_BinaryOp second_op(int tc) {
     }
 }
 
-template <typename T> static GrB_Info upload(const std::vector<T> &h, T **d, std::string *err) {
-    GB_TRY(dalloc(d, h.size(), err));
-    if (!h.empty()) CU_TRY(cudaMemcpyAsync(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, G.stream), err);
+template <typename T> static GrB_Info upload(const std::vector<T> &h, DevBuf<T> &d, std::string *err) {
+    GB_TRY(d.alloc(h.size(), err));
+    if (!h.empty()) CU_TRY(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);          // h is a caller-owned temporary
     return GrB_SUCCESS;
 }
@@ -51,11 +51,10 @@ static GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
 struct Region {
     bool all_rows = true, all_cols = true;
     std::vector<uint64_t> I, J;          // as given (after expansion), empty when all
-    uint8_t *rowflag = nullptr;          // [nrows] 1 where the row is in I   (NULL: every row)
-    uint8_t *colflag = nullptr;          // [ncols] 1 where the column is in J (NULL: every column)
-    uint32_t *jsorted = nullptr;         // sorted distinct columns of J        (NULL: 0..ncols-1)
+    DevBuf<uint8_t> rowflag;             // [nrows] 1 where the row is in I   (NULL: every row)
+    DevBuf<uint8_t> colflag;             // [ncols] 1 where the column is in J (NULL: every column)
+    DevBuf<uint32_t> jsorted;            // sorted distinct columns of J        (NULL: 0..ncols-1)
     int64_t nj_distinct = 0, ni_distinct = 0;
-    void release() { dfree(rowflag); dfree(colflag); dfree(jsorted); rowflag = colflag = nullptr; jsorted = nullptr; }
 };
 __global__ void flag_kernel(const uint64_t *idx, int64_t k, uint8_t *flag) {
     for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < k; q += (int64_t)gridDim.x * blockDim.x) flag[idx[q]] = 1;
@@ -68,22 +67,20 @@ static GrB_Info region_build(Region &R, const GrB_Index *I, GrB_Index ni, const 
     if (!R.all_rows) {
         std::vector<uint64_t> s(R.I); std::sort(s.begin(), s.end()); s.erase(std::unique(s.begin(), s.end()), s.end());
         R.ni_distinct = (int64_t)s.size();
-        uint64_t *d = nullptr; GB_TRY(upload(s, &d, err));
-        GB_TRY(dalloc(&R.rowflag, (size_t)nrows, err));
+        DevBuf<uint64_t> d; GB_TRY(upload(s, d, err));
+        GB_TRY(R.rowflag.alloc((size_t)nrows, err));
         CU_TRY(cudaMemsetAsync(R.rowflag, 0, (size_t)nrows, G.stream), err);
         if (!s.empty()) { flag_kernel<<<agrid((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.rowflag); GB_LAUNCHED(); }
-        dfree(d);
     }
     if (!R.all_cols) {
         std::vector<uint64_t> s(R.J); std::sort(s.begin(), s.end()); s.erase(std::unique(s.begin(), s.end()), s.end());
         R.nj_distinct = (int64_t)s.size();
         std::vector<uint32_t> s32(s.begin(), s.end());
-        GB_TRY(upload(s32, &R.jsorted, err));
-        uint64_t *d = nullptr; GB_TRY(upload(s, &d, err));
-        GB_TRY(dalloc(&R.colflag, (size_t)ncols, err));
+        GB_TRY(upload(s32, R.jsorted, err));
+        DevBuf<uint64_t> d; GB_TRY(upload(s, d, err));
+        GB_TRY(R.colflag.alloc((size_t)ncols, err));
         CU_TRY(cudaMemsetAsync(R.colflag, 0, (size_t)ncols, G.stream), err);
         if (!s.empty()) { flag_kernel<<<agrid((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.colflag); GB_LAUNCHED(); }
-        dfree(d);
     }
     return GrB_SUCCESS;
 }
@@ -103,12 +100,12 @@ __global__ void fill_entries_kernel(const int64_t *rowptr, int64_t nrows, const 
 }
 static GrB_Info region_filled(const Region &R, int64_t nrows, int64_t ncols, int tc, Sc x, Csr &T, std::string *err) {
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
-    GB_TRY(dalloc(&T.rowptr, (size_t)nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
     fill_count_kernel<<<agrid(nrows + 1), 256, 0, G.stream>>>(R.rowflag, nrows, R.nj_distinct, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     T.nnz = R.ni_distinct * R.nj_distinct;
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * tc_size(tc) + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(tc) + 16, err));
     if (T.nnz > 0) { fill_entries_kernel<<<agrid(nrows * 32), 256, 0, G.stream>>>(T.rowptr, nrows, R.jsorted, T.col, T.val, tc, x); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     CU_TRY(cudaGetLastError(), err);
@@ -140,12 +137,12 @@ __global__ void outside_fill_kernel(const int64_t *ptr, const uint32_t *col, con
 }
 static GrB_Info csr_outside_region(const Csr &c, size_t vsize, const Region &R, Csr &out, std::string *err) {
     out = Csr(); out.nrows = c.nrows; out.ncols = c.ncols;
-    GB_TRY(dalloc(&out.rowptr, (size_t)c.nrows + 1, err));
+    GB_TRY(out.rowptr.alloc((size_t)c.nrows + 1, err));
     outside_count_kernel<<<agrid(c.nrows + 1), 256, 0, G.stream>>>(c.rowptr, c.col, c.nrows, R.rowflag, R.colflag, out.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(out.rowptr, c.nrows + 1, err));
     GB_TRY(read_i64(out.rowptr + c.nrows, &out.nnz, err));
-    GB_TRY(dalloc(&out.col, (size_t)out.nnz, err));
-    GB_TRY(dmalloc(&out.val, (size_t)out.nnz * vsize + 16, err));
+    GB_TRY(out.col.alloc((size_t)out.nnz, err));
+    GB_TRY(out.val.alloc((size_t)out.nnz * vsize + 16, err));
     if (out.nnz > 0) {
         outside_fill_kernel<<<agrid(c.nrows), 256, 0, G.stream>>>(c.rowptr, c.col, (const uint8_t *)c.val, (int)vsize, c.nrows, R.rowflag, R.colflag,
                                                                   out.rowptr, out.col, (uint8_t *)out.val); GB_LAUNCHED();
@@ -159,15 +156,15 @@ static GrB_Info csr_outside_region(const Csr &c, size_t vsize, const Region &R, 
 // T is a CSR of C's dimensions holding the new content of the region (type ttc); consumed.
 // t_covers_region: T has an entry at every position of the region (scalar fill), so nothing needs deleting first.
 static GrB_Info assign_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f, const Region &R,
-                                 Csr &T, int ttc, bool t_covers_region, std::string *err) {
+                                 Csr &&T, int ttc, bool t_covers_region, std::string *err) {
     const int ctc = C->type->code;
-    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, T, ttc, false, err);     // nothing is let through
+    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, std::move(T), ttc, false, err);     // nothing is let through
     DescFlags plain{}; plain.replace = false; plain.mask_comp = false; plain.mask_struct = false; plain.tran0 = plain.tran1 = false; plain.axb = f.axb;
     const GrB_BinaryOp merge = accum ? accum : second_op(ctc);
     const bool whole = R.all_rows && R.all_cols;
     // Z = C with the region replaced by / merged with T, built in a scratch matrix unless it can go straight into C
     GrB_Matrix Zm = C;
-    if (Mask) { GrB_Info r = GrB_Matrix_dup(&Zm, C); if (r != GrB_SUCCESS) { csr_free(T); return r; } }
+    if (Mask) GB_TRY(GrB_Matrix_dup(&Zm, C));
     GrB_Info r = GrB_SUCCESS;
     if (!accum && !t_covers_region && !whole) {
         // entries of C inside the region that T lacks are deleted: drop the region from C first
@@ -175,19 +172,19 @@ static GrB_Info assign_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_
         if (r == GrB_SUCCESS && Zm->dev.nnz > 0) {
             Csr keep;
             r = csr_outside_region(Zm->dev, Zm->type->size, R, keep, err);
-            if (r == GrB_SUCCESS) matrix_adopt_device(Zm, keep); else csr_free(keep);
+            if (r == GrB_SUCCESS) matrix_adopt_device(Zm, std::move(keep));
         }
     }
     if (r == GrB_SUCCESS) {
-        if (!accum && whole) r = matrix_writeback(Zm, nullptr, nullptr, plain, T, ttc, false, err);        // Z = T
-        else r = matrix_writeback(Zm, nullptr, merge, plain, T, ttc, false, err);                          // Z = C (+) T
-    } else csr_free(T);
+        if (!accum && whole) r = matrix_writeback(Zm, nullptr, nullptr, plain, std::move(T), ttc, false, err);        // Z = T
+        else r = matrix_writeback(Zm, nullptr, merge, plain, std::move(T), ttc, false, err);                          // Z = C (+) T
+    }
     if (!Mask || r != GrB_SUCCESS) { if (Zm != C) GrB_Matrix_free(&Zm); return r; }
     // C<Mask> = Z  (mask and GrB_REPLACE span all of C)
     r = matrix_ensure_device(Zm);
     if (r == GrB_SUCCESS) {
-        Csr z = Zm->dev; Zm->dev = Csr(); Zm->host_valid = true;      // steal Z's CSR (values already of C's type)
-        r = matrix_writeback(C, Mask, nullptr, f, z, ctc, false, err);
+        Csr z = std::move(Zm->dev); Zm->host_valid = true;      // steal Z's CSR (values already of C's type)
+        r = matrix_writeback(C, Mask, nullptr, f, std::move(z), ctc, false, err);
     }
     GrB_Matrix_free(&Zm);
     return r;
@@ -206,15 +203,12 @@ static GrB_Info matrix_assign_scalar(GrB_Matrix C, const GrB_Matrix Mask, const 
     GbBurble burble(fn);
     const DescFlags f = desc_flags(desc);
     Region R;
-    GrB_Info r = region_build(R, I, ni, J, nj, C->nrows, C->ncols, err, fn);
-    if (r != GrB_SUCCESS) { R.release(); return r; }
-    if ((double)R.ni_distinct * (double)R.nj_distinct >= 4.0e9) { R.release(); return gb_fail(GrB_OUT_OF_MEMORY, err, "%s: the filled region would hold >= 4e9 entries", fn); }
+    GB_TRY(region_build(R, I, ni, J, nj, C->nrows, C->ncols, err, fn));
+    if ((double)R.ni_distinct * (double)R.nj_distinct >= 4.0e9) return gb_fail(GrB_OUT_OF_MEMORY, err, "%s: the filled region would hold >= 4e9 entries", fn);
     Csr T;
-    r = region_filled(R, (int64_t)C->nrows, (int64_t)C->ncols, xtc, x, T, err);
-    if (r == GrB_SUCCESS) { burble.note("region fill + write-back", (double)T.nnz * (4 + tc_size(xtc))); r = assign_writeback(C, Mask, accum, f, R, T, xtc, /*t_covers_region=*/true, err); }
-    else csr_free(T);
-    R.release();
-    return r;
+    GB_TRY(region_filled(R, (int64_t)C->nrows, (int64_t)C->ncols, xtc, x, T, err));
+    burble.note("region fill + write-back", (double)T.nnz * (4 + tc_size(xtc)));
+    return assign_writeback(C, Mask, accum, f, R, std::move(T), xtc, /*t_covers_region=*/true, err);
 }
 
 #define GB_MASSIGN(TN, CT, TC, FIELD) \
@@ -299,36 +293,33 @@ extern "C" GrB_Info GrB_Matrix_extract(GrB_Matrix C, const GrB_Matrix Mask, cons
     if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
     const Csr &a = f.tran0 ? A->devT : A->dev;
     const size_t vsize = A->type->size;
-    uint32_t *d_rows = nullptr, *d_jsv = nullptr, *d_jsq = nullptr;
+    DevBuf<uint32_t> d_rows, d_jsv, d_jsq;
     bool need_sort = false;
-    if (!all_i) { std::vector<uint32_t> r32(Iv.begin(), Iv.end()); GB_TRY(upload(r32, &d_rows, err)); }
+    if (!all_i) { std::vector<uint32_t> r32(Iv.begin(), Iv.end()); GB_TRY(upload(r32, d_rows, err)); }
     if (!all_j) {
         std::vector<uint32_t> ord(Jv.size());
         for (size_t q = 0; q < ord.size(); ++q) ord[q] = (uint32_t)q;
         std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return Jv[x] < Jv[y]; });
         std::vector<uint32_t> jsv(ord.size());
         for (size_t q = 0; q < ord.size(); ++q) { jsv[q] = (uint32_t)Jv[ord[q]]; if (ord[q] != q) need_sort = true; }
-        GB_TRY(upload(jsv, &d_jsv, err)); GB_TRY(upload(ord, &d_jsq, err));
+        GB_TRY(upload(jsv, d_jsv, err)); GB_TRY(upload(ord, d_jsq, err));
     }
     Csr T; T.nrows = (int64_t)tn; T.ncols = (int64_t)tm;
-    GrB_Info r = dalloc(&T.rowptr, (size_t)tn + 1, err);
-    if (r == GrB_SUCCESS) {
-        extract_count_kernel<<<agrid((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), T.rowptr); GB_LAUNCHED();
-        r = dev_exclusive_scan(T.rowptr, (int64_t)tn + 1, err);
-    }
-    if (r == GrB_SUCCESS) r = read_i64(T.rowptr + tn, &T.nnz, err);
-    if (r == GrB_SUCCESS) r = dalloc(&T.col, (size_t)T.nnz, err);
-    if (r == GrB_SUCCESS) r = dmalloc(&T.val, (size_t)T.nnz * vsize + 16, err);
-    if (r == GrB_SUCCESS && T.nnz > 0) {
+    GB_TRY(T.rowptr.alloc((size_t)tn + 1, err));
+    extract_count_kernel<<<agrid((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), T.rowptr); GB_LAUNCHED();
+    GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)tn + 1, err));
+    GB_TRY(read_i64(T.rowptr + tn, &T.nnz, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
+    if (T.nnz > 0) {
         extract_fill_kernel<<<agrid((int64_t)tn), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jsv, d_jsq,
                                                                     (int64_t)Jv.size(), T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
         if (need_sort) { rows_insertion_sort_kernel<<<agrid((int64_t)tn), 256, 0, G.stream>>>(T.rowptr, (int64_t)tn, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
     }
-    if (r == GrB_SUCCESS) r = dev_build_rowptr32(T, err);
-    dfree(d_rows); dfree(d_jsv); dfree(d_jsq);
-    if (r != GrB_SUCCESS) { csr_free(T); return r; }
+    GB_TRY(dev_build_rowptr32(T, err));
+    d_rows.reset(); d_jsv.reset(); d_jsq.reset();
     burble.note("row gather + column map", (double)T.nnz * (4 + vsize) * 2);
-    return matrix_writeback(C, Mask, accum, f, T, A->type->code, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }
 
 // ================================================================== GxB_Matrix_diag / GxB_Vector_diag
@@ -361,16 +352,16 @@ extern "C" GrB_Info GxB_Matrix_diag(GrB_Matrix C, const GrB_Vector v, int64_t k,
     GB_TRY(vector_ensure_device(v));
     const size_t vsize = v->type->size;
     Csr T; T.nrows = T.ncols = (int64_t)dim;
-    GB_TRY(dalloc(&T.rowptr, (size_t)dim + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)dim + 1, err));
     diag_build_kernel<<<agrid((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)dim + 1, err));
     GB_TRY(read_i64(T.rowptr + dim, &T.nnz, err));
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * vsize + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (T.nnz > 0) { diag_fill_kernel<<<agrid((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     DescFlags plain{};
-    return matrix_writeback(C, nullptr, nullptr, plain, T, v->type->code, false, err);
+    return matrix_writeback(C, nullptr, nullptr, plain, std::move(T), v->type->code, false, err);
 }
 __global__ void diag_extract_kernel(const int64_t *a_ptr, const uint32_t *a_col, const uint8_t *a_val, int vsize, int64_t nrows, int64_t ncols, int64_t k, int64_t n,
                                     uint8_t *oval, uint8_t *opres) {
@@ -398,13 +389,13 @@ extern "C" GrB_Info GxB_Vector_diag(GrB_Vector v, const GrB_Matrix A, int64_t k,
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
     GB_TRY(matrix_ensure_device(A));
     const size_t vsize = A->type->size;
-    void *oval = nullptr; uint8_t *opres = nullptr;
-    GB_TRY(dmalloc(&oval, (size_t)len * vsize + 16, err));
-    GB_TRY(dmalloc((void **)&opres, (size_t)len + 16, err));
+    DevBuf<void> oval; DevBuf<uint8_t> opres;
+    GB_TRY(oval.alloc((size_t)len * vsize + 16, err));
+    GB_TRY(opres.alloc((size_t)len, err));
     CU_TRY(cudaMemsetAsync(oval, 0, (size_t)len * vsize, G.stream), err);
     if (len > 0) { diag_extract_kernel<<<agrid(len), 256, 0, G.stream>>>(A->dev.rowptr, A->dev.col, (const uint8_t *)A->dev.val, (int)vsize, nr, nc, k, len, (uint8_t *)oval, opres); GB_LAUNCHED(); }
     DescFlags plain{};
-    return vector_write(v, nullptr, nullptr, plain, oval, opres, A->type->code, false, nullptr, true);
+    return vector_write(v, nullptr, nullptr, plain, oval, opres, A->type->code, false, nullptr, std::move(oval), std::move(opres));
 }
 
 // ================================================================== GrB_Matrix_kronecker_BinaryOp:  C<Mask> = accum(C, kron(op(A), op(B)))
@@ -453,19 +444,19 @@ extern "C" GrB_Info GrB_Matrix_kronecker_BinaryOp(GrB_Matrix C, const GrB_Matrix
     const Csr &a = f.tran0 ? A->devT : A->dev; const Csr &b = f.tran1 ? B->devT : B->dev;
     const int ztc = op->ztype->code;
     Csr T; T.nrows = (int64_t)(am * bm); T.ncols = (int64_t)(an * bn);
-    GB_TRY(dalloc(&T.rowptr, (size_t)T.nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
     kron_count_kernel<<<agrid(T.nrows + 1), 256, 0, G.stream>>>(a.rowptr, b.rowptr, (int64_t)am, (int64_t)bm, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * tc_size(ztc) + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(ztc) + 16, err));
     if (T.nnz > 0) {
         kron_fill_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, a.val, A->type->code, b.rowptr, b.col, b.val, B->type->code, (int64_t)am, (int64_t)bm,
                                                               (int64_t)bn, op->opcode, op->xtype->code, op->ytype->code, ztc, T.rowptr, T.col, T.val); GB_LAUNCHED();
     }
     GB_TRY(dev_build_rowptr32(T, err));
     burble.note("row-pair expansion", (double)T.nnz * (4 + tc_size(ztc)));
-    return matrix_writeback(C, Mask, accum, f, T, ztc, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), ztc, false, err);
 }
 
 // ================================================================== rows / columns of a matrix as vectors, and back
@@ -492,10 +483,9 @@ __global__ void col_to_dense_kernel(const int64_t *ptr, const uint32_t *col, con
 static GrB_Info slice_vector(const Csr &a, GrB_Type type, int along, uint64_t index, GrB_Vector *out, std::string *err) {
     const int64_t n = along == 0 ? a.ncols : a.nrows;
     const size_t vsize = type->size;
-    GB_TRY(GrB_Vector_new(out, type, (GrB_Index)n));
-    void *val = nullptr; uint8_t *pres = nullptr;
-    GB_TRY(dmalloc(&val, (size_t)n * vsize + 16, err));
-    GB_TRY(dmalloc((void **)&pres, (size_t)n + 16, err));
+    DevBuf<void> val; DevBuf<uint8_t> pres;
+    GB_TRY(val.alloc((size_t)n * vsize + 16, err));
+    GB_TRY(pres.alloc((size_t)n, err));
     CU_TRY(cudaMemsetAsync(val, 0, (size_t)n * vsize, G.stream), err);
     CU_TRY(cudaMemsetAsync(pres, 0, (size_t)n, G.stream), err);
     if (a.nnz > 0) {
@@ -503,7 +493,8 @@ static GrB_Info slice_vector(const Csr &a, GrB_Type type, int along, uint64_t in
         else col_to_dense_kernel<<<agrid(a.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, a.nrows, (uint32_t)index, (uint8_t *)val, pres);
         GB_LAUNCHED();
     }
-    vector_adopt_device(*out, val, pres);
+    GB_TRY(GrB_Vector_new(out, type, (GrB_Index)n));
+    vector_adopt_device(*out, val.release(), pres.release());
     return GrB_SUCCESS;
 }
 __global__ void vec_flags_kernel(const uint8_t *pres, int64_t n, int64_t *flag) {
@@ -531,20 +522,20 @@ static GrB_Info vector_as_slice_csr(GrB_Vector v, int along, uint64_t index, int
     GB_TRY(vector_ensure_device(v));
     const int64_t n = (int64_t)v->n; const size_t vsize = v->type->size;
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
-    int64_t *pos = nullptr;
-    GB_TRY(dalloc(&pos, (size_t)n + 1, err));
+    DevBuf<int64_t> pos;
+    GB_TRY(pos.alloc((size_t)n + 1, err));
     vec_flags_kernel<<<agrid(n + 1), 256, 0, G.stream>>>(v->dpres, n, pos); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(pos, n + 1, err));
     GB_TRY(read_i64(pos + n, &T.nnz, err));
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * vsize + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (along == 0) {
-        GB_TRY(dalloc(&T.rowptr, (size_t)nrows + 1, err));
+        GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
         row_only_ptr_kernel<<<agrid(nrows + 1), 256, 0, G.stream>>>(nrows, (int64_t)index, T.nnz, T.rowptr); GB_LAUNCHED();
         if (T.nnz > 0) { vec_to_row_kernel<<<agrid(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, pos, 0, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
-        dfree(pos);
+        pos.reset();
     } else {
-        T.rowptr = pos;                  // one entry per present position: the scan IS the row pointer
+        T.rowptr = std::move(pos);       // one entry per present position: the scan IS the row pointer
         if (T.nnz > 0) { vec_to_col_kernel<<<agrid(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, T.rowptr, (uint32_t)index, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
     }
     GB_TRY(dev_build_rowptr32(T, err));
@@ -572,24 +563,20 @@ static GrB_Info slice_assign(GrB_Matrix C, const GrB_Vector mask, const GrB_Bina
     Csr T;
     r = vector_as_slice_csr(sv, along, index, (int64_t)C->nrows, (int64_t)C->ncols, T, err);
     GrB_Vector_free(&sv);
-    if (r != GrB_SUCCESS) { csr_free(T); return r; }
+    if (r != GrB_SUCCESS) return r;
     Region R;
     std::vector<uint64_t> one(1, index);
     if (along == 0) { R.all_rows = false; R.I = one; R.ni_distinct = 1; R.nj_distinct = (int64_t)C->ncols; }
     else { R.all_cols = false; R.J = one; R.nj_distinct = 1; R.ni_distinct = (int64_t)C->nrows; }
-    uint64_t *d = nullptr;
-    r = upload(one, &d, err);
-    uint8_t **flag = along == 0 ? &R.rowflag : &R.colflag;
+    DevBuf<uint64_t> d;
+    GB_TRY(upload(one, d, err));
+    DevBuf<uint8_t> &flag = along == 0 ? R.rowflag : R.colflag;
     const size_t fn_ = (size_t)(along == 0 ? C->nrows : C->ncols);
-    if (r == GrB_SUCCESS) r = dalloc(flag, fn_, err);
-    if (r == GrB_SUCCESS) {
-        cudaMemsetAsync(*flag, 0, fn_, G.stream);
-        flag_kernel<<<1, 32, 0, G.stream>>>(d, 1, *flag); GB_LAUNCHED();
-        DescFlags plain{};
-        r = assign_writeback(C, nullptr, nullptr, plain, R, T, C->type->code, /*t_covers_region=*/false, err);     // the slice vector has C's type
-    } else csr_free(T);
-    dfree(d); R.release();
-    return r;
+    GB_TRY(flag.alloc(fn_, err));
+    cudaMemsetAsync(flag, 0, fn_, G.stream);
+    flag_kernel<<<1, 32, 0, G.stream>>>(d, 1, flag); GB_LAUNCHED();
+    DescFlags plain{};
+    return assign_writeback(C, nullptr, nullptr, plain, R, std::move(T), C->type->code, /*t_covers_region=*/false, err);     // the slice vector has C's type
 }
 
 extern "C" GrB_Info GrB_Row_assign(GrB_Matrix C, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Vector u, GrB_Index i, const GrB_Index *J, GrB_Index nj,
@@ -651,48 +638,40 @@ extern "C" GrB_Info GrB_Matrix_assign(GrB_Matrix C, const GrB_Matrix Mask, const
     if (Mask && (Mask->nrows != C->nrows || Mask->ncols != C->ncols)) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: the mask must have C's dimensions", fn);
     const DescFlags f = desc_flags(desc);
     Region R;
-    GrB_Info r = GrB_SUCCESS;
-    if (G.have_device && C->nrows < ((uint64_t)1 << 31) && C->ncols < ((uint64_t)1 << 31)) r = region_build(R, I, ni, J, nj, C->nrows, C->ncols, err, fn);
-    else { R.release(); return G.have_device ? gb_fail(GrB_INVALID_VALUE, err, "%s: dimensions beyond 2^31 are not supported in HBM", fn)
-                                              : gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn); }
-    if (r != GrB_SUCCESS) { R.release(); return r; }
+    if (G.have_device && C->nrows < ((uint64_t)1 << 31) && C->ncols < ((uint64_t)1 << 31)) GB_TRY(region_build(R, I, ni, J, nj, C->nrows, C->ncols, err, fn));
+    else return G.have_device ? gb_fail(GrB_INVALID_VALUE, err, "%s: dimensions beyond 2^31 are not supported in HBM", fn)
+                              : gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
     const uint64_t an = f.tran0 ? A->ncols : A->nrows, am = f.tran0 ? A->nrows : A->ncols;
     const uint64_t tn = R.all_rows ? C->nrows : R.I.size(), tm = R.all_cols ? C->ncols : R.J.size();
-    if (an != tn || am != tm) { R.release(); return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: A is %llux%llu, the index lists select %llux%llu", fn,
-                                                            (unsigned long long)an, (unsigned long long)am, (unsigned long long)tn, (unsigned long long)tm); }
+    if (an != tn || am != tm) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: A is %llux%llu, the index lists select %llux%llu", fn,
+                                             (unsigned long long)an, (unsigned long long)am, (unsigned long long)tn, (unsigned long long)tm);
     GbBurble burble(fn);
-    r = f.tran0 ? matrix_ensure_transpose(A) : matrix_ensure_device(A);
-    if (r != GrB_SUCCESS) { R.release(); return r; }
+    GB_TRY(f.tran0 ? matrix_ensure_transpose(A) : matrix_ensure_device(A));
     const Csr &a = f.tran0 ? A->devT : A->dev;
     const size_t vsize = A->type->size;
-    int32_t *d_rowsrc = nullptr; uint32_t *d_jmap = nullptr; bool need_sort = false;
+    DevBuf<int32_t> d_rowsrc; DevBuf<uint32_t> d_jmap; bool need_sort = false;
     if (!R.all_rows) {
         std::vector<int32_t> rowsrc((size_t)C->nrows, -1);
         for (size_t p = 0; p < R.I.size(); ++p) rowsrc[R.I[p]] = (int32_t)p;       // a row named twice takes the later source row
-        r = upload(rowsrc, &d_rowsrc, err);
+        GB_TRY(upload(rowsrc, d_rowsrc, err));
     }
-    if (r == GrB_SUCCESS && !R.all_cols) {
+    if (!R.all_cols) {
         std::vector<uint32_t> jmap(R.J.begin(), R.J.end());
         for (size_t q = 1; q < jmap.size(); ++q) if (jmap[q] <= jmap[q - 1]) need_sort = true;
-        r = upload(jmap, &d_jmap, err);
+        GB_TRY(upload(jmap, d_jmap, err));
     }
     Csr T; T.nrows = (int64_t)C->nrows; T.ncols = (int64_t)C->ncols;
-    if (r == GrB_SUCCESS) r = dalloc(&T.rowptr, (size_t)T.nrows + 1, err);
-    if (r == GrB_SUCCESS) {
-        massign_count_kernel<<<agrid(T.nrows + 1), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, T.rowptr); GB_LAUNCHED();
-        r = dev_exclusive_scan(T.rowptr, T.nrows + 1, err);
-    }
-    if (r == GrB_SUCCESS) r = read_i64(T.rowptr + T.nrows, &T.nnz, err);
-    if (r == GrB_SUCCESS) r = dalloc(&T.col, (size_t)T.nnz, err);
-    if (r == GrB_SUCCESS) r = dmalloc(&T.val, (size_t)T.nnz * vsize + 16, err);
-    if (r == GrB_SUCCESS && T.nnz > 0) {
+    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
+    massign_count_kernel<<<agrid(T.nrows + 1), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, T.rowptr); GB_LAUNCHED();
+    GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
+    GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
+    if (T.nnz > 0) {
         massign_fill_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jmap, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
         if (need_sort) { rows_insertion_sort_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(T.rowptr, T.nrows, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
     }
-    if (r == GrB_SUCCESS) r = dev_build_rowptr32(T, err);
-    dfree(d_rowsrc); dfree(d_jmap);
-    if (r == GrB_SUCCESS) r = assign_writeback(C, Mask, accum, f, R, T, A->type->code, /*t_covers_region=*/false, err);
-    else csr_free(T);
-    R.release();
-    return r;
+    GB_TRY(dev_build_rowptr32(T, err));
+    d_rowsrc.reset(); d_jmap.reset();
+    return assign_writeback(C, Mask, accum, f, R, std::move(T), A->type->code, /*t_covers_region=*/false, err);
 }

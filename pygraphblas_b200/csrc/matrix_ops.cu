@@ -39,9 +39,9 @@ static GrB_Info source_csr(GrB_Matrix A, bool tran, const Csr **out) {
 }
 static GrB_Info new_pattern_like(const Csr &src, size_t vsize, Csr &T, std::string *err) {
     T = Csr(); T.nrows = src.nrows; T.ncols = src.ncols; T.nnz = src.nnz;
-    GB_TRY(dalloc(&T.rowptr, (size_t)src.nrows + 1, err));
-    GB_TRY(dalloc(&T.col, (size_t)src.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)src.nnz * vsize + 16, err));
+    GB_TRY(T.rowptr.alloc((size_t)src.nrows + 1, err));
+    GB_TRY(T.col.alloc((size_t)src.nnz, err));
+    GB_TRY(T.val.alloc((size_t)src.nnz * vsize + 16, err));
     CU_TRY(cudaMemcpyAsync(T.rowptr, src.rowptr, ((size_t)src.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
     if (src.nnz) CU_TRY(cudaMemcpyAsync(T.col, src.col, (size_t)src.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
     return GrB_SUCCESS;
@@ -128,18 +128,18 @@ extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const
     const Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
     a.rowptr = src->rowptr; a.col = src->col; a.val = src->val; a.tc = A->type->code; a.nrows = src->nrows;
     Csr T; T.nrows = src->nrows; T.ncols = src->ncols;
-    GB_TRY(dalloc(&T.rowptr, (size_t)T.nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
     a.o_ptr = T.rowptr;
     select_kernel<false><<<wgrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * A->type->size + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * A->type->size + 16, err));
     a.o_col = T.col; a.o_val = T.val;
     if (T.nnz > 0) { select_kernel<true><<<wgrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
-    return matrix_writeback(C, Mask, accum, f, T, A->type->code, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }
 __global__ void vec_select_kernel(const SelectArgs a, const uint8_t *upres, uint8_t *tpres) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.nrows; i += (int64_t)gridDim.x * blockDim.x) {
@@ -162,12 +162,12 @@ extern "C" GrB_Info GxB_Vector_select(GrB_Vector w, const GrB_Vector mask, const
     a.val = u->dval; a.tc = u->type->code; a.nrows = (int64_t)u->n;
     // T keeps u's values and narrows its presence: a vector is a column, i = position, j = 0
     const size_t bytes = (size_t)u->n * u->type->size;
-    void *tval = nullptr; uint8_t *tpres = nullptr;
-    GB_TRY(dmalloc(&tval, bytes + 16, &w->err));
-    GB_TRY(dmalloc((void **)&tpres, (size_t)u->n + 16, &w->err));
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    GB_TRY(tval.alloc(bytes + 16, &w->err));
+    GB_TRY(tpres.alloc((size_t)u->n, &w->err));
     CU_TRY(cudaMemcpyAsync(tval, u->dval, bytes, cudaMemcpyDeviceToDevice, G.stream), &w->err);
     vec_select_kernel<<<egrid(a.nrows), 256, 0, G.stream>>>(a, u->dpres, tpres); GB_LAUNCHED();
-    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, true);
+    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, std::move(tval), std::move(tpres));
 }
 
 // ------------------------------------------------------------------ apply:  T has A's pattern, z = f(a) / op(x, a) / op(a, y)
@@ -196,7 +196,7 @@ static GrB_Info mat_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     a.nnz = src->nnz; a.aval = src->val; a.atc = A->type->code; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar; a.tval = T.val;
     if (a.nnz > 0) { mat_apply_kernel<<<egrid(a.nnz), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
-    return matrix_writeback(C, Mask, accum, f, T, ztc, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), ztc, false, err);
 }
 extern "C" GrB_Info GrB_Matrix_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_UnaryOp op, const GrB_Matrix A, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
@@ -282,10 +282,12 @@ static GrB_Info mat_reduce_vector(GrB_Vector w, const GrB_Vector mask, const GrB
     const Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
     RowReduceArgs a{};
     a.rowptr = src->rowptr; a.val = src->val; a.atc = A->type->code; a.nrows = src->nrows; a.op = op->opcode; a.mtc = op->ztype->code;
-    GB_TRY(dmalloc(&a.tval, (size_t)rows * tc_size(a.mtc) + 16, &w->err));
-    GB_TRY(dmalloc((void **)&a.tpres, (size_t)rows + 16, &w->err));
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    GB_TRY(tval.alloc((size_t)rows * tc_size(a.mtc) + 16, &w->err));
+    GB_TRY(tpres.alloc((size_t)rows, &w->err));
+    a.tval = tval; a.tpres = tpres;
     row_reduce_kernel<<<wgrid(a.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    return vector_write(w, mask, accum, f, a.tval, a.tpres, a.mtc, false, nullptr, true);
+    return vector_write(w, mask, accum, f, a.tval, a.tpres, a.mtc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Matrix_reduce_Monoid(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Monoid monoid, const GrB_Matrix A, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
@@ -351,18 +353,18 @@ static GrB_Info mat_ewise(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     a.b_ptr = sb->rowptr; a.b_col = sb->col; a.b_val = sb->val; a.btc = B->type->code;
     a.nrows = sa->nrows; a.mult = mult; a.op = op->opcode; a.xtc = op->xtype->code; a.ztc = op->ztype->code;
     Csr T; T.nrows = sa->nrows; T.ncols = sa->ncols;
-    GB_TRY(dalloc(&T.rowptr, (size_t)T.nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
     a.o_ptr = T.rowptr;
     merge_rows_kernel<false><<<egrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(dalloc(&T.col, (size_t)T.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)T.nnz * tc_size(a.ztc) + 16, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(a.ztc) + 16, err));
     a.o_col = T.col; a.o_val = T.val;
     if (T.nnz > 0) { merge_rows_kernel<true><<<egrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
-    return matrix_writeback(C, Mask, accum, f, T, a.ztc, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), a.ztc, false, err);
 }
 #define GB_MAT_EWISE(NAME, KIND, OPEXPR, MULT) \
     extern "C" GrB_Info NAME(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const KIND op, const GrB_Matrix A, const GrB_Matrix B, const GrB_Descriptor desc) { \

@@ -165,15 +165,22 @@ extern "C" GrB_Info B200_device_synchronize(void) {
     return GrB_SUCCESS;
 }
 
+// allocation test seam: the k-th dmalloc from now fails (0: off); blocks handed out and not yet freed
+static int64_t g_fail_alloc = 0, g_live_allocs = 0;
+extern "C" void B200_debug_fail_alloc(int64_t k) { g_fail_alloc = k > 0 ? k : 0; }
+extern "C" int64_t B200_debug_live_allocs(void) { return g_live_allocs; }
+
 GrB_Info dmalloc(void **p, size_t bytes, std::string *err) {
     *p = nullptr;
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
+    if (g_fail_alloc > 0 && --g_fail_alloc == 0) return gb_fail(GrB_OUT_OF_MEMORY, err, "device allocation failed (injected by B200_debug_fail_alloc)");
     if (bytes == 0) bytes = 16;
     bytes = (bytes + 255) & ~(size_t)255;
     CU_TRY(cudaMallocAsync(p, bytes, G.stream), err);
+    ++g_live_allocs;
     return GrB_SUCCESS;
 }
-void dfree(void *p) { if (p && G.have_device) cudaFreeAsync(p, G.stream); }
+void dfree(void *p) { if (p && G.have_device) { cudaFreeAsync(p, G.stream); --g_live_allocs; } }
 
 static void *g_ws[WS_COUNT]; static size_t g_ws_cap[WS_COUNT];
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh) {
@@ -187,22 +194,6 @@ GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh)
     }
     *p = g_ws[slot];
     return GrB_SUCCESS;
-}
-
-// the cached SpMV plans and scratch of a CSR (dropped whenever its structure changes)
-void csr_drop_plans(Csr &c) {
-    dfree(c.tile_row); c.tile_row = nullptr; c.ntiles = 0; c.tile_size = 0;
-    dfree(c.hperm); dfree(c.hcol); c.hperm = nullptr; c.hcol = nullptr; c.henc = 0; c.hot_planned = false; c.hot_cover = 0.0;
-    dfree(c.run_headw); dfree(c.run_lane); dfree(c.run_base); dfree(c.run_tail_row); dfree(c.run_tail_last); dfree(c.nzrow); dfree(c.pres_tmpl);
-    c.run_headw = nullptr; c.run_lane = nullptr; c.run_base = nullptr; c.run_tail_row = nullptr; c.run_tail_last = nullptr; c.nzrow = nullptr; c.pres_tmpl = nullptr;
-    c.nruns = 0; c.nnzrows = 0;
-    dfree(c.ws_head); dfree(c.ws_tail); dfree(c.ws_head_has); dfree(c.ws_tail_has); dfree(c.ws_uhot);
-    c.ws_head = c.ws_tail = c.ws_uhot = nullptr; c.ws_head_has = c.ws_tail_has = nullptr;
-}
-void csr_free(Csr &c) {
-    csr_drop_plans(c);
-    dfree(c.rowptr); dfree(c.rowptr32); dfree(c.col); dfree(c.val);
-    c = Csr();
 }
 
 // ------------------------------------------------------------------ operators
@@ -437,7 +428,7 @@ bool gb_valid_matrix(const GrB_Matrix A) { return A && A->magic == GB_MAGIC; }
 bool gb_valid_vector(const GrB_Vector v) { return v && v->magic == GB_MAGIC; }
 static const uint64_t DEV_DIM_MAX = ((uint64_t)1 << 31) - 1;   // 32-bit column / row ids in HBM
 
-void matrix_invalidate_device(GrB_Matrix A) { csr_free(A->dev); csr_free(A->devT); }
+void matrix_invalidate_device(GrB_Matrix A) { A->dev = Csr(); A->devT = Csr(); }
 // copies still running on the copy streams must finish before the compute stream frees (or overwrites) the buffers
 static void vector_join_copies(GrB_Vector v) {
     if (v->h2d_pending) { cudaStreamWaitEvent(G.stream, v->ev_h2d, 0); v->h2d_pending = false; }
@@ -451,9 +442,9 @@ void vector_invalidate_device(GrB_Vector v) {
     if (!v->borrowed) { dfree(v->dval); dfree(v->dpres); }       // a borrowed view (B200_Comm_result) does not own its buffers
     v->borrowed = false; v->dval = nullptr; v->dpres = nullptr; v->dev_valid = false; v->dev_nvals = -1;
 }
-void matrix_adopt_device(GrB_Matrix A, Csr &c) {
+void matrix_adopt_device(GrB_Matrix A, Csr &&c) {
     matrix_invalidate_device(A);
-    A->dev = c; A->dev.valid = true; c = Csr();
+    A->dev = std::move(c); A->dev.valid = true;
     A->hi.clear(); A->hj.clear(); A->hx.clear(); A->hi.shrink_to_fit(); A->hj.shrink_to_fit(); A->hx.shrink_to_fit();
     A->pi.clear(); A->pj.clear(); A->px.clear();
     A->host_valid = false;
@@ -557,9 +548,9 @@ GrB_Info matrix_ensure_device(GrB_Matrix A) {
     for (int64_t r = 0; r < c.nrows; ++r) rp[r + 1] += rp[r];
     std::vector<uint32_t> cj((size_t)nnz);
     for (int64_t k = 0; k < nnz; ++k) cj[k] = (uint32_t)A->hj[k];
-    GB_TRY(dalloc(&c.rowptr, rp.size(), &A->err));
-    GB_TRY(dalloc(&c.col, (size_t)nnz, &A->err));
-    GB_TRY(dmalloc(&c.val, (size_t)nnz * sz + 16, &A->err));
+    GB_TRY(c.rowptr.alloc(rp.size(), &A->err));
+    GB_TRY(c.col.alloc((size_t)nnz, &A->err));
+    GB_TRY(c.val.alloc((size_t)nnz * sz + 16, &A->err));
     CU_TRY(cudaMemcpyAsync(c.rowptr, rp.data(), rp.size() * 8, cudaMemcpyHostToDevice, G.stream), &A->err);
     if (nnz) {
         CU_TRY(cudaMemcpyAsync(c.col, cj.data(), cj.size() * 4, cudaMemcpyHostToDevice, G.stream), &A->err);
@@ -568,7 +559,7 @@ GrB_Info matrix_ensure_device(GrB_Matrix A) {
     CU_TRY(cudaStreamSynchronize(G.stream), &A->err);   // host staging vectors go out of scope
     GB_TRY(dev_build_rowptr32(c, &A->err));
     c.valid = true;
-    A->dev = c;
+    A->dev = std::move(c);
     return GrB_SUCCESS;
 }
 
@@ -577,7 +568,7 @@ GrB_Info matrix_ensure_transpose(GrB_Matrix A) {
     if (A->devT.valid) return GrB_SUCCESS;
     Csr t;
     GB_TRY(dev_transpose(A->dev, A->type->size, t, &A->err));
-    t.valid = true; A->devT = t;
+    t.valid = true; A->devT = std::move(t);
     return GrB_SUCCESS;
 }
 
@@ -610,33 +601,34 @@ GrB_Info vector_ensure_device(GrB_Vector v) {
     if (v->dev_valid) return GrB_SUCCESS;
     if (v->n > DEV_DIM_MAX) return gb_fail(GrB_INVALID_VALUE, &v->err, "vector size %llu exceeds the 2^31-1 limit of the HBM layout", (unsigned long long)v->n);
     const size_t sz = v->type->size, n = (size_t)v->n, k = v->hi.size();
-    GB_TRY(dmalloc(&v->dval, n * sz + 16, &v->err));
+    DevBuf<void> dval; DevBuf<uint8_t> dpres;        // committed to v only once filled
+    GB_TRY(dval.alloc(n * sz + 16, &v->err));
     const bool full = k == n && n > 0;
-    if (!full) GB_TRY(dmalloc((void **)&v->dpres, n + 16, &v->err));
+    if (!full) GB_TRY(dpres.alloc(n, &v->err));
     if (n && k < n / 8) {
         // few entries (a BFS source, a seed set): ship the tuples and scatter them in HBM rather than two dense arrays
-        CU_TRY(cudaMemsetAsync(v->dval, 0, n * sz, G.stream), &v->err);
-        CU_TRY(cudaMemsetAsync(v->dpres, 0, n, G.stream), &v->err);
+        CU_TRY(cudaMemsetAsync(dval, 0, n * sz, G.stream), &v->err);
+        CU_TRY(cudaMemsetAsync(dpres, 0, n, G.stream), &v->err);
         if (k) {
-            uint64_t *di = nullptr; void *dx = nullptr;
-            GB_TRY(dmalloc((void **)&di, k * sizeof(uint64_t), &v->err));
-            GB_TRY(dmalloc(&dx, k * sz, &v->err));
+            DevBuf<void> di, dx;
+            GB_TRY(di.alloc(k * sizeof(uint64_t), &v->err));
+            GB_TRY(dx.alloc(k * sz, &v->err));
             CU_TRY(cudaMemcpyAsync(di, v->hi.data(), k * sizeof(uint64_t), cudaMemcpyHostToDevice, G.stream), &v->err);
             CU_TRY(cudaMemcpyAsync(dx, v->hx.data(), k * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
             const int grid = (int)std::min<size_t>((k + 255) / 256, 4096);
-            vec_scatter_kernel<<<grid, 256, 0, G.stream>>>(di, (const uint8_t *)dx, (uint8_t *)v->dval, v->dpres, (int)sz, (int64_t)k);
+            vec_scatter_kernel<<<grid, 256, 0, G.stream>>>((const uint64_t *)di, (const uint8_t *)dx, (uint8_t *)dval, dpres, (int)sz, (int64_t)k);
             G.launches++;
             CU_TRY(cudaGetLastError(), &v->err);
-            dfree(di); dfree(dx);
         }
     } else if (n) {
         std::vector<uint8_t> vals(n * sz, 0), pres(full ? 0 : n, 0);
         for (size_t q = 0; q < k; ++q) { memcpy(&vals[v->hi[q] * sz], &v->hx[q * sz], sz); if (!full) pres[v->hi[q]] = 1; }
-        CU_TRY(cudaMemcpyAsync(v->dval, vals.data(), n * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
-        if (!full) CU_TRY(cudaMemcpyAsync(v->dpres, pres.data(), n, cudaMemcpyHostToDevice, G.stream), &v->err);
+        CU_TRY(cudaMemcpyAsync(dval, vals.data(), n * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
+        if (!full) CU_TRY(cudaMemcpyAsync(dpres, pres.data(), n, cudaMemcpyHostToDevice, G.stream), &v->err);
         CU_TRY(cudaStreamSynchronize(G.stream), &v->err);      // the staging vectors die here
     }
     CU_TRY(cudaStreamSynchronize(G.stream), &v->err);
+    v->dval = dval.release(); v->dpres = dpres.release();
     v->dev_valid = true; v->dev_nvals = (int64_t)v->hi.size();
     return GrB_SUCCESS;
 }
@@ -658,7 +650,7 @@ extern "C" GrB_Info GrB_Matrix_new(GrB_Matrix *A, GrB_Type type, GrB_Index nrows
 extern "C" GrB_Info GrB_Matrix_free(GrB_Matrix *A) {
     GB_LOCK;
     if (!A || !*A) return GrB_SUCCESS;
-    if ((*A)->magic == GB_MAGIC) { matrix_invalidate_device(*A); (*A)->magic = GB_FREED; delete *A; }
+    if ((*A)->magic == GB_MAGIC) { (*A)->magic = GB_FREED; delete *A; }
     *A = nullptr; return GrB_SUCCESS;
 }
 #define GB_MATRIX_OK(A, fn) do { if (!(A)) return gb_fail(GrB_NULL_POINTER, nullptr, fn ": NULL matrix"); \
@@ -668,9 +660,9 @@ extern "C" GrB_Info GrB_Matrix_free(GrB_Matrix *A) {
 
 static GrB_Info csr_clone(const Csr &a, size_t vsize, Csr &c, std::string *err) {
     c = Csr(); c.nrows = a.nrows; c.ncols = a.ncols; c.nnz = a.nnz;
-    GB_TRY(dalloc(&c.rowptr, (size_t)a.nrows + 1, err));
-    GB_TRY(dalloc(&c.col, (size_t)a.nnz, err));
-    GB_TRY(dmalloc(&c.val, (size_t)a.nnz * vsize + 16, err));
+    GB_TRY(c.rowptr.alloc((size_t)a.nrows + 1, err));
+    GB_TRY(c.col.alloc((size_t)a.nnz, err));
+    GB_TRY(c.val.alloc((size_t)a.nnz * vsize + 16, err));
     CU_TRY(cudaMemcpyAsync(c.rowptr, a.rowptr, ((size_t)a.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
     if (a.nnz) {
         CU_TRY(cudaMemcpyAsync(c.col, a.col, (size_t)a.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
@@ -873,12 +865,13 @@ extern "C" GrB_Info GrB_Vector_dup(GrB_Vector *w, const GrB_Vector u) {
     } else {
         o->host_valid = false;
         const size_t sz = u->type->size, n = (size_t)u->n;
-        GrB_Info r = dmalloc(&o->dval, n * sz + 16, &u->err);
-        if (r == GrB_SUCCESS && u->dpres) r = dmalloc((void **)&o->dpres, n + 16, &u->err);
-        if (r != GrB_SUCCESS) { dfree(o->dval); delete o; return r; }
-        cudaMemcpyAsync(o->dval, u->dval, n * sz, cudaMemcpyDeviceToDevice, G.stream);
-        if (u->dpres) cudaMemcpyAsync(o->dpres, u->dpres, n, cudaMemcpyDeviceToDevice, G.stream);
-        o->dev_valid = true; o->dev_nvals = u->dev_nvals;
+        DevBuf<void> dval; DevBuf<uint8_t> dpres;
+        GrB_Info r = dval.alloc(n * sz + 16, &u->err);
+        if (r == GrB_SUCCESS && u->dpres) r = dpres.alloc(n, &u->err);
+        if (r != GrB_SUCCESS) { delete o; return r; }
+        cudaMemcpyAsync(dval, u->dval, n * sz, cudaMemcpyDeviceToDevice, G.stream);
+        if (u->dpres) cudaMemcpyAsync(dpres, u->dpres, n, cudaMemcpyDeviceToDevice, G.stream);
+        o->dval = dval.release(); o->dpres = dpres.release(); o->dev_valid = true; o->dev_nvals = u->dev_nvals;
     }
     *w = o; return GrB_SUCCESS;
 }
@@ -1078,9 +1071,9 @@ extern "C" GrB_Info B200_Matrix_import_CSR(GrB_Matrix *A, GrB_Type type, GrB_Ind
     GrB_Matrix m = *A;
     Csr c; c.nrows = (int64_t)nrows; c.ncols = (int64_t)ncols; c.nnz = (int64_t)nvals;
     const size_t sz = type->size;
-    GrB_Info r = dalloc(&c.rowptr, (size_t)nrows + 1, &m->err);
-    if (r == GrB_SUCCESS) r = dalloc(&c.col, (size_t)nvals, &m->err);
-    if (r == GrB_SUCCESS) r = dmalloc(&c.val, (size_t)nvals * sz + 16, &m->err);
+    GrB_Info r = c.rowptr.alloc((size_t)nrows + 1, &m->err);
+    if (r == GrB_SUCCESS) r = c.col.alloc((size_t)nvals, &m->err);
+    if (r == GrB_SUCCESS) r = c.val.alloc((size_t)nvals * sz + 16, &m->err);
     if (r == GrB_SUCCESS) r = copy_in(c.rowptr, Ap, ((size_t)nrows + 1) * 8, where, &m->err);
     if (r == GrB_SUCCESS) r = copy_in(c.col, Aj, (size_t)nvals * 4, where, &m->err);
     if (r == GrB_SUCCESS) {
@@ -1095,8 +1088,8 @@ extern "C" GrB_Info B200_Matrix_import_CSR(GrB_Matrix *A, GrB_Type type, GrB_Ind
     }
     if (r == GrB_SUCCESS && !where && cudaStreamSynchronize(G.stream) != cudaSuccess) r = GrB_PANIC;
     if (r == GrB_SUCCESS) r = dev_build_rowptr32(c, &m->err);
-    if (r != GrB_SUCCESS) { csr_free(c); GrB_Matrix_free(A); return r; }
-    matrix_adopt_device(m, c);
+    if (r != GrB_SUCCESS) { GrB_Matrix_free(A); return r; }
+    matrix_adopt_device(m, std::move(c));
     return GrB_SUCCESS;
 }
 

@@ -897,8 +897,6 @@ template <bool FILL> __global__ void mat_finalize_kernel(const MatFinalizeArgs a
 #include "spgemm_stream.cuh"
 
 // ------------------------------------------------------------------ host side
-struct TypedCsr { Csr c; int tc; };   // a CSR whose values have type code tc
-
 static GrB_Info read_counts(const unsigned int *d, unsigned int *h, int n, std::string *err) {
     CU_TRY(cudaMemcpyAsync(h, d, n * sizeof(unsigned int), cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
@@ -957,21 +955,20 @@ static constexpr int MIDSMALL_TABLE = 1024;                       // masked: CTA
         if (!done_) return gb_fail(GrB_DOMAIN_MISMATCH, err, "mxm: unsupported semiring domains (x=%d, z=%d)", xt, zt); \
     } while (0)
 
-struct RowBins { int32_t *rows = nullptr; unsigned int count[4] = {0, 0, 0, 0}; unsigned int offset[4] = {0, 0, 0, 0}; };
+struct RowBins { DevBuf<int32_t> rows; unsigned int count[4] = {0, 0, 0, 0}; unsigned int offset[4] = {0, 0, 0, 0}; };
 
 static GrB_Info make_bins(const int64_t *work, int64_t nrows, BinLimits lim, RowBins &b, std::string *err) {
-    unsigned int *d = nullptr;
-    GB_TRY(dalloc(&d, 12, err));                       // counts[4] | offsets[4] | cursor[4]
+    DevBuf<unsigned int> d;
+    GB_TRY(d.alloc(12, err));                          // counts[4] | offsets[4] | cursor[4]
     CU_TRY(cudaMemsetAsync(d, 0, 12 * sizeof(unsigned int), G.stream), err);
     bin_count_kernel<<<grid_for(nrows), 256, 0, G.stream>>>(work, nrows, lim, d); GB_LAUNCHED();
     GB_TRY(read_counts(d, b.count, 4, err));
     b.offset[0] = 0;
     for (int k = 1; k < 4; ++k) b.offset[k] = b.offset[k - 1] + b.count[k - 1];
     CU_TRY(cudaMemcpyAsync(d + 4, b.offset, 4 * sizeof(unsigned int), cudaMemcpyHostToDevice, G.stream), err);
-    GB_TRY(dalloc(&b.rows, (size_t)nrows, err));
+    GB_TRY(b.rows.alloc((size_t)nrows, err));
     bin_fill_kernel<<<grid_for(nrows), 256, 0, G.stream>>>(work, nrows, lim, d + 4, d + 8, b.rows); GB_LAUNCHED();
     CU_TRY(cudaStreamSynchronize(G.stream), err);      // b.offset (host) was the source of an async copy
-    dfree(d);
     return GrB_SUCCESS;
 }
 
@@ -986,17 +983,17 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
                                 int add, int mul, bool need_a, bool need_b, Csr &T, std::string *err) {
     const int64_t nrows = A.nrows, ncols = B.ncols;
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
-    GB_TRY(dalloc(&T.rowptr, (size_t)nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-    int64_t *flops = nullptr; unsigned long long *total = nullptr;
-    GB_TRY(dalloc(&flops, (size_t)nrows, err)); GB_TRY(dalloc(&total, 1, err));
+    DevBuf<int64_t> flops; DevBuf<unsigned long long> total;
+    GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
     CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
     flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
     RowBins bins;
     GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
     int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
     G.last_flops = (uint64_t)total_flops;
-    dfree(flops); dfree(total);
+    flops.reset(); total.reset();
 
     GemmArgs g{};
     g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
@@ -1004,12 +1001,13 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     g.c_cnt = T.rowptr;
     const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
     const int spa_ctas = std::max(1, std::min<int>((int)bins.count[3], G.num_sms * 2));
-    unsigned int *queue = nullptr;
+    DevBuf<unsigned int> queue; DevBuf<uint32_t> spa_bits;
     if (bins.count[3]) {
         g.spa_words = ceil_div(ncols, 32);
-        GB_TRY(dalloc(&g.spa_bits, (size_t)spa_ctas * g.spa_words, err));
+        GB_TRY(spa_bits.alloc((size_t)spa_ctas * g.spa_words, err));
+        g.spa_bits = spa_bits;
         CU_TRY(cudaMemsetAsync(g.spa_bits, 0, (size_t)spa_ctas * g.spa_words * 4, G.stream), err);
-        GB_TRY(dalloc(&queue, 2, err));
+        GB_TRY(queue.alloc(2, err));
         CU_TRY(cudaMemsetAsync(queue, 0, 8, G.stream), err);
     }
     // ---- symbolic
@@ -1028,8 +1026,8 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
     T.nnz = nnz; G.last_nnz_out = (uint64_t)nnz;
-    GB_TRY(dalloc(&T.col, (size_t)nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)nnz * tc_size(zt) + 16, err));
+    GB_TRY(T.col.alloc((size_t)nnz, err));
+    GB_TRY(T.val.alloc((size_t)nnz * tc_size(zt) + 16, err));
     g.c_ptr = T.rowptr; g.c_col = T.col; g.c_val = T.val;
     // ---- numeric (shared-memory bins: expand-sort-compress unless B200GRB_SPGEMM_ESC=0 selects the hash kernels)
     const bool esc = tunables().spgemm_esc;
@@ -1053,14 +1051,15 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     }
     if (bins.count[3]) {
         g.rows = bins.rows + bins.offset[3]; g.nbin = bins.count[3]; g.queue = queue + 1;
-        GB_TRY(dmalloc(&g.spa_val, (size_t)spa_ctas * ncols * wsize + 16, err));
+        DevBuf<void> spa_val;
+        GB_TRY(spa_val.alloc((size_t)spa_ctas * ncols * wsize + 16, err));
+        g.spa_val = spa_val;
 #define K_SPA(XT, ZT, A_, M_) do { \
         spa_fill_identity<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
         spa_kernel<XT, ZT, A_, M_, true><<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2;
-        dfree(g.spa_val);
     }
-    dfree(g.spa_bits); dfree(queue); dfree(bins.rows);
+    spa_bits.reset(); queue.reset(); bins.rows.reset();
     GB_TRY(dev_build_rowptr32(T, err));
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
@@ -1098,7 +1097,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
     g.m_ptr = M.rowptr32; g.m_col = M.col; g.m_val = M.val; g.m_tc = mtc; g.m_struct = m_struct;
     g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
     PhaseTrace trace;
-    bool words_owned = false;
+    DevBuf<void> typed;                                        // 1- and 2-byte types: the accumulator words narrowed
     void *words = nullptr; uint8_t *found = nullptr;          // per mask entry: accumulator word, "has a value"
     GB_TRY(ws_get(WS_WORDS, &words, (size_t)M.nnz * wsize + 16, err));
     GB_TRY(ws_get(WS_FOUND, (void **)&found, (size_t)M.nnz + 16, err));
@@ -1187,27 +1186,26 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
             }
         }
         if (zsz < 4) {      // narrow 32-bit accumulator words to the 1- or 2-byte type, in a second buffer
-            void *typed = nullptr;
-            GB_TRY(dmalloc(&typed, (size_t)M.nnz * zsz + 16, err));
+            GB_TRY(typed.alloc((size_t)M.nnz * zsz + 16, err));
             narrow_words_kernel<<<grid_for(M.nnz), 256, 0, G.stream>>>((const uint32_t *)words, (uint8_t *)typed, (int)zsz, M.nnz); GB_LAUNCHED();
-            words = typed; words_owned = true;
+            words = typed;
         }
     }
     void *tval = words;
     // compact (pattern of M, found) -> CSR
-    GB_TRY(dalloc(&T.rowptr, (size_t)nrows + 1, err));
+    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
     if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, found, nrows, T.rowptr); GB_LAUNCHED(); }
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
     T.nnz = nnz; G.last_nnz_out = (uint64_t)nnz;
-    GB_TRY(dalloc(&T.col, (size_t)nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)nnz * zsz + 16, err));
+    GB_TRY(T.col.alloc((size_t)nnz, err));
+    GB_TRY(T.val.alloc((size_t)nnz * zsz + 16, err));
     if (nnz > 0) {
         row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)zsz,
                                                                           nrows, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
     }
-    if (words_owned) dfree(tval);
+    typed.reset();
     GB_TRY(dev_build_rowptr32(T, err));
     trace.mark("compaction");
     CU_TRY(cudaGetLastError(), err);
@@ -1228,15 +1226,15 @@ static GrB_Info matrix_finalize(const Csr *C, int ctc, const Csr &T, int ttc, co
     a.accum_op = accum ? accum->opcode : -1;
     a.accum_tc = accum ? accum->xtype->code : 0; a.accum_ztc = accum ? accum->ztype->code : 0;
     out = Csr(); out.nrows = T.nrows; out.ncols = T.ncols;
-    GB_TRY(dalloc(&out.rowptr, (size_t)nrows + 1, err));
+    GB_TRY(out.rowptr.alloc((size_t)nrows + 1, err));
     CU_TRY(cudaMemsetAsync(out.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
     a.o_cnt = out.rowptr;
     mat_finalize_kernel<false><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(out.rowptr, nrows + 1, err));
     int64_t nnz = 0; GB_TRY(read_i64(out.rowptr + nrows, &nnz, err));
     out.nnz = nnz;
-    GB_TRY(dalloc(&out.col, (size_t)nnz, err));
-    GB_TRY(dmalloc(&out.val, (size_t)nnz * tc_size(ctc) + 16, err));
+    GB_TRY(out.col.alloc((size_t)nnz, err));
+    GB_TRY(out.val.alloc((size_t)nnz * tc_size(ctc) + 16, err));
     a.o_ptr = out.rowptr; a.o_col = out.col; a.o_val = out.val;
     if (nnz > 0) { mat_finalize_kernel<true><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(out, err));
@@ -1246,11 +1244,12 @@ static GrB_Info matrix_finalize(const Csr *C, int ctc, const Csr &T, int ttc, co
 
 // write T (type ttc) back into C under mask / accum / replace; consumes T
 GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f,
-                          Csr &T, int ttc, bool t_already_masked, std::string *err) {
+                          Csr &&t_in, int ttc, bool t_already_masked, std::string *err) {
+    Csr T = std::move(t_in);
     const int ctc = C->type->code;
     if (!Mask && f.mask_comp) {
         // C<!NULL>: nothing is written; GrB_REPLACE clears C (C API 1.3 section 4.3, SuiteSparse's quick-mask exit)
-        csr_free(T);
+        T = Csr();
         if (f.replace) {
             matrix_invalidate_device(C);
             C->hi.clear(); C->hj.clear(); C->hx.clear(); C->pi.clear(); C->pj.clear(); C->px.clear(); C->host_valid = true;
@@ -1262,11 +1261,11 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     const bool plain = !accum && (!Mask || (t_already_masked && (f.replace || c_empty)));
     if (plain || (accum && !Mask && c_empty)) {
         if (ttc != ctc) {
-            void *cv = nullptr;
-            GB_TRY(dev_cast_values(&cv, ctc, T.val, ttc, T.nnz, err));
-            dfree(T.val); T.val = cv;
+            DevBuf<void> cv;
+            GB_TRY(dev_cast_values(cv, ctc, T.val, ttc, T.nnz, err));
+            T.val = std::move(cv);
         }
-        matrix_adopt_device(C, T);
+        matrix_adopt_device(C, std::move(T));
         return GrB_SUCCESS;
     }
     if (!c_empty) GB_TRY(matrix_ensure_device(C));
@@ -1274,9 +1273,9 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     Csr out;
     GrB_Info r = matrix_finalize(c_empty ? nullptr : &C->dev, ctc, T, ttc, Mask ? &Mask->dev : nullptr,
                                  Mask ? Mask->type->code : 0, f, accum, out, err);
-    csr_free(T);
-    if (r != GrB_SUCCESS) { csr_free(out); return r; }
-    matrix_adopt_device(C, out);
+    T = Csr();
+    if (r != GrB_SUCCESS) return r;
+    matrix_adopt_device(C, std::move(out));
     return GrB_SUCCESS;
 }
 
@@ -1302,7 +1301,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
     const bool need_a = op_uses_x(mul), need_b = op_uses_y(mul);
     GbBurble burble("GrB_mxm");
-    if (!Mask && f.mask_comp) { Csr none; return matrix_writeback(C, nullptr, accum, f, none, zt, false, err); }   // C<!NULL>: no product needed
+    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
 
     // masked methods apply to non-complemented masks
     const bool use_mask = Mask && !f.mask_comp;
@@ -1318,17 +1317,17 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     if (!a.rowptr32 || !b.rowptr32 || (Mask && !Mask->dev.rowptr32))
         return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
 
-    void *a_cast = nullptr, *b_cast = nullptr;
+    DevBuf<void> a_cast, b_cast;
     const void *aval = a.val, *bval = b.val;
-    if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(&a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
-    if (need_b && B->type->code != xt) { GB_TRY(dev_cast_values(&b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
+    if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
+    if (need_b && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
 
     Csr T; GrB_Info r;
     if (use_mask) r = spgemm_masked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, Mask->dev, Mask->type->code, f.mask_struct, dot, T, err);
     else r = spgemm_unmasked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, T, err);
-    dfree(a_cast); dfree(b_cast);
-    if (r != GrB_SUCCESS) { csr_free(T); return r; }
-    return matrix_writeback(C, Mask, accum, f, T, zt, use_mask, err);
+    a_cast.reset(); b_cast.reset();
+    if (r != GrB_SUCCESS) return r;
+    return matrix_writeback(C, Mask, accum, f, std::move(T), zt, use_mask, err);
 }
 
 // C<M> = accum(C, A')  -- used by the reference around the hot path (Matrix.transpose,
@@ -1349,14 +1348,14 @@ extern "C" GrB_Info GrB_transpose(GrB_Matrix C, const GrB_Matrix Mask, const GrB
     // T = copy of src (C may alias A)
     Csr T; T.nrows = src.nrows; T.ncols = src.ncols; T.nnz = src.nnz;
     const size_t sz = A->type->size;
-    GB_TRY(dalloc(&T.rowptr, (size_t)src.nrows + 1, err));
-    GB_TRY(dalloc(&T.col, (size_t)src.nnz, err));
-    GB_TRY(dmalloc(&T.val, (size_t)src.nnz * sz + 16, err));
+    GB_TRY(T.rowptr.alloc((size_t)src.nrows + 1, err));
+    GB_TRY(T.col.alloc((size_t)src.nnz, err));
+    GB_TRY(T.val.alloc((size_t)src.nnz * sz + 16, err));
     CU_TRY(cudaMemcpyAsync(T.rowptr, src.rowptr, ((size_t)src.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
     if (src.nnz) {
         CU_TRY(cudaMemcpyAsync(T.col, src.col, (size_t)src.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
         CU_TRY(cudaMemcpyAsync(T.val, src.val, (size_t)src.nnz * sz, cudaMemcpyDeviceToDevice, G.stream), err);
     }
     GB_TRY(dev_build_rowptr32(T, err));
-    return matrix_writeback(C, Mask, accum, f, T, A->type->code, false, err);
+    return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }

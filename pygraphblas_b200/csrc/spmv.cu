@@ -55,14 +55,16 @@ __global__ void spmv_plan_kernel(const uint32_t *rowptr, int64_t nrows, int64_t 
 }
 
 static GrB_Info spmv_plan(Csr &c, int tile, std::string *err) {
-    if (c.tile_row && c.tile_size == tile) return GrB_SUCCESS;
+    if (c.tile.row && c.tile.size == tile) return GrB_SUCCESS;
     if (!c.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "mxv: matrices with >= 2^32 entries are not supported");
-    dfree(c.tile_row); c.tile_row = nullptr;
-    c.ntiles = ceil_div(c.nnz, tile); c.tile_size = tile;
-    GB_TRY(dalloc(&c.tile_row, (size_t)c.ntiles + 1, err));
-    const int64_t n = c.ntiles + 1;
-    spmv_plan_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, G.stream>>>(c.rowptr32, c.nrows, c.ntiles, tile, c.tile_row); GB_LAUNCHED();
+    c.tile = TilePlan();
+    TilePlan p;
+    p.ntiles = ceil_div(c.nnz, tile); p.size = tile;
+    GB_TRY(p.row.alloc((size_t)p.ntiles + 1, err));
+    const int64_t n = p.ntiles + 1;
+    spmv_plan_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, G.stream>>>(c.rowptr32, c.nrows, p.ntiles, tile, p.row); GB_LAUNCHED();
     CU_TRY(cudaGetLastError(), err);
+    c.tile = std::move(p);
     return GrB_SUCCESS;
 }
 
@@ -378,7 +380,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const int xt = mulop->xtype->code, zt = addop->ztype->code;
     const int add = addop->opcode, mul = mulop->opcode;
     if (!mask && f.mask_comp)      // w<!NULL>: nothing is let through, no product needed (vector_write clears w under REPLACE)
-        return vector_write(w, nullptr, accum, f, nullptr, nullptr, zt, false, nullptr, true);
+        return vector_write(w, nullptr, accum, f, nullptr, nullptr, zt, false, nullptr);
 
     // ---- operands in HBM
     if (use_transpose) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
@@ -405,21 +407,22 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const int tile = SPMV_THREADS * (fast ? g_items_fast : g_items_generic);
     GB_TRY(spmv_plan(c, tile, err));
 
-    void *a_cast = nullptr, *u_cast = nullptr;
+    DevBuf<void> a_cast, u_cast;
     const void *aval = c.val, *uval = u->dval;
-    if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(&a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-    if (need_u && u->type->code != xt) { GB_TRY(dev_cast_values(&u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+    if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
+    if (need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
     // run-time-operator kernels always read both operands: give them something readable of the right type
-    if (!fast && !need_a && A->type->code != xt) { GB_TRY(dev_cast_values(&a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-    if (!fast && !need_u && u->type->code != xt) { GB_TRY(dev_cast_values(&u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+    if (!fast && !need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
+    if (!fast && !need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
 
     const int64_t n = (int64_t)out_n;
     const size_t zsz = (size_t)tc_size(zt);
     // T's buffers become w (no mask, no accumulator: w<-T).  When w already owns device buffers of the right shape and is not an
     // operand of this call, T is formed in place -- the iterated call `A.mxv(u, out=w)` then allocates nothing.
     void *tval = nullptr; uint8_t *tpres = nullptr;
+    DevBuf<void> t_val; DevBuf<uint8_t> t_pres;      // T's own buffers when it is not formed in w's
     const bool w_reusable = !need_final && w != u && w->dev_valid && w->dval && w->dpres && w->type->code == zt && !w->borrowed &&
-                            a_cast != w->dval && u_cast != w->dval;
+                            a_cast.get() != w->dval && u_cast.get() != w->dval;
     const bool in_place = w_reusable && (tn.mxv_inplace == 2 || (tn.mxv_inplace == 1 && !w->h2d_pending && !w->d2h_pending));
     if (in_place && tn.mxv_inplace == 2) {      // whatever the flags say: the kernels below start after w's last overlapped copies
         if (w->ev_h2d) { cudaStreamWaitEvent(G.stream, w->ev_h2d, 0); cudaStreamWaitEvent(G.stream, w->ev_d2h, 0); }
@@ -427,16 +430,17 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     }
     if (in_place) { tval = w->dval; tpres = w->dpres; }
     else {
-        GB_TRY(dmalloc(&tval, (size_t)n * zsz + 16, err));
-        GB_TRY(dmalloc((void **)&tpres, (size_t)n + 16, err));
+        GB_TRY(t_val.alloc((size_t)n * zsz + 16, err));
+        GB_TRY(t_pres.alloc((size_t)n, err));
+        tval = t_val; tpres = t_pres;
     }
 
     // mask + saturating monoid (BFS-shaped): skip masked-out rows, stop rows at the first hit
     const bool use_pull = mask != nullptr && (add == OP_LOR || add == OP_LAND || add == OP_ANY) && c.nnz > 0 && !tn.no_pull;
     if (use_pull) {
         // the run-time-operator kernel reads both operands: make sure both are of the operand type
-        if (aval == c.val && A->type->code != xt) { GB_TRY(dev_cast_values(&a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-        if (uval == u->dval && u->type->code != xt) { GB_TRY(dev_cast_values(&u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+        if (aval == c.val && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
+        if (uval == u->dval && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
         // few frontier edges: push along the rows of the other orientation (already in HBM) instead of pulling every row
         bool pushed = false;
         const Csr &o = use_transpose ? A->dev : A->devT;
@@ -453,12 +457,12 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         pa.tval = tval; pa.tpres = tpres; pa.add_op = add; pa.mul_op = kmul; pa.flip = kflip;
         // rows longer than PULL_LONG: at most nnz / PULL_LONG of them
         pa.long_cap = c.nnz / (int64_t)PULL_LONG + 1; pa.has_long = c.nnz > (int64_t)PULL_LONG;
-        GB_TRY(dalloc(&pa.long_rows, (size_t)pa.long_cap + 1, err));
-        GB_TRY(dalloc(&pa.long_count, 4, err));
+        DevBuf<uint32_t> long_rows; DevBuf<int> long_count;
+        GB_TRY(long_rows.alloc((size_t)pa.long_cap + 1, err));
+        GB_TRY(long_count.alloc(4, err));
+        pa.long_rows = long_rows; pa.long_count = long_count;
         CU_TRY(cudaMemsetAsync(pa.long_count, 0, sizeof(int), G.stream), err);
-        GrB_Info r = pushed ? GrB_SUCCESS : spmv_masked_pull_dispatch(xt, zt, pa, err);
-        dfree(pa.long_rows); dfree(pa.long_count);
-        if (r != GrB_SUCCESS) { if (!in_place) { dfree(tval); dfree(tpres); } dfree(a_cast); dfree(u_cast); return r; }
+        if (!pushed) GB_TRY(spmv_masked_pull_dispatch(xt, zt, pa, err));
     }
     // dense u + specialised semiring: warp-independent run kernel on the cached run plan
     const bool run_ok = !use_pull && (fast_sr || xt == zt || zt == TC_BOOL);     // specialised or run-time operators; dense or sparse u
@@ -470,61 +474,62 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     } else if (use_run) {
         GB_TRY(spmv_run_plan(c, err));
         RunArgs ra{};
-        ra.col = c.col; ra.aval = aval; ra.uval = uval; ra.headw = c.run_headw; ra.lane_rank = c.run_lane; ra.run_base = c.run_base;
-        ra.nzrow = c.nzrow; ra.rowptr = c.rowptr32; ra.nruns = c.nruns; ra.nnz = c.nnz; ra.tval = tval;
-        ra.tail_row = c.run_tail_row; ra.tail_last = c.run_tail_last;
+        const RunPlan &rp = c.run;
+        ra.col = c.col; ra.aval = aval; ra.uval = uval; ra.headw = rp.headw; ra.lane_rank = rp.lane; ra.run_base = rp.base;
+        ra.nzrow = rp.nzrow; ra.rowptr = c.rowptr32; ra.nruns = rp.nruns; ra.nnz = c.nnz; ra.tval = tval;
+        ra.tail_row = rp.tail_row; ra.tail_last = rp.tail_last;
         ra.add_op = add; ra.mul_op = kmul; ra.flip = kflip;
-        ra.head_val = c.ws_head; ra.tail_val = c.ws_tail;            // scratch kept with the plan (the library serialises calls)
-        if (sparse_u) { ra.upres = u->dpres; ra.tpres = tpres; ra.head_has = c.ws_head_has; ra.tail_has = c.ws_tail_has; }
+        ra.head_val = rp.ws_head; ra.tail_val = rp.ws_tail;            // scratch kept with the plan (the library serialises calls)
+        if (sparse_u) { ra.upres = u->dpres; ra.tpres = tpres; ra.head_has = rp.ws_head_has; ra.tail_has = rp.ws_tail_has; }
         // hot-column table: on by default for large matrices whose gathers are concentrated (R-MAT-like);
         // B200GRB_SPMV_HOT=0 disables it, =<KB> caps the table size (and forces the kernel whatever the coverage)
         int hot_kb = tn.spmv_hot_kb >= 0 ? tn.spmv_hot_kb : 128;     // stage + table stay inside the 196 KB carve-out: the 228 KB one leaves no L1
         if (fast && need_u && hot_kb > 0 && c.nnz >= ((int64_t)1 << 20) && c.ncols >= (1 << 16)) {
             GB_TRY(spmv_hot_plan(c, err));
-            if (!c.hcol || (tn.spmv_hot_kb < 0 && c.hot_cover < 0.25)) hot_kb = 0;
+            if (!c.hot.col || (tn.spmv_hot_kb < 0 && c.hot.cover < 0.25)) hot_kb = 0;
         } else hot_kb = 0;
         Hot2Args hot{};
         if (hot_kb > 0) {
             // one launch: u at the hot columns, T cleared, T's presence from the plan
             spmv_hot2_prep(c, uval, tc_size(xt), tval, (size_t)n * zsz, tpres);
-            ra.col = c.hcol; hot.u_hot = c.ws_uhot; hot.henc = c.henc; hot.tab_n = 0;
+            ra.col = c.hot.col; hot.u_hot = c.hot.ws_uhot; hot.henc = c.hot.henc; hot.tab_n = 0;
             kernel_name = "run+hot-table (TMA-staged)";
         } else {
             CU_TRY(cudaMemsetAsync(tval, 0, (size_t)n * zsz, G.stream), err);
             if (sparse_u) CU_TRY(cudaMemsetAsync(tpres, 0, (size_t)n, G.stream), err);     // presence follows u: written row by row
-            else CU_TRY(cudaMemcpyAsync(tpres, c.pres_tmpl, (size_t)n, cudaMemcpyDeviceToDevice, G.stream), err);
+            else CU_TRY(cudaMemcpyAsync(tpres, rp.pres_tmpl, (size_t)n, cudaMemcpyDeviceToDevice, G.stream), err);
             kernel_name = sparse_u ? "run (sparse u)" : "run";
         }
         const bool ok = fast_sr ? spmv_run_dispatch(xt, add, kmul, ra, hot_kb > 0 ? &hot : nullptr, (size_t)hot_kb << 10) : spmv_run_generic(xt, zt, ra);
-        if (!ok) { if (!in_place) { dfree(tval); dfree(tpres); } dfree(a_cast); dfree(u_cast); return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error"); }
+        if (!ok) return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
     } else if (c.nnz == 0) {
         clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
         kernel_name = "empty";
     } else {
         kernel_name = "tile";
         SpmvArgs a{};
-        a.rowptr = c.rowptr32; a.col = c.col; a.aval = aval; a.tile_row = c.tile_row; a.ntiles = c.ntiles;
+        a.rowptr = c.rowptr32; a.col = c.col; a.aval = aval; a.tile_row = c.tile.row; a.ntiles = c.tile.ntiles;
         a.nrows = c.nrows; a.nnz = c.nnz; a.uval = uval; a.upres = u->dpres; a.tval = tval; a.tpres = tpres;
         a.add_op = add; a.mul_op = kmul; a.flip = kflip; a.tile = tile;
-        GB_TRY(dmalloc(&a.head_val, (size_t)c.ntiles * zsz + 16, err));
-        GB_TRY(dmalloc(&a.tail_val, (size_t)c.ntiles * zsz + 16, err));
-        GB_TRY(dmalloc((void **)&a.head_has, (size_t)c.ntiles + 16, err));
-        GB_TRY(dmalloc((void **)&a.tail_has, (size_t)c.ntiles + 16, err));
-        GB_TRY(dalloc(&a.tail_row, (size_t)c.ntiles, err));
-        if (SPMV_PHASE_TIMERS && tn.spmv_debug) { GB_TRY(dalloc(&a.dbg, 8, err)); CU_TRY(cudaMemsetAsync(a.dbg, 0, 64, G.stream), err); }
-        GrB_Info r = spmv_dispatch(xt, zt, add, kmul, sparse_u, a, err);
+        const size_t nt = (size_t)c.tile.ntiles;
+        DevBuf<void> head_val, tail_val; DevBuf<uint8_t> head_has, tail_has; DevBuf<int32_t> tail_row; DevBuf<unsigned long long> dbg;
+        GB_TRY(head_val.alloc(nt * zsz + 16, err));
+        GB_TRY(tail_val.alloc(nt * zsz + 16, err));
+        GB_TRY(head_has.alloc(nt, err));
+        GB_TRY(tail_has.alloc(nt, err));
+        GB_TRY(tail_row.alloc(nt, err));
+        a.head_val = head_val; a.tail_val = tail_val; a.head_has = head_has; a.tail_has = tail_has; a.tail_row = tail_row;
+        if (SPMV_PHASE_TIMERS && tn.spmv_debug) { GB_TRY(dbg.alloc(8, err)); a.dbg = dbg; CU_TRY(cudaMemsetAsync(a.dbg, 0, 64, G.stream), err); }
+        GB_TRY(spmv_dispatch(xt, zt, add, kmul, sparse_u, a, err));
         if (a.dbg) {
             unsigned long long h[5];
             cudaMemcpyAsync(h, a.dbg, 40, cudaMemcpyDeviceToHost, G.stream); cudaStreamSynchronize(G.stream);
             if (h[4]) fprintf(stderr, "[spmv phases, avg cycles per tile] load+issue %.0f | rows+gather %.0f | fold+scan %.0f | carry+store %.0f | tiles %llu\n",
                               (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4], h[4]);
-            dfree(a.dbg);
         }
-        dfree(a.head_val); dfree(a.tail_val); dfree(a.head_has); dfree(a.tail_has); dfree(a.tail_row);
-        if (r != GrB_SUCCESS) { if (!in_place) { dfree(tval); dfree(tpres); } dfree(a_cast); dfree(u_cast); return r; }
     }
     if (burble.on) burble.note(kernel_name, (double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
-    dfree(a_cast); dfree(u_cast);
+    a_cast.reset(); u_cast.reset();
     vector_mark_used(u); if (mask) vector_mark_used(mask);          // an overlapped import into u may start as soon as these kernels are done
 
     if (in_place) {                    // T was formed in w's own buffers: only the bookkeeping changes
@@ -533,7 +538,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         return GrB_SUCCESS;
     }
     // ---- w<mask> = accum(w, t)   (vector_ops.cu)
-    return vector_write(w, mask, accum, f, tval, tpres, zt, /*t_scalar=*/false, /*region=*/nullptr, /*own_t=*/true);
+    return vector_write(w, mask, accum, f, tval, tpres, zt, /*t_scalar=*/false, /*region=*/nullptr, std::move(t_val), std::move(t_pres));
 }
 
 static GrB_Info mxv_check(GrB_Vector w, const GrB_Vector mask, const GrB_Semiring s, const GrB_Matrix A, const GrB_Vector u, const char *fn) {

@@ -251,7 +251,9 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     // LOR / LAND results are normalised only when the monoid type is BOOL (every builtin); ANY stores the product as is
     if ((a.add_op == OP_LOR || a.add_op == OP_LAND) && zt != TC_BOOL) return GrB_SUCCESS;
     if (!(xt == zt || zt == TC_BOOL)) return GrB_SUCCESS;
-    GB_TRY(dalloc(&a.counters, 4, err));
+    DevBuf<unsigned long long> counters; DevBuf<uint32_t> list; DevBuf<int64_t> chunk_scan;
+    GB_TRY(counters.alloc(4, err));
+    a.counters = counters;
     CU_TRY(cudaMemsetAsync(a.counters, 0, 32, G.stream), err);
     const int g = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nin, 256 * 4), (int64_t)G.num_sms * 8));
     push_stats_kernel<<<g, 256, 0, G.stream>>>(a); GB_LAUNCHED();
@@ -260,13 +262,15 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     CU_TRY(cudaStreamSynchronize(G.stream), err);
     const int64_t count = (int64_t)h[0], edges = (int64_t)h[1];
     // push pays per frontier vertex and per frontier edge, pull per unmasked row: push only small frontiers
-    if ((edges * 16 > nnz_total || count * 32 > a.nin) && !tunables().force_push) { dfree(a.counters); return GrB_SUCCESS; }
-    GB_TRY(dalloc(&a.list, (size_t)count + 1, err));
+    if ((edges * 16 > nnz_total || count * 32 > a.nin) && !tunables().force_push) return GrB_SUCCESS;
+    GB_TRY(list.alloc((size_t)count + 1, err));
+    a.list = list;
     if (count > 0) {
         const int gf = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nin, 256), (int64_t)G.num_sms * 16));
         push_frontier_kernel<<<gf, 256, 0, G.stream>>>(a); GB_LAUNCHED();
     }
-    GB_TRY(dalloc(&a.chunk_scan, (size_t)count + 2, err));
+    GB_TRY(chunk_scan.alloc((size_t)count + 2, err));
+    a.chunk_scan = chunk_scan;
     if (count > 0) {
         const int g2 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count + 1, 256), (int64_t)G.num_sms * 16));
         push_chunks_kernel<<<g2, 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
@@ -295,8 +299,6 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
         }
     }
 #undef GB_PUSH
-    dfree(a.list); dfree(a.counters); dfree(a.chunk_scan);
-    a.list = nullptr;
     CU_TRY(cudaGetLastError(), err);
     *done = ok;
     return GrB_SUCCESS;

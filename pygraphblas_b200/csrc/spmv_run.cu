@@ -47,41 +47,43 @@ __global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzro
 static inline int rgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 16)); }
 
 GrB_Info spmv_run_plan(Csr &c, std::string *err) {
-    if (c.run_headw) return GrB_SUCCESS;
+    if (c.run.headw) return GrB_SUCCESS;
     if (!c.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "mxv: matrices with >= 2^32 entries are not supported");
+    RunPlan p;                 // moved into c only once complete
     const int64_t nwords = ceil_div(c.nnz, 32);
-    c.nruns = ceil_div(c.nnz, RUN);
-    int64_t *flag = nullptr, *cnt = nullptr;
-    GB_TRY(dalloc(&flag, (size_t)c.nrows + 1, err));
-    GB_TRY(dalloc(&cnt, (size_t)c.nruns + 1, err));
-    GB_TRY(dalloc(&c.pres_tmpl, (size_t)c.nrows, err));
-    GB_TRY(dalloc(&c.run_headw, (size_t)nwords + 8, err));
-    GB_TRY(dalloc(&c.run_lane, (size_t)c.nruns * 32, err));
-    GB_TRY(dalloc(&c.run_base, (size_t)c.nruns + 1, err));
-    GB_TRY(dalloc(&c.run_tail_row, (size_t)c.nruns, err));
-    GB_TRY(dalloc(&c.run_tail_last, (size_t)c.nruns, err));
-    CU_TRY(cudaMemsetAsync(c.run_headw, 0, ((size_t)nwords + 8) * 4, G.stream), err);
+    p.nruns = ceil_div(c.nnz, RUN);
+    DevBuf<int64_t> flag, cnt;
+    GB_TRY(flag.alloc((size_t)c.nrows + 1, err));
+    GB_TRY(cnt.alloc((size_t)p.nruns + 1, err));
+    GB_TRY(p.pres_tmpl.alloc((size_t)c.nrows, err));
+    GB_TRY(p.headw.alloc((size_t)nwords + 8, err));
+    GB_TRY(p.lane.alloc((size_t)p.nruns * 32, err));
+    GB_TRY(p.base.alloc((size_t)p.nruns + 1, err));
+    GB_TRY(p.tail_row.alloc((size_t)p.nruns, err));
+    GB_TRY(p.tail_last.alloc((size_t)p.nruns, err));
+    CU_TRY(cudaMemsetAsync(p.headw, 0, ((size_t)nwords + 8) * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(flag + c.nrows, 0, 8, G.stream), err);
-    plan_nonempty_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, c.nrows, flag, c.pres_tmpl); GB_LAUNCHED();
+    plan_nonempty_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, c.nrows, flag, p.pres_tmpl); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(flag, c.nrows + 1, err));
     int64_t nz = 0;
     CU_TRY(cudaMemcpyAsync(&nz, flag + c.nrows, 8, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
-    c.nnzrows = nz;
-    GB_TRY(dalloc(&c.nzrow, (size_t)nz, err));
-    plan_rows_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, flag, c.nrows, c.nzrow, c.run_headw); GB_LAUNCHED();
-    CU_TRY(cudaMemsetAsync(cnt + c.nruns, 0, 8, G.stream), err);
-    plan_runs_kernel<<<(unsigned)ceil_div(c.nruns * 32, 256), 256, 0, G.stream>>>(c.run_headw, c.nruns, nwords, c.run_lane, cnt); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(cnt, c.nruns + 1, err));
-    plan_base_kernel<<<rgrid(c.nruns + 1), 256, 0, G.stream>>>(cnt, c.nruns, c.run_base); GB_LAUNCHED();
-    plan_tails_kernel<<<rgrid(c.nruns), 256, 0, G.stream>>>(c.run_base, c.nzrow, c.rowptr32, c.nruns, c.run_tail_row, c.run_tail_last); GB_LAUNCHED();
-    dfree(flag); dfree(cnt);
+    p.nnzrows = nz;
+    GB_TRY(p.nzrow.alloc((size_t)nz, err));
+    plan_rows_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
+    CU_TRY(cudaMemsetAsync(cnt + p.nruns, 0, 8, G.stream), err);
+    plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, p.lane, cnt); GB_LAUNCHED();
+    GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
+    plan_base_kernel<<<rgrid(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
+    plan_tails_kernel<<<rgrid(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, c.rowptr32, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
+    flag.reset(); cnt.reset();
     // per-call scratch lives with the plan: partials of the rows that straddle runs (8 bytes covers every type)
-    GB_TRY(dmalloc(&c.ws_head, (size_t)c.nruns * 8 + 16, err));
-    GB_TRY(dmalloc(&c.ws_tail, (size_t)c.nruns * 8 + 16, err));
-    GB_TRY(dmalloc((void **)&c.ws_head_has, (size_t)c.nruns + 16, err));
-    GB_TRY(dmalloc((void **)&c.ws_tail_has, (size_t)c.nruns + 16, err));
+    GB_TRY(p.ws_head.alloc((size_t)p.nruns * 8 + 16, err));
+    GB_TRY(p.ws_tail.alloc((size_t)p.nruns * 8 + 16, err));
+    GB_TRY(p.ws_head_has.alloc((size_t)p.nruns, err));
+    GB_TRY(p.ws_tail_has.alloc((size_t)p.nruns, err));
     CU_TRY(cudaGetLastError(), err);
+    c.run = std::move(p);
     return GrB_SUCCESS;
 }
 
@@ -112,39 +114,40 @@ __global__ void hot_encode_kernel(const uint32_t *col, const uint32_t *inv, int6
 }
 
 GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
-    if (c.hot_planned) return GrB_SUCCESS;
+    if (c.hot.planned) return GrB_SUCCESS;
     const int64_t n = c.ncols;
-    if (n + (int64_t)HOT_ENC >= ((int64_t)1 << 32)) { c.hot_planned = true; return GrB_SUCCESS; }
-    uint32_t *deg = nullptr, *deg_sorted = nullptr, *ids = nullptr, *inv = nullptr, *perm = nullptr; unsigned long long *stats = nullptr;
-    GB_TRY(dalloc(&deg, (size_t)n, err)); GB_TRY(dalloc(&deg_sorted, (size_t)n, err)); GB_TRY(dalloc(&ids, (size_t)n, err));
-    GB_TRY(dalloc(&inv, (size_t)n, err)); GB_TRY(dalloc(&perm, (size_t)n, err)); GB_TRY(dalloc(&stats, 2, err));
+    if (n + (int64_t)HOT_ENC >= ((int64_t)1 << 32)) { c.hot.planned = true; return GrB_SUCCESS; }
+    HotPlan p;                 // moved into c only once complete
+    DevBuf<uint32_t> deg, deg_sorted, ids, inv, perm; DevBuf<unsigned long long> stats;
+    GB_TRY(deg.alloc((size_t)n, err)); GB_TRY(deg_sorted.alloc((size_t)n, err)); GB_TRY(ids.alloc((size_t)n, err));
+    GB_TRY(inv.alloc((size_t)n, err)); GB_TRY(perm.alloc((size_t)n, err)); GB_TRY(stats.alloc(2, err));
     CU_TRY(cudaMemsetAsync(deg, 0, (size_t)n * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(inv, 0xff, (size_t)n * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(stats, 0, 16, G.stream), err);
     hot_count_kernel<<<hgrid(c.nnz), 256, 0, G.stream>>>(c.col, c.nnz, deg); GB_LAUNCHED();
     hot_iota_kernel<<<hgrid(n), 256, 0, G.stream>>>(ids, n); GB_LAUNCHED();
     size_t tmp_bytes = 0;     // stable sort: equal degrees keep ascending column order (deterministic plan)
-    CU_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, deg, deg_sorted, ids, perm, n, 0, 32, G.stream), err);
-    void *tmp = nullptr; GB_TRY(dmalloc(&tmp, tmp_bytes, err));
-    CU_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_bytes, deg, deg_sorted, ids, perm, n, 0, 32, G.stream), err);
+    CU_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, deg.get(), deg_sorted.get(), ids.get(), perm.get(), n, 0, 32, G.stream), err);
+    DevBuf<void> tmp; GB_TRY(tmp.alloc(tmp_bytes, err));
+    CU_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tmp_bytes, deg.get(), deg_sorted.get(), ids.get(), perm.get(), n, 0, 32, G.stream), err);
     G.launches += 8;
     const int64_t topk = std::min<int64_t>(n, HOT_ENC);
     hot_invert_kernel<<<hgrid(topk), 256, 0, G.stream>>>(perm, deg_sorted, topk, inv, stats); GB_LAUNCHED();
     unsigned long long h[2] = {0, 0};
     CU_TRY(cudaMemcpyAsync(h, stats, 16, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
-    c.hot_cover = c.nnz ? (double)h[1] / (double)c.nnz : 0.0;
-    c.hot_planned = true;
+    p.cover = c.nnz ? (double)h[1] / (double)c.nnz : 0.0;
+    p.planned = true;
     if (h[0] >= 16) {
-        c.henc = (uint32_t)h[0];
-        GB_TRY(dalloc(&c.hperm, (size_t)c.henc, err));
-        GB_TRY(dalloc(&c.hcol, (size_t)c.nnz, err));
-        GB_TRY(dmalloc(&c.ws_uhot, (size_t)c.henc * 8 + 16, err));
-        CU_TRY(cudaMemcpyAsync(c.hperm, perm, (size_t)c.henc * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-        hot_encode_kernel<<<hgrid(c.nnz), 256, 0, G.stream>>>(c.col, inv, c.nnz, c.henc, c.hcol); GB_LAUNCHED();
+        p.henc = (uint32_t)h[0];
+        GB_TRY(p.perm.alloc((size_t)p.henc, err));
+        GB_TRY(p.col.alloc((size_t)c.nnz, err));
+        GB_TRY(p.ws_uhot.alloc((size_t)p.henc * 8 + 16, err));
+        CU_TRY(cudaMemcpyAsync(p.perm, perm, (size_t)p.henc * 4, cudaMemcpyDeviceToDevice, G.stream), err);
+        hot_encode_kernel<<<hgrid(c.nnz), 256, 0, G.stream>>>(c.col, inv, c.nnz, p.henc, p.col); GB_LAUNCHED();
     }
-    dfree(tmp); dfree(deg); dfree(deg_sorted); dfree(ids); dfree(inv); dfree(perm); dfree(stats);
     CU_TRY(cudaGetLastError(), err);
+    c.hot = std::move(p);
     return GrB_SUCCESS;
 }
 
@@ -169,8 +172,8 @@ __global__ void __launch_bounds__(256) spmv_hot2_prep_kernel(const uint32_t *hpe
 // one launch ahead of the hot-table kernel: u at the hot columns, T cleared, T's presence from the plan's template
 void spmv_hot2_prep(const Csr &c, const void *u, int vsize, void *tval, size_t tval_bytes, uint8_t *tpres) {
     const int64_t tv16 = (int64_t)((tval_bytes + 15) / 16), pr16 = (c.nrows + 15) / 16;      // buffers are padded by >= 16 bytes
-    spmv_hot2_prep_kernel<<<G.num_sms * 8, 256, 0, G.stream>>>(c.hperm, (const uint8_t *)u, (uint8_t *)c.ws_uhot, vsize, c.henc,
-                                                               (uint4 *)tval, tv16, (const uint4 *)c.pres_tmpl, (uint4 *)tpres, pr16);
+    spmv_hot2_prep_kernel<<<G.num_sms * 8, 256, 0, G.stream>>>(c.hot.perm, (const uint8_t *)u, (uint8_t *)c.hot.ws_uhot, vsize, c.hot.henc,
+                                                               (uint4 *)tval, tv16, (const uint4 *)c.run.pres_tmpl, (uint4 *)tpres, pr16);
     GB_LAUNCHED();
 }
 

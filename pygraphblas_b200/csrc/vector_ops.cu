@@ -121,29 +121,29 @@ static bool finalize_typed(const VecFinalizeArgs &g) {
 }
 
 GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const DescFlags &f,
-                      void *tval, uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region, bool own_t) {
+                      const void *tval, const uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region,
+                      DevBuf<void> &&own_val, DevBuf<uint8_t> &&own_pres) {
     std::string *err = &w->err;
     const int64_t n = (int64_t)w->n;
     const int wtc = w->type->code;
     if (!mask && f.mask_comp) {
         // w<!NULL>: the complement of "no mask" lets nothing through -- w keeps its entries, or loses all of
         // them under GrB_REPLACE (GraphBLAS C API 1.3 section 4.3; SuiteSparse's quick-mask exit)
-        if (own_t) { dfree(tval); dfree(tpres); }
+        own_val.reset(); own_pres.reset();
         if (f.replace) {
             vector_invalidate_device(w);
             w->hi.clear(); w->hx.clear(); w->pi.clear(); w->px.clear(); w->host_valid = true;
         }
         return GrB_SUCCESS;
     }
-    const bool need_final = mask != nullptr || accum != nullptr || region != nullptr || t_scalar || !own_t;
-    if (!need_final) {
-        if (wtc == ttc) vector_adopt_device(w, tval, tpres);
-        else {
-            void *cv = nullptr;
-            GB_TRY(dev_cast_values(&cv, wtc, tval, ttc, n, err));
-            dfree(tval);
-            vector_adopt_device(w, cv, tpres);
+    const bool need_final = mask != nullptr || accum != nullptr || region != nullptr || t_scalar || !own_val;
+    if (!need_final) {      // w takes T's buffers
+        if (wtc != ttc) {
+            DevBuf<void> cv;
+            GB_TRY(dev_cast_values(cv, wtc, tval, ttc, n, err));
+            own_val = std::move(cv);
         }
+        vector_adopt_device(w, own_val.release(), own_pres.release());
         CU_TRY(cudaGetLastError(), err);
         return GrB_SUCCESS;
     }
@@ -158,17 +158,19 @@ GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp ac
     fa.accum_op = accum ? accum->opcode : -1;
     fa.accum_tc = accum ? accum->xtype->code : 0; fa.accum_ztc = accum ? accum->ztype->code : 0;
     fa.region = region;
-    GB_TRY(dmalloc(&fa.oval, (size_t)n * tc_size(wtc) + 16, err));
+    DevBuf<void> oval; DevBuf<uint8_t> opres;
+    GB_TRY(oval.alloc((size_t)n * tc_size(wtc) + 16, err));
+    fa.oval = oval;
     // a full w stays full under an accumulator (and a mask that does not replace), and a full T over the whole
     // vector without a mask gives a full result: no presence bytes, and the next mxv sees a dense operand
     // (SSSP: v = min(v, A' min.+ v))
     const bool w_full = !w_empty && w->dpres == nullptr;
     const bool out_full = (w_full && !(mask && f.replace) && (accum != nullptr || (region != nullptr && tpres == nullptr))) ||
                           (tpres == nullptr && !mask && !region);
-    if (!out_full) GB_TRY(dmalloc((void **)&fa.opres, (size_t)n + 16, err));
+    if (!out_full) { GB_TRY(opres.alloc((size_t)n, err)); fa.opres = opres; }
     if (!finalize_typed(fa)) { vec_finalize_kernel<<<vgrid(n), 256, 0, G.stream>>>(fa); GB_LAUNCHED(); }
-    if (own_t) { dfree(tval); dfree(tpres); }
-    vector_adopt_device(w, fa.oval, fa.opres);
+    own_val.reset(); own_pres.reset();
+    vector_adopt_device(w, oval.release(), opres.release());
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
@@ -227,11 +229,13 @@ static GrB_Info vec_ewise(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     EwiseArgs a{};
     a.n = n; a.mode = mode; a.op = op->opcode; a.xtc = op->xtype->code; a.ztc = op->ztype->code;
     a.uval = u->dval; a.upres = u->dpres; a.utc = u->type->code; a.vval = v->dval; a.vpres = v->dpres; a.vtc = v->type->code;
-    GB_TRY(dmalloc(&a.tval, (size_t)n * tc_size(a.ztc) + 16, &w->err));
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    GB_TRY(tval.alloc((size_t)n * tc_size(a.ztc) + 16, &w->err));
     const bool t_full = mode == EW_ADD ? (!u->dpres || !v->dpres) : (!u->dpres && !v->dpres);
-    if (!t_full) GB_TRY(dmalloc((void **)&a.tpres, (size_t)n + 16, &w->err));
+    if (!t_full) GB_TRY(tpres.alloc((size_t)n, &w->err));
+    a.tval = tval; a.tpres = tpres;
     vec_ewise_kernel<<<vgrid(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, a.ztc, false, nullptr, true);
+    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, a.ztc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Vector_eWiseAdd_BinaryOp(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_BinaryOp op,
                                                   const GrB_Vector u, const GrB_Vector v, const GrB_Descriptor desc) {
@@ -280,10 +284,12 @@ static GrB_Info vec_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     EwiseArgs a{};
     a.n = n; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar;
     a.uval = u->dval; a.upres = u->dpres; a.utc = u->type->code;
-    GB_TRY(dmalloc(&a.tval, (size_t)n * tc_size(ztc) + 16, &w->err));
-    if (u->dpres) GB_TRY(dmalloc((void **)&a.tpres, (size_t)n + 16, &w->err));
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    GB_TRY(tval.alloc((size_t)n * tc_size(ztc) + 16, &w->err));
+    if (u->dpres) GB_TRY(tpres.alloc((size_t)n, &w->err));
+    a.tval = tval; a.tpres = tpres;
     vec_ewise_kernel<<<vgrid(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, ztc, false, nullptr, true);
+    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, ztc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Vector_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_UnaryOp op, const GrB_Vector u, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
@@ -328,9 +334,9 @@ GrB_Info index_list(const GrB_Index *I, GrB_Index ni, uint64_t dim, bool *all, s
     if (out.size() == dim) { bool iota = true; for (uint64_t k = 0; k < dim && iota; ++k) iota = out[k] == k; if (iota) { *all = true; out.clear(); } }
     return GrB_SUCCESS;
 }
-static GrB_Info upload_indices(const std::vector<uint64_t> &idx, uint64_t **d, std::string *err) {
-    GB_TRY(dalloc(d, idx.size(), err));
-    CU_TRY(cudaMemcpyAsync(*d, idx.data(), idx.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, G.stream), err);
+static GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err) {
+    GB_TRY(d.alloc(idx.size(), err));
+    CU_TRY(cudaMemcpyAsync(d, idx.data(), idx.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);          // idx is a caller-owned temporary
     return GrB_SUCCESS;
 }
@@ -367,26 +373,23 @@ static GrB_Info vec_assign_scalar(GrB_Vector w, const GrB_Vector mask, const GrB
     GB_NEED_DEVICE(w, fn);
     // T: one value (of w's type) standing for every position of the region
     const int wtc = w->type->code;
-    void *tval = nullptr;
-    GB_TRY(dmalloc(&tval, 16, &w->err));
+    DevBuf<void> tval;
+    GB_TRY(tval.alloc(16, &w->err));
     uint64_t word[2] = {0, 0};
     sc_store(wtc, word, 0, sc_cast(sc_load(xtc, x, 0), xtc, wtc));
     CU_TRY(cudaMemcpyAsync(tval, word, 8, cudaMemcpyHostToDevice, G.stream), &w->err);
     CU_TRY(cudaStreamSynchronize(G.stream), &w->err);
-    uint8_t *region = nullptr;
+    DevBuf<uint8_t> region;
     if (!all) {
-        GB_TRY(dmalloc((void **)&region, (size_t)w->n + 16, &w->err));
+        GB_TRY(region.alloc((size_t)w->n, &w->err));
         CU_TRY(cudaMemsetAsync(region, 0, (size_t)w->n, G.stream), &w->err);
         if (!idx.empty()) {
-            uint64_t *didx = nullptr;
-            GB_TRY(upload_indices(idx, &didx, &w->err));
+            DevBuf<uint64_t> didx;
+            GB_TRY(upload_indices(idx, didx, &w->err));
             region_mark_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), region); GB_LAUNCHED();
-            dfree(didx);
         }
     }
-    const GrB_Info r = vector_write(w, mask, accum, desc_flags(desc), tval, nullptr, wtc, true, region, true);
-    dfree(region);
-    return r;
+    return vector_write(w, mask, accum, desc_flags(desc), tval, nullptr, wtc, true, region, std::move(tval));
 }
 
 extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Vector u, const GrB_Index *I, GrB_Index ni,
@@ -406,23 +409,21 @@ extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const
     const int utc = u->type->code;
     if (all) {
         if (w == u && !mask && !accum) return GrB_SUCCESS;
-        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr, /*own_t=*/false);
+        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr);
     }
-    void *tval = nullptr; uint8_t *tpres = nullptr, *region = nullptr; uint64_t *didx = nullptr;
+    DevBuf<void> tval; DevBuf<uint8_t> tpres, region;
     const size_t n = (size_t)w->n;
-    GB_TRY(dmalloc(&tval, n * tc_size(utc) + 16, &w->err));
-    GB_TRY(dmalloc((void **)&tpres, n + 16, &w->err));
-    GB_TRY(dmalloc((void **)&region, n + 16, &w->err));
+    GB_TRY(tval.alloc(n * tc_size(utc) + 16, &w->err));
+    GB_TRY(tpres.alloc(n, &w->err));
+    GB_TRY(region.alloc(n, &w->err));
     CU_TRY(cudaMemsetAsync(tpres, 0, n, G.stream), &w->err);
     CU_TRY(cudaMemsetAsync(region, 0, n, G.stream), &w->err);
     if (!idx.empty()) {
-        GB_TRY(upload_indices(idx, &didx, &w->err));
+        DevBuf<uint64_t> didx;
+        GB_TRY(upload_indices(idx, didx, &w->err));
         vec_scatter_u_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres, region); GB_LAUNCHED();
-        dfree(didx);
     }
-    const GrB_Info r = vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, region, true);
-    dfree(region);
-    return r;
+    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, region, std::move(tval), std::move(tpres));
 }
 
 extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Vector u, const GrB_Index *I, GrB_Index ni,
@@ -437,14 +438,14 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
         // a contiguous range (the slice v[a:b] of reference: pygraphblas/base.py:216-252): two device copies, no index list
         GB_TRY(vector_ensure_device(u));
         const size_t n = (size_t)w->n, sz = (size_t)tc_size(u->type->code);
-        void *tval = nullptr; uint8_t *tpres = nullptr;
-        GB_TRY(dmalloc(&tval, n * sz + 16, &w->err));
+        DevBuf<void> tval; DevBuf<uint8_t> tpres;
+        GB_TRY(tval.alloc(n * sz + 16, &w->err));
         CU_TRY(cudaMemcpyAsync(tval, (const uint8_t *)u->dval + (size_t)I[0] * sz, n * sz, cudaMemcpyDeviceToDevice, G.stream), &w->err);
         if (u->dpres) {
-            GB_TRY(dmalloc((void **)&tpres, n + 16, &w->err));
+            GB_TRY(tpres.alloc(n, &w->err));
             CU_TRY(cudaMemcpyAsync(tpres, u->dpres + I[0], n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
         }
-        return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, true);
+        return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, std::move(tval), std::move(tpres));
     }
     bool all; std::vector<uint64_t> idx;
     GB_TRY(index_list(I, ni, u->n, &all, idx, &w->err, fn));
@@ -455,18 +456,18 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
     const int utc = u->type->code;
     if (all) {
         if (w == u && !mask && !accum) return GrB_SUCCESS;
-        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr, /*own_t=*/false);
+        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr);
     }
-    void *tval = nullptr; uint8_t *tpres = nullptr; uint64_t *didx = nullptr;
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
     const size_t n = (size_t)w->n;
-    GB_TRY(dmalloc(&tval, n * tc_size(utc) + 16, &w->err));
-    GB_TRY(dmalloc((void **)&tpres, n + 16, &w->err));
+    GB_TRY(tval.alloc(n * tc_size(utc) + 16, &w->err));
+    GB_TRY(tpres.alloc(n, &w->err));
     if (!idx.empty()) {
-        GB_TRY(upload_indices(idx, &didx, &w->err));
+        DevBuf<uint64_t> didx;
+        GB_TRY(upload_indices(idx, didx, &w->err));
         vec_gather_u_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres); GB_LAUNCHED();
-        dfree(didx);
     }
-    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, nullptr, true);
+    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, nullptr, std::move(tval), std::move(tpres));
 }
 
 // ------------------------------------------------------------------ reduce to a scalar
@@ -503,8 +504,10 @@ GrB_Info dev_reduce_values(const void *val, const uint8_t *pres, int vtc, int64_
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256 * 8), (int64_t)G.num_sms * 8));
     ReduceArgs a{};
     a.n = n; a.val = val; a.pres = pres; a.vtc = vtc; a.op = op; a.mtc = mtc;
-    GB_TRY(dalloc(&a.part, (size_t)grid + 1, err));
-    GB_TRY(dalloc(&a.part_has, (size_t)grid + 1, err));
+    DevBuf<Sc> part; DevBuf<uint8_t> part_has;
+    GB_TRY(part.alloc((size_t)grid + 1, err));
+    GB_TRY(part_has.alloc((size_t)grid + 1, err));
+    a.part = part; a.part_has = part_has;
     vec_reduce_kernel<<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED();
     ReduceArgs b = a; b.n = grid; b.stage2 = 1;
     vec_reduce_kernel<<<1, 256, 0, G.stream>>>(b); GB_LAUNCHED();
@@ -512,7 +515,6 @@ GrB_Info dev_reduce_values(const void *val, const uint8_t *pres, int vtc, int64_
     CU_TRY(cudaMemcpyAsync(out, a.part + grid, sizeof(Sc), cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaMemcpyAsync(&rh, a.part_has + grid, 1, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
-    dfree(a.part); dfree(a.part_has);
     *has = rh != 0;
     return GrB_SUCCESS;
 }

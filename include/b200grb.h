@@ -224,6 +224,10 @@ uint64_t B200_kernel_launches(void);
  * the device (k = 0 switches it off); and the number of device blocks allocated and not yet freed */
 void B200_debug_fail_alloc(int64_t k);
 int64_t B200_debug_live_allocs(void);
+/* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("tile (specialised, 8 items)",
+ * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "hash-medium", "spa", "masked-warp", "stream-L",
+ * "dot", ...); recorded whether the burble is on or not, valid until the next such call */
+const char *B200_debug_last_kernel(void);
 /* per-matrix SpGEMM/SpMV work figures of the most recent GrB_mxm (flops = number of
  * multiplies, nnz_out = nvals of the semiring product before accum/mask) */
 GrB_Info B200_last_mxm_stats(uint64_t *flops, uint64_t *nnz_out);

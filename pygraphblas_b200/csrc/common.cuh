@@ -184,9 +184,11 @@ struct GBGlobal {
     uint64_t last_flops = 0, last_nnz_out = 0;
     int burble = 0;
     cudaEvent_t burble_e0 = nullptr, burble_e1 = nullptr;
+    std::string last_kernel;      // kernel paths of the last GrB_mxv / GrB_vxm / GrB_mxm, separated by ';' (B200_debug_last_kernel)
     std::recursive_mutex mu;
 };
 extern GBGlobal G;
+static inline void gb_kernel_used(const char *k) { if (!G.last_kernel.empty()) G.last_kernel += ';'; G.last_kernel += k; }
 extern thread_local std::string tl_error;
 
 GrB_Info gb_fail(GrB_Info code, std::string *where, const char *fmt, ...);

@@ -169,6 +169,7 @@ extern "C" GrB_Info B200_device_synchronize(void) {
 static int64_t g_fail_alloc = 0, g_live_allocs = 0;
 extern "C" void B200_debug_fail_alloc(int64_t k) { g_fail_alloc = k > 0 ? k : 0; }
 extern "C" int64_t B200_debug_live_allocs(void) { return g_live_allocs; }
+extern "C" const char *B200_debug_last_kernel(void) { return G.last_kernel.c_str(); }
 
 GrB_Info dmalloc(void **p, size_t bytes, std::string *err) {
     *p = nullptr;

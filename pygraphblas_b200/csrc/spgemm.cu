@@ -19,6 +19,7 @@
 // accumulator, typecasts) is a row-wise three-way merge (matrix_finalize).
 #include "common.cuh"
 #include <algorithm>
+#include <limits>
 #include <type_traits>
 
 static inline int grid_for(int64_t n, int threads = 256) {
@@ -44,11 +45,32 @@ template <typename ZT> __host__ __device__ __forceinline__ ZT unpack_slot(typena
     ZT v; memcpy(&v, &w, sizeof(ZT)); return v;
 }
 
-// *addr = add(*addr, v) atomically; works on shared and global addresses
+// Starting value of an accumulator slot that the products of one entry are folded into (its presence is kept apart: keys,
+// bitmaps or found flags).  Integer and BOOL monoids start from their identity.  FP monoids start from the identity of the IEEE
+// operation, which fmin / fmax / + leave every x unchanged with: fmin(NaN, x) = fmax(NaN, x) = x and -0.0 + x = x.  The monoid
+// identities are not that: fmin(+Inf, NaN) = +Inf and +0.0 + -0.0 = +0.0, so an entry whose only product is NaN (or -0.0)
+// would come out +Inf (or +0.0) where the fold from the first product gives NaN (-0.0).
+template <typename ZT> __host__ __device__ __forceinline__ ZT accum_init(int add) {
+    if constexpr (std::is_floating_point<ZT>::value) {
+        if (add == OP_MIN || add == OP_MAX) return std::numeric_limits<ZT>::quiet_NaN();
+        if (add == OP_PLUS) return (ZT)-0.0;
+    }
+    return monoid_identity<ZT>(add);
+}
+
+// *addr = add(*addr, v) atomically; works on shared and global addresses.
+//
+// FP32 PLUS: atomicAdd(float *) on a global address is RED.ADD.F32.FTZ on sm_90, which flushes subnormal operands and results to
+// zero.  For |v| >= 2^-100 (or v = +-Inf) the flush cannot change the sum, so the reduction is used there: (i) a subnormal *addr
+// is below half an ulp of v, so the exact sum rounds to v, which is what the flushed operand gives; (ii) for a normal *addr the
+// sum is 0 or at least 2^-124 in magnitude (either |*addr| < |v| / 2, or both are multiples of 2^-124), never subnormal.
+// Smaller v, zeros and NaN take the compare-and-swap loop, whose plain add keeps subnormals.
 template <typename ZT> __device__ __forceinline__ void atomic_combine(typename SlotWord<ZT>::W *addr, ZT v, int add) {
     typedef typename SlotWord<ZT>::W W;
     if (add == OP_ANY) { *addr = pack_slot<ZT>(v); return; }
-    if constexpr (std::is_same<ZT, float>::value) { if (add == OP_PLUS) { atomicAdd(reinterpret_cast<float *>(addr), v); return; } }
+    if constexpr (std::is_same<ZT, float>::value) {
+        if (add == OP_PLUS && fabsf(v) >= 0x1p-100f) { atomicAdd(reinterpret_cast<float *>(addr), v); return; }
+    }
     if constexpr (std::is_same<ZT, double>::value) { if (add == OP_PLUS) { atomicAdd(reinterpret_cast<double *>(addr), v); return; } }
     if constexpr (std::is_same<ZT, int32_t>::value || std::is_same<ZT, uint32_t>::value) {
         if (add == OP_PLUS) { atomicAdd(reinterpret_cast<unsigned int *>(addr), (unsigned int)v); return; }
@@ -98,7 +120,7 @@ struct GemmArgs {
     int table;                                   // hash table size (power of two)
     int group;                                   // threads per row: 32 (warp) or blockDim (CTA)
     // dense accumulator workspace (one slice per CTA)
-    uint32_t *spa_bits; void *spa_val; int32_t *spa_slot; int64_t spa_words; unsigned int *queue;
+    uint32_t *spa_bits; void *spa_val; int64_t spa_words; unsigned int *queue;
 };
 
 // ------------------------------------------------------------------ flop count + binning
@@ -231,7 +253,7 @@ __global__ void __launch_bounds__(256) hash_numeric_kernel(const GemmArgs p) {
     const bool active = idx < p.nbin;
     const uint32_t tmask = (uint32_t)p.table - 1;
     const int hshift = __clz(p.table) + 1;                            // 32 - log2(table)
-    const W ident = pack_slot<ZT>(monoid_identity<ZT>(add));
+    const W ident = pack_slot<ZT>(accum_init<ZT>(add));
     for (int s = tid; s < p.table; s += gsize) { packed[s] = ((unsigned long long)EMPTY_KEY << 32) | (unsigned)s; vals[s] = ident; }
     group_sync<WARP>();
     const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
@@ -444,7 +466,7 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
     const int mul = MUL >= 0 ? MUL : p.mul_op;
     uint32_t *bits = p.spa_bits + (size_t)blockIdx.x * p.spa_words;
     W *spa = NUMERIC ? static_cast<W *>(p.spa_val) + (size_t)blockIdx.x * p.ncols : nullptr;
-    const W ident = pack_slot<ZT>(monoid_identity<ZT>(add));
+    const W ident = pack_slot<ZT>(accum_init<ZT>(add));
     const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     while (true) {
@@ -506,16 +528,14 @@ template <typename W> __global__ void fill_words_kernel(W *a, W v, int64_t n) {
 }
 
 // ------------------------------------------------------------------ masked: shared-memory hash of the mask row
-// Work unit = a "chunk": (row i, a slice of A(i,:)) whose flop count is bounded, so that hub rows are
-// spread over many CTAs.  Every chunk hashes the mask row M(i,:) (keys -> position inside the row),
-// then streams the B rows named by its slice of A(i,:) and accumulates products that hit the mask.
-// A warp handles 32 A entries at a time: each lane fetches one (k, B row range) up front, the ranges
-// are broadcast by shuffle and the lanes stride the B row -- the dependent-load chain per A entry
-// is paid once per 32 entries.
+// Rows whose products and mask row are both short (the warp class): one warp per row hashes the mask row M(i,:)
+// (keys -> position inside the row), then streams the B rows named by A(i,:) and accumulates the products that hit it.
+// The warp handles 32 A entries at a time: each lane fetches one (k, B row range) up front, the ranges are broadcast by
+// shuffle and the lanes stride the B row -- the dependent-load chain per A entry is paid once per 32 entries.
+// Heavier rows are cut into chunks and go to the streaming kernel (spgemm_stream.cuh).
 struct MaskedArgs {
     GemmArgs g;
-    const int32_t *chunk_row; const uint32_t *chunk_idx; const uint32_t *chunk_cnt; int64_t nchunks;
-    void *t_words;     // nnz(M) accumulator words (pre-set to the monoid identity)
+    void *t_words;     // nnz(M) accumulator words
 };
 
 template <typename XT, typename ZT, typename Hit>
@@ -540,69 +560,16 @@ __device__ __forceinline__ void stream_b_rows(const GemmArgs &p, uint32_t pa0, u
     }
 }
 
-// Load-balanced streaming of the B rows named by A entries [c0, c1) for a whole CTA of NT threads:
-// NT entries at a time, the B-row lengths are prefix-summed in shared memory and the flattened
-// (entry, position) space is dealt out in runs of 8 consecutive positions per thread, so a hub B row
-// is spread over the whole CTA and short rows do not leave lanes idle.
-template <int NT, typename XT, typename Hit>
-__device__ __forceinline__ void flat_stream(const GemmArgs &p, uint32_t c0, uint32_t c1, uint32_t *s_off, uint32_t *s_bs, XT *s_av,
-                                            int *s_warp, Hit &&hit) {
-    const XT *aval = static_cast<const XT *>(p.a_val);
-    const int tid = threadIdx.x;
-    for (uint32_t base = c0; base < c1; base += NT) {
-        const uint32_t pa = base + tid;
-        const bool valid = pa < c1;
-        uint32_t bs = 0, len = 0;
-        XT av = (XT)1;
-        if (valid) {
-            const uint32_t k = __ldg(p.a_col + pa);
-            bs = __ldg(p.b_ptr + k); len = __ldg(p.b_ptr + k + 1) - bs;
-            if (p.need_a) av = gload<XT>(aval + pa);
-        }
-        int total = 0;
-        const int off = block_exclusive_scan((int)len, s_warp, &total);
-        s_off[tid] = (uint32_t)off; s_bs[tid] = bs; s_av[tid] = av;
-        __syncthreads();
-        const int nent = (int)min((uint32_t)NT, c1 - base);
-        constexpr uint32_t RUN = 8;
-        for (uint32_t f0 = (uint32_t)tid * RUN; f0 < (uint32_t)total; f0 += NT * RUN) {
-            int lo = 0, hi = nent - 1;                       // largest e with s_off[e] <= f0
-            while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (s_off[mid] <= f0) lo = mid; else hi = mid - 1; }
-            int e = lo;
-            // locate the run's positions first, then issue all its column loads back to back, then probe
-            uint32_t pbv[RUN], jv[RUN]; XT avv[RUN]; int cnt = 0;
-#pragma unroll
-            for (uint32_t i = 0; i < RUN; ++i) {
-                const uint32_t f = f0 + i;
-                if (f < (uint32_t)total) {
-                    while (e + 1 < nent && s_off[e + 1] <= f) ++e;
-                    pbv[i] = s_bs[e] + (f - s_off[e]); avv[i] = s_av[e]; cnt = (int)i + 1;
-                }
-            }
-#pragma unroll
-            for (uint32_t i = 0; i < RUN; ++i) if ((int)i < cnt) jv[i] = __ldg(p.b_col + pbv[i]);
-#pragma unroll
-            for (uint32_t i = 0; i < RUN; ++i) if ((int)i < cnt) hit(jv[i], avv[i], pbv[i]);
-        }
-        __syncthreads();
-    }
-}
-
-template <typename XT, typename ZT, int ADD, int MUL, bool WARP>
+template <typename XT, typename ZT, int ADD, int MUL>
 __global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgs ma) {
     typedef typename SlotWord<ZT>::W W;
     const GemmArgs &p = ma.g;
     extern __shared__ unsigned char smem_raw[];
-    __shared__ unsigned int s_next;
     const int add = ADD >= 0 ? ADD : p.add_op;
     const int mul = MUL >= 0 ? MUL : p.mul_op;
-    const int gsize = WARP ? 32 : blockDim.x;
-    const int gid = WARP ? (threadIdx.x >> 5) : 0;
-    const int tid = WARP ? (threadIdx.x & 31) : threadIdx.x;
-    const int groups = WARP ? (blockDim.x >> 5) : 1;
-    const int lane = threadIdx.x & 31;
+    const int gid = threadIdx.x >> 5, lane = threadIdx.x & 31, groups = blockDim.x >> 5;
     const int half = p.table >> 1;                                    // max mask-row length
-    // layout per group: keys[table] u32 | slot[table] u32 | vals[half] W | found[half] u8
+    // layout per warp: keys[table] u32 | slot[table] u32 | vals[half] W | found[half] u8
     const size_t per_group = (size_t)p.table * 8 + (size_t)half * sizeof(W) + (size_t)half;
     unsigned char *basep = smem_raw + (size_t)gid * ((per_group + 15) & ~(size_t)15);
     uint32_t *keys = reinterpret_cast<uint32_t *>(basep);
@@ -610,121 +577,46 @@ __global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgs ma) {
     W *vals = reinterpret_cast<W *>(slot + p.table);
     uint8_t *found = reinterpret_cast<uint8_t *>(vals + half);
     const int64_t idx = (int64_t)blockIdx.x * groups + gid;
-    const bool active = WARP ? idx < p.nbin : idx < ma.nchunks;
+    if (idx >= p.nbin) return;                                        // a whole warp
     const uint32_t tmask = (uint32_t)p.table - 1;
     const int hshift = __clz(p.table) + 1;                            // 32 - log2(table)
-    const W ident = pack_slot<ZT>(monoid_identity<ZT>(add));
-    int64_t row = 0; uint32_t ms = 0, me = 0, nparts = 1, part = 0;
-    if (active) {
-        if (WARP) row = p.rows[idx];
-        else { row = ma.chunk_row[idx]; part = ma.chunk_idx[idx]; nparts = ma.chunk_cnt[idx]; }
-        ms = p.m_ptr[row]; me = p.m_ptr[row + 1];
-    }
+    const W ident = pack_slot<ZT>(accum_init<ZT>(add));
+    const int64_t row = p.rows[idx];
+    const uint32_t ms = p.m_ptr[row], me = p.m_ptr[row + 1];
     const int mlen = (int)(me - ms);
-    for (int s = tid; s < p.table; s += gsize) keys[s] = EMPTY_KEY;
-    for (int s = tid; s < mlen; s += gsize) { vals[s] = ident; found[s] = 0; }
-    if (!WARP && threadIdx.x == 0) s_next = 0;
-    group_sync<WARP>();
-    if (active) {
-        for (uint32_t q = ms + tid; q < me; q += gsize) {
-            bool on = true;
-            if (!p.m_struct) on = sc_cast(sc_load(p.m_tc, p.m_val, q), p.m_tc, TC_BOOL).u != 0;
-            if (!on) continue;
-            const uint32_t j = p.m_col[q];
-            uint32_t s = hash_col(j, hshift);
-            while (atomicCAS(&keys[s], EMPTY_KEY, j) != EMPTY_KEY) s = (s + 1) & tmask;   // mask columns are unique
-            slot[s] = q - ms;
-        }
+    for (int s = lane; s < p.table; s += 32) keys[s] = EMPTY_KEY;
+    for (int s = lane; s < mlen; s += 32) { vals[s] = ident; found[s] = 0; }
+    __syncwarp();
+    for (uint32_t q = ms + lane; q < me; q += 32) {
+        bool on = true;
+        if (!p.m_struct) on = sc_cast(sc_load(p.m_tc, p.m_val, q), p.m_tc, TC_BOOL).u != 0;
+        if (!on) continue;
+        const uint32_t j = p.m_col[q];
+        uint32_t s = hash_col(j, hshift);
+        while (atomicCAS(&keys[s], EMPTY_KEY, j) != EMPTY_KEY) s = (s + 1) & tmask;   // mask columns are unique
+        slot[s] = q - ms;
     }
-    group_sync<WARP>();
-    if (active) {
-        const XT *bval = static_cast<const XT *>(p.b_val);
-        auto hit = [&](uint32_t j, XT av, uint32_t pb) {
-            uint32_t s = hash_col(j, hshift);
-            while (true) {
-                const uint32_t kk = keys[s];
-                if (kk == j) {
-                    const uint32_t q = slot[s];
-                    const XT bv = p.need_b ? gload<XT>(bval + pb) : (XT)1;
-                    atomic_combine<ZT>(&vals[q], MulApply<XT, ZT>::f(mul, av, bv), add);
-                    found[q] = 1;
-                    return;
-                }
-                if (kk == EMPTY_KEY) return;
-                s = (s + 1) & tmask;
-            }
-        };
-        const uint32_t as = p.a_ptr[row], ae = p.a_ptr[row + 1];
-        if (WARP) stream_b_rows<XT, ZT>(p, as, ae, lane, hit);
-        else {
-            // this chunk's slice of A(i,:): flattened over the whole CTA
-            __shared__ uint32_t s_off[256], s_bs[256];
-            __shared__ XT s_av[256];
-            __shared__ int s_warp[33];
-            const uint32_t alen = ae - as;
-            const uint32_t c0 = as + (uint32_t)(((uint64_t)alen * part) / nparts), c1 = as + (uint32_t)(((uint64_t)alen * (part + 1)) / nparts);
-            flat_stream<256, XT>(p, c0, c1, s_off, s_bs, s_av, s_warp, hit);
-        }
-    }
-    group_sync<WARP>();
-    if (active) {
-        W *tw = static_cast<W *>(ma.t_words);
-        if (nparts == 1) {
-            for (int q = tid; q < mlen; q += gsize) { tw[ms + q] = vals[q]; p.t_found[ms + q] = found[q]; }
-        } else {
-            for (int q = tid; q < mlen; q += gsize) if (found[q]) {
-                atomic_combine<ZT>(&tw[ms + q], unpack_slot<ZT>(vals[q]), add);
-                p.t_found[ms + q] = 1;
-            }
-        }
-    }
-}
-
-// masked, long mask rows: a dense column -> mask-position map in HBM owned by a persistent CTA;
-// chunks come from a queue and accumulate straight into the global accumulator words.
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(512) masked_spa_kernel(const MaskedArgs ma) {
-    typedef typename SlotWord<ZT>::W W;
-    const GemmArgs &p = ma.g;
-    __shared__ unsigned int s_next;
-    __shared__ uint32_t s_off[512], s_bs[512];
-    __shared__ XT s_av[512];
-    __shared__ int s_warp[33];
-    const int add = ADD >= 0 ? ADD : p.add_op;
-    const int mul = MUL >= 0 ? MUL : p.mul_op;
-    int32_t *slot = p.spa_slot + (size_t)blockIdx.x * p.ncols;      // -1 everywhere when idle
+    __syncwarp();
     const XT *bval = static_cast<const XT *>(p.b_val);
-    W *tw = static_cast<W *>(ma.t_words);
-    const int lane = threadIdx.x & 31;
-    while (true) {
-        if (threadIdx.x == 0) s_next = atomicAdd(p.queue, 1u);
-        __syncthreads();
-        const unsigned int idx = s_next;
-        if (idx >= ma.nchunks) break;
-        const int64_t row = ma.chunk_row[idx];
-        const uint32_t part = ma.chunk_idx[idx], nparts = ma.chunk_cnt[idx];
-        const uint32_t ms = p.m_ptr[row], me = p.m_ptr[row + 1];
-        for (uint32_t q = ms + threadIdx.x; q < me; q += blockDim.x) {
-            bool on = true;
-            if (!p.m_struct) on = sc_cast(sc_load(p.m_tc, p.m_val, q), p.m_tc, TC_BOOL).u != 0;
-            if (on) slot[p.m_col[q]] = (int32_t)q;
-        }
-        __syncthreads();
-        auto hit = [&](uint32_t j, XT av, uint32_t pb) {
-            const int32_t q = slot[j];
-            if (q >= 0) {
+    auto hit = [&](uint32_t j, XT av, uint32_t pb) {
+        uint32_t s = hash_col(j, hshift);
+        while (true) {
+            const uint32_t kk = keys[s];
+            if (kk == j) {
+                const uint32_t q = slot[s];
                 const XT bv = p.need_b ? gload<XT>(bval + pb) : (XT)1;
-                atomic_combine<ZT>(&tw[q], MulApply<XT, ZT>::f(mul, av, bv), add);
-                p.t_found[q] = 1;
+                atomic_combine<ZT>(&vals[q], MulApply<XT, ZT>::f(mul, av, bv), add);
+                found[q] = 1;
+                return;
             }
-        };
-        const uint32_t as = p.a_ptr[row], ae = p.a_ptr[row + 1], alen = ae - as;
-        const uint32_t c0 = as + (uint32_t)(((uint64_t)alen * part) / nparts), c1 = as + (uint32_t)(((uint64_t)alen * (part + 1)) / nparts);
-        flat_stream<512, XT>(p, c0, c1, s_off, s_bs, s_av, s_warp, hit);
-        __syncthreads();
-        for (uint32_t q = ms + threadIdx.x; q < me; q += blockDim.x) slot[p.m_col[q]] = -1;
-        __syncthreads();
-    }
+            if (kk == EMPTY_KEY) return;
+            s = (s + 1) & tmask;
+        }
+    };
+    stream_b_rows<XT, ZT>(p, p.a_ptr[row], p.a_ptr[row + 1], lane, hit);
+    __syncwarp();
+    W *tw = static_cast<W *>(ma.t_words);
+    for (int q = lane; q < mlen; q += 32) { tw[ms + q] = vals[q]; p.t_found[ms + q] = found[q]; }
 }
 
 // per-row chunk counts: class 1 rows (warp kernel) get 0 chunks
@@ -756,9 +648,9 @@ __global__ void chunk_fill_kernel(const int64_t *off_small, const int64_t *off_m
     }
 }
 
-template <typename ZT> static void spa_fill_identity(void *words, int64_t n, int add) {
+template <typename ZT> static void fill_accum_init(void *words, int64_t n, int add) {
     typedef typename SlotWord<ZT>::W W;
-    fill_words_kernel<W><<<grid_for(n), 256, 0, G.stream>>>(static_cast<W *>(words), pack_slot<ZT>(monoid_identity<ZT>(add)), n);
+    fill_words_kernel<W><<<grid_for(n), 256, 0, G.stream>>>(static_cast<W *>(words), pack_slot<ZT>(accum_init<ZT>(add)), n);
 }
 
 // accumulator words (32-bit) -> 1- or 2-byte typed values
@@ -1037,7 +929,7 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
 #define K_SMALL(XT, ZT, A_, M_) hash_numeric_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(g.nbin, 8), 256, sm, G.stream>>>(g)
 #define K_ESC_SMALL(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
         if (esc) GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); else GB_FOR_SEMIRING(xt, zt, add, mul, K_SMALL, err);
-        GB_LAUNCHED();
+        GB_LAUNCHED(); gb_kernel_used(esc ? "esc-small" : "hash-small");
     }
     if (bins.count[2]) {
         g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
@@ -1047,7 +939,7 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
         hash_numeric_kernel<XT, ZT, A_, M_, false><<<(unsigned)g.nbin, 256, sm, G.stream>>>(g); } while (0)
 #define K_ESC_MEDIUM(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, false><<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
         if (esc) GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); else GB_FOR_SEMIRING(xt, zt, add, mul, K_MEDIUM, err);
-        GB_LAUNCHED();
+        GB_LAUNCHED(); gb_kernel_used(esc ? "esc-medium" : "hash-medium");
     }
     if (bins.count[3]) {
         g.rows = bins.rows + bins.offset[3]; g.nbin = bins.count[3]; g.queue = queue + 1;
@@ -1055,9 +947,9 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
         GB_TRY(spa_val.alloc((size_t)spa_ctas * ncols * wsize + 16, err));
         g.spa_val = spa_val;
 #define K_SPA(XT, ZT, A_, M_) do { \
-        spa_fill_identity<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
+        fill_accum_init<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
         spa_kernel<XT, ZT, A_, M_, true><<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2;
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2; gb_kernel_used("spa");
     }
     spa_bits.reset(); queue.reset(); bins.rows.reset();
     GB_TRY(dev_build_rowptr32(T, err));
@@ -1106,15 +998,15 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
     if (M.nnz > 0 && dot) {
         // the dot kernel writes typed values directly
 #define K_DOT(XT, ZT, A_, M_) masked_dot_kernel<XT, ZT, A_, M_><<<grid_for(nrows * 32), 256, 0, G.stream>>>(g)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_DOT, err); GB_LAUNCHED();
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_DOT, err); GB_LAUNCHED(); gb_kernel_used("dot");
     } else if (M.nnz > 0) {
         int64_t *flops = nullptr; unsigned long long *total = nullptr;
         GB_TRY(ws_array(WS_FLOPS, &flops, (size_t)nrows, err)); GB_TRY(ws_array(WS_TOTAL, &total, 1, err));
         CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
         flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
-        // accumulators start at the identity, flags at 0
+        // accumulators start at accum_init, flags at 0
         CU_TRY(cudaMemsetAsync(found, 0, (size_t)M.nnz, G.stream), err);
-#define K_IDENT(XT, ZT, A_, M_) spa_fill_identity<ZT>(words, M.nnz, (A_) >= 0 ? (A_) : add)
+#define K_IDENT(XT, ZT, A_, M_) fill_accum_init<ZT>(words, M.nnz, (A_) >= 0 ? (A_) : add)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_IDENT, err); GB_LAUNCHED();
         // classify rows and cut heavy ones into flop-bounded chunks
         int64_t *cs = nullptr, *cm = nullptr, *cl = nullptr, *c1 = nullptr;
@@ -1143,8 +1035,8 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
         if (n_warp) {
             g.rows = w_rows; g.nbin = n_warp; g.table = SMALL_TABLE;
             const size_t sm = masked_smem(SMALL_TABLE, 8, wsize);
-#define K_MSMALL(XT, ZT, A_, M_) masked_hash_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(n_warp, 8), 256, sm, G.stream>>>(ma)
-            GB_FOR_SEMIRING(xt, zt, add, mul, K_MSMALL, err); GB_LAUNCHED();
+#define K_MSMALL(XT, ZT, A_, M_) masked_hash_kernel<XT, ZT, A_, M_><<<(unsigned)ceil_div(n_warp, 8), 256, sm, G.stream>>>(ma)
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_MSMALL, err); GB_LAUNCHED(); gb_kernel_used("masked-warp");
         }
         // chunked classes: the streaming kernel (spgemm_stream.cuh), persistent CTAs over blocks of consecutive chunks
         {
@@ -1182,6 +1074,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
                             ctas = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(sa.nchunks, sa.grab), (int64_t)G.num_sms * std::max(per_sm, 1))); } \
                 kern<<<ctas, nt, sm, G.stream>>>(sa); } while (0)
                 GB_FOR_SEMIRING(xt, zt, add, mul, K_MSTREAM, err); GB_LAUNCHED();
+                gb_kernel_used(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
                 trace.mark(k == 0 ? "stream S" : (k == 1 ? "stream M" : "stream L"));
             }
         }
@@ -1301,6 +1194,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
     const bool need_a = op_uses_x(mul), need_b = op_uses_y(mul);
     GbBurble burble("GrB_mxm");
+    G.last_kernel.clear();
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
 
     // masked methods apply to non-complemented masks

@@ -22,7 +22,7 @@
 struct StreamArgs {
     GemmArgs g;
     const int32_t *chunk_row; const uint32_t *chunk_idx; const uint32_t *chunk_cnt; int64_t nchunks;
-    void *t_words;                  // nnz(M) accumulator words (pre-set to the monoid identity)
+    void *t_words;                  // nnz(M) accumulator words (pre-set to accum_init)
     unsigned int *queue;            // next block of chunks
     int bm_log2;                    // bitmap bits = 1 << bm_log2
     int exact;                      // 1: bit index = column id (ncols <= bitmap bits); 0: one multiplicative hash
@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
     const uint32_t item_len = 1u << sa.blk_log2;               // positions of a long B row one work item covers
     const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
     W *tw = static_cast<W *>(sa.t_words);
-    const W ident = pack_slot<ZT>(monoid_identity<ZT>(add));
+    const W ident = pack_slot<ZT>(accum_init<ZT>(add));
     uint2 *myq = s_q + warp * STREAM_QCAP;
     uint16_t *myqe = s_qe + warp * STREAM_QCAP;
 

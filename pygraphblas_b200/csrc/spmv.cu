@@ -298,7 +298,7 @@ template <typename T> static bool spmv_fast(int add, int mul, int items, const S
     return false;
 }
 static bool spmv_fast_bool(int add, int mul, int items, const SpmvArgs &a) {
-#define GB_FAST(A, M) if (add == A && mul == M) { if (items == 16) spmv_launch<bool, bool, A, M, false, 16>(a); else spmv_launch<bool, bool, A, M, false, 8>(a); return true; }
+#define GB_FAST(A, M) if (add == A && mul == M) { if (items == 16) spmv_launch<bool, bool, A, M, false, 16>(a); else if (items == 4) spmv_launch<bool, bool, A, M, false, 4>(a); else spmv_launch<bool, bool, A, M, false, 8>(a); return true; }
     GB_FAST(OP_LOR, OP_LAND) GB_FAST(OP_ANY, OP_PAIR) GB_FAST(OP_LOR, OP_PAIR) GB_FAST(OP_LOR, OP_SECOND) GB_FAST(OP_LOR, OP_FIRST)
 #undef GB_FAST
     return false;
@@ -379,6 +379,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
     const int xt = mulop->xtype->code, zt = addop->ztype->code;
     const int add = addop->opcode, mul = mulop->opcode;
+    G.last_kernel.clear();
     if (!mask && f.mask_comp)      // w<!NULL>: nothing is let through, no product needed (vector_write clears w under REPLACE)
         return vector_write(w, nullptr, accum, f, nullptr, nullptr, zt, false, nullptr);
 
@@ -437,12 +438,12 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
 
     // mask + saturating monoid (BFS-shaped): skip masked-out rows, stop rows at the first hit
     const bool use_pull = mask != nullptr && (add == OP_LOR || add == OP_LAND || add == OP_ANY) && c.nnz > 0 && !tn.no_pull;
+    bool pushed = false;
     if (use_pull) {
         // the run-time-operator kernel reads both operands: make sure both are of the operand type
         if (aval == c.val && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
         if (uval == u->dval && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
         // few frontier edges: push along the rows of the other orientation (already in HBM) instead of pulling every row
-        bool pushed = false;
         const Csr &o = use_transpose ? A->dev : A->devT;
         if (sparse_u && o.valid && o.rowptr32 && o.nnz == c.nnz && A->type->code == xt && !tn.no_push) {
             PushArgs ps{};
@@ -470,7 +471,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     if (tn.spmv_run >= 0) use_run = run_ok && c.nnz > 0 && tn.spmv_run != 0;
     const char *kernel_name = "pull";
     if (use_pull) {
-        // done above
+        if (pushed) kernel_name = "push";
     } else if (use_run) {
         GB_TRY(spmv_run_plan(c, err));
         RunArgs ra{};
@@ -493,7 +494,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
             // one launch: u at the hot columns, T cleared, T's presence from the plan
             spmv_hot2_prep(c, uval, tc_size(xt), tval, (size_t)n * zsz, tpres);
             ra.col = c.hot.col; hot.u_hot = c.hot.ws_uhot; hot.henc = c.hot.henc; hot.tab_n = 0;
-            kernel_name = "run+hot-table (TMA-staged)";
+            kernel_name = tc_size(xt) <= 4 && tn.spmv_pipe ? "run+hot-table (TMA-staged, pipelined)" : "run+hot-table (TMA-staged)";
         } else {
             CU_TRY(cudaMemsetAsync(tval, 0, (size_t)n * zsz, G.stream), err);
             if (sparse_u) CU_TRY(cudaMemsetAsync(tpres, 0, (size_t)n, G.stream), err);     // presence follows u: written row by row
@@ -506,7 +507,8 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
         kernel_name = "empty";
     } else {
-        kernel_name = "tile";
+        kernel_name = !fast ? "tile (run-time operators)" : g_items_fast == 4 ? "tile (specialised, 4 items)"
+                    : g_items_fast == 16 ? "tile (specialised, 16 items)" : "tile (specialised, 8 items)";
         SpmvArgs a{};
         a.rowptr = c.rowptr32; a.col = c.col; a.aval = aval; a.tile_row = c.tile.row; a.ntiles = c.tile.ntiles;
         a.nrows = c.nrows; a.nnz = c.nnz; a.uval = uval; a.upres = u->dpres; a.tval = tval; a.tpres = tpres;
@@ -528,6 +530,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
                               (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4], h[4]);
         }
     }
+    gb_kernel_used(kernel_name);
     if (burble.on) burble.note(kernel_name, (double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
     a_cast.reset(); u_cast.reset();
     vector_mark_used(u); if (mask) vector_mark_used(mask);          // an overlapped import into u may start as soon as these kernels are done

@@ -149,3 +149,84 @@ def test_fast_kernels_match_oracle():
     L.fast_masked_dot_plus_pair_i64(ctypes.c_int64(n), p(lp), p(lj), p(lp), p(lj), p(lp), p(lj), p(cval2), p(chas2))
     Cd = orc.mxm(orc.SpMat("INT64", n, n), Lo, None, ("PLUS", "PAIR", "INT64"), Lo, Lo, "ST1")
     assert int(cval2.sum()) == int(Cd.X.sum()) and int(chas2.sum()) == Cd.nvals
+
+
+# ------------------------------------------------------------------ the oracle at the edges of each type
+def _dot(sr, a, b, atype=None, btype=None, ctype=None):
+    """C(0,0) of the 1 x n times n x 1 product under semiring sr, or None when it has no entry."""
+    atype, btype = atype or sr[2], btype or sr[2]
+    n = len(a)
+    A = orc.SpMat(atype, 1, n, np.zeros(n), np.arange(n), np.asarray(a, orc.DTYPES[atype]))
+    B = orc.SpMat(btype, n, 1, np.arange(n), np.zeros(n), np.asarray(b, orc.DTYPES[btype]))
+    C = orc.mxm(orc.SpMat(ctype or orc.semiring_ztype(sr), 1, 1), None, None, sr, A, B)
+    return C.X[0] if C.nvals else None
+
+
+def _bits(x):
+    return np.asarray(x).view(np.uint64 if np.asarray(x).dtype.itemsize == 8 else np.uint32).item()
+
+
+def test_oracle_integers_wrap():
+    assert _dot(("PLUS", "TIMES", "INT8"), [127, 1], [2, 1]) == -1               # 254 -> -2, then + 1
+    assert _dot(("PLUS", "FIRST", "INT8"), [127, 1], [0, 0]) == -128
+    assert _dot(("TIMES", "SECOND", "INT16"), [1, 1], [256, 256]) == 0          # 2^16 wraps to 0
+    assert _dot(("PLUS", "MINUS", "INT32"), [-2**31], [1]) == 2**31 - 1
+    assert _dot(("PLUS", "TIMES", "UINT64"), [2**63, 2**63], [1, 1]) == 0
+    assert _dot(("MAX", "FIRST", "UINT64"), [2**63, 1], [0, 0]) == 2**63          # unsigned order
+    assert _dot(("MIN", "SECOND", "UINT64"), [0, 0], [2**64 - 1, 2**63]) == 2**63
+    assert _dot(("BXNOR", "BXNOR", "UINT8"), [0], [0]) == 255
+
+
+def test_oracle_integer_division_rules():
+    div = lambda t, x, y: _dot(("PLUS", "DIV", t), [x], [y])
+    assert div("INT32", -2**31, -1) == -2**31                                    # INT_MIN / -1 wraps
+    assert div("INT8", -128, -1) == -128
+    assert div("INT32", 5, 0) == 2**31 - 1 and div("INT32", -5, 0) == -2**31 and div("INT32", 0, 0) == 0
+    assert div("UINT8", 5, 0) == 255 and div("UINT8", 0, 0) == 0
+    assert div("INT16", -7, 2) == -3                                               # truncation toward zero
+    assert _dot(("PLUS", "RDIV", "INT64"), [-1], [-2**63]) == -2**63
+
+
+def test_oracle_float_to_integer_casts_saturate():
+    # operands cast to the multiply's type: NaN -> 0, out of range -> the nearest end, fractions truncate
+    a = np.array([np.nan, 1e10, -1e10, 3.7, -3.7, np.inf, -np.inf], np.float64)
+    for k, want in enumerate([0, 127, -128, 3, -3, 127, -128]):
+        assert _dot(("PLUS", "FIRST", "INT8"), [a[k]], [1], atype="FP64") == want, a[k]
+    for k, want in enumerate([0, 10**10, 0, 3, 0, 2**64 - 1, 0]):
+        assert _dot(("PLUS", "FIRST", "UINT64"), [a[k]], [1], atype="FP64") == want, a[k]
+    # the write-back cast of the result: FP32 result into an INT16 output
+    assert _dot(("PLUS", "TIMES", "FP32"), [np.inf], [1], ctype="INT16") == 2**15 - 1
+    assert _dot(("PLUS", "TIMES", "FP32"), [np.nan], [1], ctype="INT16") == 0
+    assert _dot(("PLUS", "TIMES", "FP32"), [-1e30], [1], ctype="UINT32") == 0
+    assert _dot(("PLUS", "TIMES", "FP64"), [1e300], [1], ctype="UINT64") == 2**64 - 1
+
+
+def test_oracle_fp_min_max_ignore_nan_and_keep_signs():
+    nan, inf = np.nan, np.inf
+    assert _dot(("MIN", "FIRST", "FP32"), [nan, 2.0], [0, 0]) == 2.0
+    assert _dot(("MIN", "FIRST", "FP32"), [2.0, nan], [0, 0]) == 2.0
+    assert np.isnan(_dot(("MIN", "FIRST", "FP32"), [nan], [0]))                   # a sole NaN product stays NaN (an entry)
+    assert np.isnan(_dot(("MIN", "PLUS", "FP32"), [inf], [-inf]))                 # +Inf + -Inf = NaN, not +Inf
+    assert _dot(("MAX", "FIRST", "FP64"), [-inf, nan], [0, 0]) == -inf
+    assert np.isnan(_dot(("MAX", "TIMES", "FP64"), [0.0], [inf]))
+    m = _dot(("PLUS", "FIRST", "FP32"), [-0.0], [1])                              # a sole -0.0 keeps its sign
+    assert _bits(m) == _bits(np.float32(-0.0))
+    assert _bits(_dot(("PLUS", "FIRST", "FP64"), [-0.0, 0.0], [1, 1])) == 0       # -0 + +0 = +0
+    tiny = np.finfo(np.float32).smallest_subnormal
+    assert _dot(("PLUS", "TIMES", "FP32"), [tiny, tiny], [1, 2]) == np.float32(3) * tiny      # subnormals are kept
+    assert _dot(("PLUS", "DIV", "FP64"), [1.0, -1.0], [0.0, 0.0]) is not None and np.isnan(_dot(("PLUS", "DIV", "FP64"), [1.0, -1.0], [0.0, 0.0]))
+
+
+def test_edge_value_pools():
+    for t in util.ALL_T:
+        pool = util.edge_values(t)
+        assert pool.dtype == orc.DTYPES[t] and len(np.unique(pool.view(f"u{pool.dtype.itemsize}") if t != "BOOL" else pool)) == len(pool)
+    f32 = util.edge_values("FP32")
+    assert np.isnan(f32).sum() == 1 and (f32 == np.inf).sum() == 1 and np.signbit(f32[f32 == 0]).sum() == 1
+    sub = f32[(f32 != 0) & (np.abs(f32) < np.finfo(np.float32).tiny)]
+    assert len(sub) == 4 and np.abs(sub).min() == np.finfo(np.float32).smallest_subnormal
+    assert set(util.edge_values("UINT64").tolist()) == {0, 1, 2, 2**63 - 1, 2**63, 2**64 - 2, 2**64 - 1}
+    assert util.edge_values("INT16").min() == -2**15
+    rng = np.random.default_rng(0)
+    v = util.rand_edge_values(rng, "INT32", 4000, 0.5)
+    assert 600 < (np.abs(v.astype(np.int64)) > 5).sum() < 1200                   # half from the pool, 4 of its 9 values are large

@@ -132,3 +132,50 @@ def semirings_for(typ):
            ("MAX", "PLUS", typ), ("PLUS", "MINUS", typ), ("TIMES", "PLUS", typ), ("PLUS", "LAND", typ),
            ("LOR", "EQ", typ), ("LOR", "GT", typ), ("LXOR", "LT", typ), ("ANY", "PAIR", typ)]
     return out
+
+
+# ------------------------------------------------------------------ edge values
+FP_T = ["FP32", "FP64"]
+
+
+def edge_values(typ):
+    """A fixed pool of the values where kernels and CPU references part ways, for each type: the ends of the integer
+    range (and UINT* values at and above 2^(w-1)), and for FP NaN, +-Inf, +-0, the smallest and largest subnormal, the
+    smallest normal and the largest finite value (both signs), and a few ordinary values."""
+    dt = orc.DTYPES[typ]
+    if typ == "BOOL":
+        return np.array([False, True])
+    if typ in FP_T:
+        fi = np.finfo(dt)
+        sub_lo, sub_hi, norm_lo = fi.smallest_subnormal, fi.tiny - fi.smallest_subnormal, fi.tiny
+        vals = [np.nan, np.inf, -np.inf, 0.0, -0.0, sub_lo, -sub_lo, sub_hi, -sub_hi, norm_lo, -norm_lo,
+                fi.max, -fi.max, 1.0, -1.0, 0.5, 3.0]
+        return np.array(vals, dtype=dt)
+    info = np.iinfo(dt)
+    if info.min < 0:
+        vals = [info.min, info.min + 1, -2, -1, 0, 1, 2, info.max - 1, info.max]
+    else:
+        half = 1 << (info.bits - 1)
+        vals = [0, 1, 2, half - 1, half, info.max - 1, info.max]
+    return np.array(vals, dtype=dt)
+
+
+def rand_edge_values(rng, typ, n, ratio=0.5, pool=None):
+    """n values: each drawn from `pool` (default edge_values(typ)) with probability `ratio`, else from rand_values."""
+    pool = edge_values(typ) if pool is None else np.asarray(pool, dtype=orc.DTYPES[typ])
+    out = rand_values(rng, typ, n)
+    pick = rng.random(n) < ratio
+    out[pick] = pool[rng.integers(0, len(pool), int(pick.sum()))]
+    return out
+
+
+def rand_edge_mat(rng, typ, nrows, ncols, density, ratio=0.5, pool=None):
+    d = rand_mat(rng, typ, nrows, ncols, density)
+    d["X"] = rand_edge_values(rng, typ, len(d["I"]), ratio, pool).tolist()
+    return d
+
+
+def rand_edge_vec(rng, typ, size, density, ratio=0.5, pool=None):
+    d = rand_vec(rng, typ, size, density)
+    d["X"] = rand_edge_values(rng, typ, len(d["I"]), ratio, pool).tolist()
+    return d

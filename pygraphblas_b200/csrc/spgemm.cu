@@ -1043,6 +1043,11 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
             unsigned int *queues = nullptr;
             GB_TRY(ws_array(WS_QUEUES, &queues, 4, err));
             CU_TRY(cudaMemsetAsync(queues, 0, 16, G.stream), err);
+            // The 128-bit loads of a trip reach up to 3 positions past B's last entry, into the padding of its allocation (dmalloc
+            // rounds to 256 bytes).  The filter indexes its bitmap with a loaded id before the position test drops it, so with an
+            // exact bitmap a stray id there would read shared memory out of range: those positions must hold valid ids (0).
+            if (B.nnz % 4 && (n_small || n_medium || n_long))
+                CU_TRY(cudaMemsetAsync(B.col.get() + B.nnz, 0, (size_t)(4 - B.nnz % 4) * sizeof(uint32_t), G.stream), err);
             StreamArgs sa{}; sa.g = g; sa.t_words = words;
             struct Cls { int64_t n; const int32_t *row; const uint32_t *idx, *cnt; int nt, bm_log2, vals_cap, grab; };
             const Cls cls[3] = {{n_small, s_row, s_idx, s_cnt, 256, 14, MIDSMALL_TABLE / 2, 8},
@@ -1075,6 +1080,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
                 kern<<<ctas, nt, sm, G.stream>>>(sa); } while (0)
                 GB_FOR_SEMIRING(xt, zt, add, mul, K_MSTREAM, err); GB_LAUNCHED();
                 gb_kernel_used(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
+                gb_kernel_used(sa.exact ? "filter=exact" : "filter=bloom");
                 trace.mark(k == 0 ? "stream S" : (k == 1 ? "stream M" : "stream L"));
             }
         }

@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
                     uint32_t tb = s & ~3u;
                     uint32_t pb = tb + (uint32_t)lane * 4u;
                     uint4 c = make_uint4(0u, 0u, 0u, 0u);
-                    if (pb < e) c = __ldg(reinterpret_cast<const uint4 *>(p.b_col + pb));      // arrays are padded: reading past e is safe
+                    if (pb < e) c = __ldg(reinterpret_cast<const uint4 *>(p.b_col + pb));      // past e: inside B's allocation, valid ids (spgemm_masked)
                     for (; tb < e || (flush && qn > 0); tb += 128u) {
                         const uint32_t pbn = pb + 128u;
                         uint4 cn = make_uint4(0u, 0u, 0u, 0u);

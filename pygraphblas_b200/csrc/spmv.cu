@@ -531,6 +531,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         }
     }
     gb_kernel_used(kernel_name);
+    if (in_place) gb_kernel_used("mxv=in-place");
     if (burble.on) burble.note(kernel_name, (double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
     a_cast.reset(); u_cast.reset();
     vector_mark_used(u); if (mask) vector_mark_used(mask);          // an overlapped import into u may start as soon as these kernels are done

@@ -111,10 +111,10 @@ struct RunPlan {
 struct HotPlan {
     DevBuf<uint32_t> perm;           // [henc] hot rank -> original column
     DevBuf<uint32_t> col;            // [nnz] encoded column ids
-    DevBuf<void> ws_uhot;            // [henc] x 8 bytes: u at the hot columns
+    DevBuf<void> ws_uhot;            // [henc + 256] x 8 bytes: u at the hot columns, in the tier layout of the launch (spmv_args.cuh)
     uint32_t henc = 0;               // ids below this are hot ranks
     bool planned = false;            // the plan was attempted (col stays NULL when the gathers are not concentrated)
-    double cover = 0.0;              // share of the entries whose column is among the henc most referenced
+    double cover = 0.0;              // share of the entries whose column is among the HOT_ENC most referenced
 };
 
 // Device CSR panel: rows sorted, columns sorted inside each row.  Owns its arrays and cached plans.
@@ -216,6 +216,8 @@ struct Tunables {
     int spmv_hot_kb = -1;      // B200GRB_SPMV_HOT     -1 default (on when the gathers are concentrated), 0 off, >0 table cap in KB
     bool no_pull = false, no_push = false, force_push = false, spmv_debug = false;
     bool spmv_pipe = false;    // B200GRB_SPMV_PIPE    software-pipeline two runs per warp in the hot-table kernel (4-byte types)
+    int spmv_cluster = 2;      // B200GRB_SPMV_CLUSTER thread-block cluster size of the hot-table kernel (1 / 2 / 4 / 8 / 16)
+    int spmv_hot_repl_kb = 32; // B200GRB_SPMV_HOT_REPL KB of the hot table replicated in every CTA of a cluster (the rest is spread)
     bool spgemm_trace = false; // B200GRB_SPGEMM_TRACE phase times of GrB_mxm (masked) on stderr
     int stream_blk_log2 = 7;   // B200GRB_STREAM_BLK   log2 of the block of a long B row one warp takes (masked SpGEMM)
     int spgemm_v = 0;          // B200GRB_SPGEMM_V     masked SpGEMM kernel generation (0 = default)

@@ -42,6 +42,8 @@ static void tunables_load() {
     t.no_pull = getenv("B200GRB_NO_PULL") != nullptr; t.no_push = getenv("B200GRB_NO_PUSH") != nullptr;
     t.force_push = getenv("B200GRB_FORCE_PUSH") != nullptr; t.spmv_debug = getenv("B200GRB_SPMV_DEBUG") != nullptr;
     t.spmv_pipe = geti("B200GRB_SPMV_PIPE", 0) != 0;
+    t.spmv_cluster = geti("B200GRB_SPMV_CLUSTER", Tunables().spmv_cluster);
+    t.spmv_hot_repl_kb = std::max(0, geti("B200GRB_SPMV_HOT_REPL", Tunables().spmv_hot_repl_kb));
     t.spgemm_trace = getenv("B200GRB_SPGEMM_TRACE") != nullptr;
     t.stream_blk_log2 = std::min(12, std::max(7, geti("B200GRB_STREAM_BLK", 7)));
     t.spgemm_v = geti("B200GRB_SPGEMM_V", 0);

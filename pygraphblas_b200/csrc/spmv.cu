@@ -403,6 +403,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const bool fast_sr = !kflip && spmv_is_fast(xt, zt, add, kmul, false);      // a compile-time specialised semiring
     const bool fast = fast_sr && !sparse_u;
     const Tunables &tn = tunables();
+    std::string hot_note;                    // the burble line names the cluster; it is printed when `burble` is destroyed
     GbBurble burble(fn);
     g_items_fast = (tn.spmv_items == 16 || tn.spmv_items == 4) ? tn.spmv_items : 8;
     const int tile = SPMV_THREADS * (fast ? g_items_fast : g_items_generic);
@@ -470,6 +471,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     bool use_run = run_ok && c.nnz >= 4096;
     if (tn.spmv_run >= 0) use_run = run_ok && c.nnz > 0 && tn.spmv_run != 0;
     const char *kernel_name = "pull";
+    int hot_cluster = 0, hot_ctas = 0; uint32_t hot_t0 = 0, hot_t1 = 0, hot_henc = 0;      // cluster size, grid and tiers of the hot-table launch
     if (use_pull) {
         if (pushed) kernel_name = "push";
     } else if (use_run) {
@@ -491,9 +493,13 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         } else hot_kb = 0;
         Hot2Args hot{};
         if (hot_kb > 0) {
-            // one launch: u at the hot columns, T cleared, T's presence from the plan
-            spmv_hot2_prep(c, uval, tc_size(xt), tval, (size_t)n * zsz, tpres);
-            ra.col = c.hot.col; hot.u_hot = c.hot.ws_uhot; hot.henc = c.hot.henc; hot.tab_n = 0;
+            // the launch runs the prep kernel first: u at the hot columns, T cleared, T's presence from the plan
+            ra.col = c.hot.col;
+            hot.u_hot = c.hot.ws_uhot; hot.hperm = c.hot.perm; hot.henc = c.hot.henc; hot.u = uval; hot.vsize = tc_size(xt);
+            hot.tval = tval; hot.tval_bytes = (size_t)n * zsz; hot.pres_tmpl = rp.pres_tmpl; hot.tpres = tpres; hot.nrows = c.nrows;
+            hot.want_cluster = 1;
+            while (hot.want_cluster < 16 && hot.want_cluster * 2 <= tn.spmv_cluster) hot.want_cluster *= 2;
+            hot.want_repl = (uint32_t)(((size_t)tn.spmv_hot_repl_kb << 10) / tc_size(xt));
             kernel_name = tc_size(xt) <= 4 && tn.spmv_pipe ? "run+hot-table (TMA-staged, pipelined)" : "run+hot-table (TMA-staged)";
         } else {
             CU_TRY(cudaMemsetAsync(tval, 0, (size_t)n * zsz, G.stream), err);
@@ -503,6 +509,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         }
         const bool ok = fast_sr ? spmv_run_dispatch(xt, add, kmul, ra, hot_kb > 0 ? &hot : nullptr, (size_t)hot_kb << 10) : spmv_run_generic(xt, zt, ra);
         if (!ok) return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
+        if (hot_kb > 0) { hot_cluster = hot.cluster; hot_ctas = hot.ctas; hot_t0 = hot.t0; hot_t1 = hot.t1; hot_henc = hot.henc; }
     } else if (c.nnz == 0) {
         clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
         kernel_name = "empty";
@@ -532,7 +539,13 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     }
     gb_kernel_used(kernel_name);
     if (in_place) gb_kernel_used("mxv=in-place");
-    if (burble.on) burble.note(kernel_name, (double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
+    if (hot_cluster > 0) {
+        gb_kernel_used(("hot-cluster=" + std::to_string(hot_cluster)).c_str());
+        gb_kernel_used(("hot-ctas=" + std::to_string(hot_ctas)).c_str());
+        gb_kernel_used(("hot-tiers=" + std::to_string(hot_t0) + "," + std::to_string(hot_t1) + "," + std::to_string(hot_henc)).c_str());
+        if (burble.on) { hot_note = std::string(kernel_name) + " cluster " + std::to_string(hot_cluster) + ", T0 " + std::to_string(hot_t0); kernel_name = hot_note.c_str(); }
+    }
+    if (burble.on) burble.note(kernel_name,(double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
     a_cast.reset(); u_cast.reset();
     vector_mark_used(u); if (mask) vector_mark_used(mask);          // an overlapped import into u may start as soon as these kernels are done
 

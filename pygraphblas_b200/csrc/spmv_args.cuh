@@ -15,11 +15,22 @@ struct RunArgs {
     uint8_t *tpres; uint8_t *head_has; uint8_t *tail_has;      // ... and of everything they produce
 };
 
-// hot-table run kernel (spmv_run.cuh)
+// hot-table run kernel (spmv_run.cuh).  The host fills u_hot .. tpres and the two requests; spmv_run_launch lays out the
+// table tiers, runs the prep kernel and the hot-table kernel, and fills in the layout and the cluster size it used.
+// u_hot layout: [T0 ranks, replicated in every CTA | slice 0 | ... | slice C-1 (S entries each) | ranks T0+T1 .. henc-1]
+// hot rank T0 + k (k < T1) lives in slice k mod C at index k / C, in the shared memory of the cluster's CTA k mod C.
 struct Hot2Args {
-    const void *u_hot;        // [henc] u at the hottest columns (prep kernel)
+    void *u_hot;              // the plan's u_hot buffer (written by the prep kernel)
+    const uint32_t *hperm;    // [henc] column of each hot rank
+    const void *u; int vsize; // u and its value size (prep kernel)
+    void *tval; size_t tval_bytes; const uint8_t *pres_tmpl; uint8_t *tpres; int64_t nrows;   // T cleared, T's presence (prep kernel)
     uint32_t henc;            // ids below this are hot ranks
-    uint32_t tab_n;           // entries of u_hot kept in shared memory (<= henc)
+    int want_cluster;         // requested cluster size C (1, 2, 4, 8, 16)
+    uint32_t want_repl;       // requested replicated tier T0 (entries), used when C > 1
+    // filled in by spmv_run_launch
+    int cluster;              // cluster size launched
+    int ctas;                 // grid of the launch: (clusters the device co-schedules) x C, or fewer when the runs run out
+    uint32_t t0, t1, slice;   // replicated tier, distributed tier (C * slice >= t1), slice entries per CTA
 };
 
 // ------------------------------------------------------------------ masked pull with early exit (BFS-shaped calls)

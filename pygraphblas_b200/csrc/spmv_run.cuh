@@ -2,6 +2,8 @@
 // spmv_run_int.cu (integer / BOOL semirings) and spmv_run_generic.cu (run-time operator codes).
 #pragma once
 #include "spmv_args.cuh"
+#include <map>
+#include <tuple>
 
 // ==================================================================================================
 // Dense-u kernel for the specialised semirings: warp-independent RUNS.
@@ -155,7 +157,7 @@ __global__ void __launch_bounds__(256) spmv_run_kernel(const RunArgs p) {
 // Hot-table run kernel (dense u, specialised semirings, large skewed matrices) -- the benchmarked kernel.
 //
 // One persistent 1024-thread CTA per SM.  Shared memory holds
-//   * the HOT TABLE: u at the tab_n most referenced columns (a scattered 4-byte gather costs one L1 wavefront
+//   * the HOT TABLE: u at the most referenced columns, in the tiers below (a scattered 4-byte gather costs one L1 wavefront
 //     per lane; a shared-memory lookup a few bank-conflict cycles per warp), filled once per CTA by bulk TMA
 //     copies (cp.async.bulk -> SASS UBLKCP) from the gathered copy u_hot that the prep kernel writes;
 //   * one STAGE per warp: the column ids and values of the warp's NEXT run, brought in by two bulk TMA copies
@@ -163,8 +165,16 @@ __global__ void __launch_bounds__(256) spmv_run_kernel(const RunArgs p) {
 //     while the warp gathers and folds run r (registers are the second buffer: a run is copied out of the
 //     stage before the next copy is issued).  A warp is its own producer and consumer: no CTA barrier after
 //     the table is in.
-// Column ids are ENCODED by the cached plan: id < henc -> rank among the hottest columns (table if < tab_n,
-// else u_hot in L2); id >= henc -> original column + henc, gathered from u itself.  u needs no permutation.
+// Column ids are ENCODED by the cached plan: id < henc -> rank among the hottest columns; id >= henc -> original column
+// + henc, gathered from u itself.  u needs no permutation.
+// The kernel runs as thread-block clusters of C CTAs (C = 1: plain CTAs), and the hot ranks fall in tiers:
+//   id < T0        the replicated tier, in every CTA's own table: LDS;
+//   id < T0 + T1   the distributed tier: rank T0 + k sits in the table of the cluster's CTA k mod C (index k / C), read
+//                  through distributed shared memory (mapa + ld.shared::cluster), so a cluster holds C times more of the
+//                  hottest columns on chip than one SM can;
+//   id < henc      u_hot, in L2;   otherwise u itself.
+// Every CTA passes a cluster barrier after its table is in (no peer reads a table before it is complete) and another
+// before it exits (no CTA leaves while a peer may still read its table) -- CTAs without runs included.
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
@@ -181,6 +191,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\t"
                  "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
                  "@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+// a value in the shared memory of CTA `cta` of the cluster, at the address `saddr` has in this CTA's shared memory
+template <typename XT> __device__ __forceinline__ XT ld_dsmem(uint32_t saddr, uint32_t cta) {
+    uint32_t a; asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(saddr), "r"(cta));
+    if constexpr (sizeof(XT) == 8) { unsigned long long v; asm("ld.shared::cluster.b64 %0, [%1];" : "=l"(v) : "r"(a)); return reinterpret_cast<const XT &>(v); }
+    else if constexpr (sizeof(XT) == 4) { uint32_t v; asm("ld.shared::cluster.b32 %0, [%1];" : "=r"(v) : "r"(a)); return reinterpret_cast<const XT &>(v); }
+    else { uint16_t v; asm("ld.shared::cluster.u8 %0, [%1];" : "=h"(v) : "r"(a)); return (XT)(uint8_t)v; }
 }
 
 template <typename XT> __host__ __device__ constexpr int hot2_stage_bytes(bool need_a) { return RUN * 4 + (need_a ? RUN * (int)sizeof(XT) : 0); }
@@ -212,26 +234,34 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         if (NEED_A) tma_bulk_g2s(stage + RUN * 4, static_cast<const XT *>(p.aval) + q, ab, bar);
     };
 
+    const uint32_t t0 = h.t0, t1 = h.t1, slice = h.slice, henc = h.henc;
+    const int lc = __ffs(h.cluster) - 1;                                   // C is a power of two
     if (lane == 0) mbar_init(bar, 1);
     if (threadIdx.x == 0) mbar_init(s_bar + HOT2_WARPS, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
-    if (threadIdx.x == 0 && h.tab_n) {        // the table: bulk copies of <= 16 KB
-        const uint32_t total = h.tab_n * (uint32_t)sizeof(XT);
-        mbar_expect_tx(s_bar + HOT2_WARPS, total);
-        for (uint32_t off = 0; off < total; off += 16384u)
-            tma_bulk_g2s(reinterpret_cast<unsigned char *>(s_hot) + off, static_cast<const unsigned char *>(h.u_hot) + off,
-                         min(16384u, total - off), s_bar + HOT2_WARPS);
+    const uint32_t tab_n = t0 + slice;
+    if (threadIdx.x == 0 && tab_n) {          // the table: the replicated tier and this CTA's slice, bulk copies of <= 16 KB
+        const unsigned char *src = static_cast<const unsigned char *>(h.u_hot);
+        unsigned char *dst = reinterpret_cast<unsigned char *>(s_hot);
+        const uint32_t rb = t0 * (uint32_t)sizeof(XT), sb = slice * (uint32_t)sizeof(XT);
+        mbar_expect_tx(s_bar + HOT2_WARPS, rb + sb);
+        for (uint32_t off = 0; off < rb; off += 16384u) tma_bulk_g2s(dst + off, src + off, min(16384u, rb - off), s_bar + HOT2_WARPS);
+        src += rb + (size_t)cluster_ctarank() * sb; dst += rb;
+        for (uint32_t off = 0; off < sb; off += 16384u) tma_bulk_g2s(dst + off, src + off, min(16384u, sb - off), s_bar + HOT2_WARPS);
     }
     if (lane == 0 && run < p.nruns) issue(run);
-    if (h.tab_n) mbar_wait(s_bar + HOT2_WARPS, 0);
+    if (tab_n) mbar_wait(s_bar + HOT2_WARPS, 0);
+    cluster_sync_all();                       // every table of the cluster is in
 
     const XT *uval = static_cast<const XT *>(p.uval);
-    const XT *uhot = static_cast<const XT *>(h.u_hot);
-    const uint32_t tab_n = h.tab_n, henc = h.henc;
+    const XT *urest = static_cast<const XT *>(h.u_hot) + ((slice << lc) - t1);   // ranks past the tiers (spmv_args.cuh)
+    const uint32_t s_slice = smem_u32(s_hot + t0);
     auto gather = [=](uint32_t col) -> XT {
-        if (col < tab_n) return s_hot[col];
-        if (col < henc) return gload<XT>(uhot + col);
+        if (col < t0) return s_hot[col];
+        const uint32_t k = col - t0;
+        if (k < t1) return ld_dsmem<XT>(s_slice + (k >> lc) * (uint32_t)sizeof(XT), k & ((1u << lc) - 1u));
+        if (col < henc) return gload<XT>(urest + col);
         return gload<XT>(uval + (col - henc));
     };
     // Software pipeline over the warp's runs: the words of run r+1 are copied out of the stage and its gathers of u
@@ -294,6 +324,7 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
             if (more) { cur = nxt; cur_run = run; run += stride; } else cur_run = -1;
         }
     }
+    cluster_sync_all();                       // no peer reads this CTA's table any more
 }
 
 // rows that continue past their run: tail partial (+) head partials of the following runs, 8 lanes per open row.
@@ -331,28 +362,74 @@ template <typename XT> static inline uint32_t hot2_table_entries(bool need_a, ui
     return (uint32_t)std::min<size_t>(henc, avail / sizeof(XT)) & ~15u;
 }
 
+// tiers of a cluster of C CTAs whose tables hold `cap` entries each (spmv_args.cuh).  Plain CTAs (cluster = 1, the whole
+// table local) when C = 1, when one table already holds every hot rank (cap = henc rounded down to 16 entries), and when
+// the replicated tier takes the whole table: a cluster would then only read peers' tables for ranks it could hold itself,
+// and clusters of 4 or more leave SMs idle (DESIGN.md section 3.1).
+static inline void hot2_tiers(Hot2Args &h, int C, uint32_t cap) {
+    h.cluster = 1; h.t0 = cap; h.t1 = 0; h.slice = 0;
+    if (C == 1 || h.henc - cap < 16) return;                                  // cap <= henc
+    const uint32_t t0 = std::min(h.want_repl & ~15u, cap);
+    const uint32_t need = h.henc - t0;
+    const uint32_t slice = std::min(cap - t0, (uint32_t)((ceil_div((int64_t)need, C) + 15) & ~15ll));
+    if (slice == 0) return;
+    h.cluster = C; h.t0 = t0; h.slice = slice; h.t1 = std::min<uint32_t>(need, slice * (uint32_t)C);
+}
+
+// how many clusters of C CTAs of this kernel the device runs at once (asked once per kernel, C and shared-memory size)
+template <typename Kernel> static int hot2_max_clusters(Kernel kernel, int C, size_t smem) {
+    static std::map<std::tuple<Kernel, int, size_t>, int> known;
+    auto it = known.find({kernel, C, smem});
+    if (it != known.end()) return it->second;
+    if (C > 8) cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)(C * ((G.num_sms + C - 1) / C))); cfg.blockDim = dim3(HOT2_WARPS * 32); cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {(unsigned)C, 1, 1};
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+    known[{kernel, C, smem}] = n;
+    return n;
+}
+
+template <typename XT, typename ZT, int ADD, int MUL, bool PIPE>
+static void hot2_launch(const RunArgs &a, Hot2Args &h, size_t table_limit) {
+    constexpr bool NEED_A = mul_reads_x(MUL);
+    auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL, PIPE>;
+    const uint32_t cap = hot2_table_entries<XT>(NEED_A, h.henc, table_limit);
+    const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(NEED_A) + (HOT2_WARPS + 1) * 8 + 8;
+    const size_t smem_max = fixed + (size_t)cap * sizeof(XT);
+    // the dynamic shared-memory limit of a kernel is raised once per size (a driver call per launch is host time the
+    // multi-GPU step cannot hide: its kernels take tens of microseconds)
+    static size_t set_for = 0;
+    if (set_for != smem_max) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max); set_for = smem_max; }
+    const int64_t want_ctas = ceil_div(a.nruns, HOT2_WARPS);
+    // the largest cluster size up to the requested one that the device co-schedules, and the tiers it holds
+    int C = 1, clusters = G.num_sms;
+    for (int c = h.want_cluster; c > 1; c >>= 1) {
+        hot2_tiers(h, c, cap);
+        if (h.cluster == 1) break;                                            // nothing to spread: plain CTAs
+        const int m = hot2_max_clusters(kernel, c, fixed + (size_t)(h.t0 + h.slice) * sizeof(XT));
+        if (m > 0) { C = c; clusters = m; break; }
+    }
+    if (C == 1) hot2_tiers(h, 1, cap);
+    const size_t smem = fixed + (size_t)(h.t0 + h.slice) * sizeof(XT);
+    const int64_t ctas = std::min<int64_t>((int64_t)clusters * C, ceil_div(want_ctas, C) * C);
+    h.ctas = (int)ctas;
+    spmv_hot2_prep(h);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(HOT2_WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = G.stream;
+    cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {(unsigned)C, 1, 1};
+    cfg.attrs = at; cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, a, (const Hot2Args)h); GB_LAUNCHED();
+}
+
 template <typename XT, typename ZT, int ADD, int MUL>
-static void spmv_run_launch(const RunArgs &a, const Hot2Args *hot, size_t table_limit) {
+static void spmv_run_launch(const RunArgs &a, Hot2Args *hot, size_t table_limit) {
     if constexpr (ADD >= 0) {
         if (hot && !a.upres) {
-            constexpr bool NEED_A = mul_reads_x(MUL);
-            Hot2Args h = *hot;
-            h.tab_n = hot2_table_entries<XT>(NEED_A, h.henc, table_limit);
-            const size_t smem = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(NEED_A) + (HOT2_WARPS + 1) * 8 + 8 + (size_t)h.tab_n * sizeof(XT);
-            const int ctas = (int)std::min<int64_t>(G.num_sms, ceil_div(a.nruns, HOT2_WARPS));
-            // the dynamic shared-memory limit of a kernel is raised once per size (a driver call per launch is host time the
-            // multi-GPU step cannot hide: its kernels take tens of microseconds)
-            if (sizeof(XT) <= 4 && tunables().spmv_pipe) {
-                auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL, true>;
-                static size_t set_for = 0;
-                if (set_for != smem) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); set_for = smem; }
-                kernel<<<ctas, HOT2_WARPS * 32, smem, G.stream>>>(a, h); GB_LAUNCHED();
-            } else {
-                auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL, false>;
-                static size_t set_for = 0;
-                if (set_for != smem) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); set_for = smem; }
-                kernel<<<ctas, HOT2_WARPS * 32, smem, G.stream>>>(a, h); GB_LAUNCHED();
-            }
+            if (sizeof(XT) <= 4 && tunables().spmv_pipe) hot2_launch<XT, ZT, ADD, MUL, true>(a, *hot, table_limit);
+            else hot2_launch<XT, ZT, ADD, MUL, false>(a, *hot, table_limit);
             spmv_run_fixup_kernel<ZT, ADD, false><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
             return;
         }

@@ -19,7 +19,8 @@ stream = torch.cuda.ExternalStream(int(gb.ffi.cast("uintptr_t", sp_[0])))
 
 def run(label, sr, env):
     keep_run = os.environ.get("B200GRB_SPMV_RUN")
-    for k in ("B200GRB_SPMV_ITEMS", "B200GRB_SPMV_HOT", "B200GRB_HOT_GROUPS", "B200GRB_SPMV_DEBUG", "B200GRB_SPMV_RUN", "B200GRB_SPMV_PIPE"):
+    for k in ("B200GRB_SPMV_ITEMS", "B200GRB_SPMV_HOT", "B200GRB_HOT_GROUPS", "B200GRB_SPMV_DEBUG", "B200GRB_SPMV_RUN", "B200GRB_SPMV_PIPE",
+              "B200GRB_SPMV_CLUSTER", "B200GRB_SPMV_HOT_REPL"):
         os.environ.pop(k, None)
     if keep_run is not None and "B200GRB_SPMV_RUN" not in env:
         os.environ["B200GRB_SPMV_RUN"] = keep_run
@@ -36,6 +37,28 @@ def run(label, sr, env):
     gb.lib.B200_device_synchronize(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 30
     print(f"{label:44s} {ms*1e3:8.1f} us", flush=True)
+    return ms * 1e3
+
+if len(sys.argv) > 2 and sys.argv[2] == "cluster":
+    # hot-table kernel as clusters of C CTAs (C x T0 replicated KB x PIPE), three repetitions each; the route names the C launched
+    rows = {}
+    for rep in range(3):
+        for C in (1, 2, 4, 8, 16):
+            for t0kb in ((0, 32, 64, 96) if C > 1 else (128,)):
+                for pipe in ("0", "1"):
+                    us = run(f"rep {rep} C={C:2d} T0={t0kb:3d}KB pipe={pipe}", FP32.PLUS_TIMES,
+                             {"B200GRB_SPMV_CLUSTER": str(C), "B200GRB_SPMV_HOT_REPL": str(t0kb), "B200GRB_SPMV_PIPE": pipe})
+                    tok = dict(t.split("=", 1) for t in gb.ffi.string(gb.lib.B200_debug_last_kernel()).decode().split(";") if "=" in t)
+                    rows.setdefault((C, t0kb, pipe), []).append((us, tok.get("hot-cluster", "-"), tok.get("hot-ctas", "-")))
+    # launched C and the clusters of its grid.  The grid is min(cudaOccupancyMaxActiveClusters, clusters the runs fill) x C;
+    # the bench graph fills far more, so on it the launched clusters are the device's co-scheduling limit
+    print(" C T0KB pipe  launched  grid_ctas  clusters_launched   min_us   max_us  mean_us")
+    for (C, t0kb, pipe), v in sorted(rows.items()):
+        us = [x for x, _, _ in v]
+        lc, ctas = v[0][1], v[0][2]
+        ncl = int(ctas) // int(lc) if lc != "-" else "-"
+        print(f"{C:2d} {t0kb:4d} {pipe:>4s}  {lc:>8s}  {ctas:>9s}  {ncl!s:>17s}  {min(us):7.1f}  {max(us):7.1f}  {sum(us)/len(us):7.1f}", flush=True)
+    sys.exit(0)
 
 if len(sys.argv) > 2 and sys.argv[2] == "sweep":
     for rep in range(3):

@@ -225,7 +225,7 @@ uint64_t B200_kernel_launches(void);
 void B200_debug_fail_alloc(int64_t k);
 int64_t B200_debug_live_allocs(void);
 /* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("tile (specialised, 8 items)",
- * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "hash-medium", "spa", "masked-warp", "stream-L",
+ * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-L",
  * "dot", ...); recorded whether the burble is on or not, valid until the next such call.  Host-decided variants follow
  * their entry as "key=value" tokens: "filter=exact" or "filter=bloom" after each "stream-S" / "stream-M" / "stream-L"
  * (the mask-row membership filter is an exact bitmap or a one-hash Bloom filter), and "mxv=in-place" after an mxv / vxm

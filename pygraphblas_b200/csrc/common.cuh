@@ -11,6 +11,7 @@
 #include <math.h>
 #include <float.h>
 #include <limits.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 #include <mutex>
@@ -91,7 +92,6 @@ public:
 struct TilePlan {
     DevBuf<uint32_t> row;            // [ntiles+1]
     int64_t ntiles = 0;
-    int size = 0;
 };
 // run plan (spmv_run.cu, warp-independent kernels): entries cut into warp-sized runs of 256
 struct RunPlan {
@@ -211,17 +211,13 @@ static inline void gb_thread_enter() {
 // kernel-choice switches read from the environment ONCE (GrB_init) and again only on B200_reload_tunables()
 // (tests flip them between calls); nothing on a call path touches getenv
 struct Tunables {
-    int spmv_items = 8;        // B200GRB_SPMV_ITEMS   entries per thread of the tile kernel (4 / 8 / 16)
     int spmv_run = -1;         // B200GRB_SPMV_RUN     -1 default choice, 0 never, 1 always the run kernel
     int spmv_hot_kb = -1;      // B200GRB_SPMV_HOT     -1 default (on when the gathers are concentrated), 0 off, >0 table cap in KB
-    bool no_pull = false, no_push = false, force_push = false, spmv_debug = false;
-    bool spmv_pipe = false;    // B200GRB_SPMV_PIPE    software-pipeline two runs per warp in the hot-table kernel (4-byte types)
+    bool no_pull = false, no_push = false, force_push = false;
     int spmv_cluster = 2;      // B200GRB_SPMV_CLUSTER thread-block cluster size of the hot-table kernel (1 / 2 / 4 / 8 / 16)
     int spmv_hot_repl_kb = 32; // B200GRB_SPMV_HOT_REPL KB of the hot table replicated in every CTA of a cluster (the rest is spread)
     bool spgemm_trace = false; // B200GRB_SPGEMM_TRACE phase times of GrB_mxm (masked) on stderr
     int stream_blk_log2 = 7;   // B200GRB_STREAM_BLK   log2 of the block of a long B row one warp takes (masked SpGEMM)
-    int spgemm_v = 0;          // B200GRB_SPGEMM_V     masked SpGEMM kernel generation (0 = default)
-    bool spgemm_esc = true;    // B200GRB_SPGEMM_ESC   0: the shared-memory bins of the unmasked numeric pass use the hash kernels instead of expand-sort-compress
     int mxv_inplace = 1;       // B200GRB_MXV_INPLACE  0: mxv / vxm never form T in w's own buffers; 1: when w has no copy in flight;
                                //                      2: always, the compute stream first joins w's last overlapped copies
 };
@@ -693,6 +689,47 @@ __host__ __device__ static inline bool mask_value_true(int mtc, const void *mval
     }
 }
 
+// which operands a multiply reads (compile-time for the specialised semirings)
+__host__ __device__ constexpr bool mul_reads_x(int op) { return !(op == OP_SECOND || op == OP_PAIR); }
+__host__ __device__ constexpr bool mul_reads_y(int op) { return !(op == OP_FIRST || op == OP_PAIR || op == OP_ANY); }
+
+// gather of one value through the read-only path (1-byte types as unsigned char: there is no __ldg of bool)
+template <typename T> __device__ __forceinline__ T gload(const T *p) {
+    if constexpr (sizeof(T) == 1) { const unsigned char v = __ldg(reinterpret_cast<const unsigned char *>(p)); return reinterpret_cast<const T &>(v); }
+    else return __ldg(p);
+}
+
+// The (x, z) domains of the kernels with run-time operator codes: z = x on the 11 types, z = BOOL (comparisons) on the 10
+// others.  Runs the statement BODY with XT_ / ZT_ naming the C++ types of (xt, zt), and sets `matched` to whether the pair
+// is one of them.
+#define GB_DOMAIN_CASE_(TC, X, Z, ...) case TC: { typedef X XT_; typedef Z ZT_; __VA_ARGS__; } break;
+#define GB_FOR_DOMAINS(xt, zt, matched, ...)                                                                                \
+    do {                                                                                                                   \
+        matched = true;                                                                                                    \
+        if ((xt) == (zt)) switch (xt) {                                                                                    \
+            GB_DOMAIN_CASE_(TC_BOOL, bool, bool, __VA_ARGS__)          GB_DOMAIN_CASE_(TC_INT8, int8_t, int8_t, __VA_ARGS__)         \
+            GB_DOMAIN_CASE_(TC_INT16, int16_t, int16_t, __VA_ARGS__)   GB_DOMAIN_CASE_(TC_INT32, int32_t, int32_t, __VA_ARGS__)      \
+            GB_DOMAIN_CASE_(TC_INT64, int64_t, int64_t, __VA_ARGS__)   GB_DOMAIN_CASE_(TC_UINT8, uint8_t, uint8_t, __VA_ARGS__)      \
+            GB_DOMAIN_CASE_(TC_UINT16, uint16_t, uint16_t, __VA_ARGS__) GB_DOMAIN_CASE_(TC_UINT32, uint32_t, uint32_t, __VA_ARGS__)  \
+            GB_DOMAIN_CASE_(TC_UINT64, uint64_t, uint64_t, __VA_ARGS__) GB_DOMAIN_CASE_(TC_FP32, float, float, __VA_ARGS__)          \
+            GB_DOMAIN_CASE_(TC_FP64, double, double, __VA_ARGS__)      default: matched = false;                                    \
+        } else if ((zt) == TC_BOOL) switch (xt) {                                                                          \
+            GB_DOMAIN_CASE_(TC_INT8, int8_t, bool, __VA_ARGS__)        GB_DOMAIN_CASE_(TC_INT16, int16_t, bool, __VA_ARGS__)         \
+            GB_DOMAIN_CASE_(TC_INT32, int32_t, bool, __VA_ARGS__)      GB_DOMAIN_CASE_(TC_INT64, int64_t, bool, __VA_ARGS__)         \
+            GB_DOMAIN_CASE_(TC_UINT8, uint8_t, bool, __VA_ARGS__)      GB_DOMAIN_CASE_(TC_UINT16, uint16_t, bool, __VA_ARGS__)       \
+            GB_DOMAIN_CASE_(TC_UINT32, uint32_t, bool, __VA_ARGS__)    GB_DOMAIN_CASE_(TC_UINT64, uint64_t, bool, __VA_ARGS__)       \
+            GB_DOMAIN_CASE_(TC_FP32, float, bool, __VA_ARGS__)         GB_DOMAIN_CASE_(TC_FP64, double, bool, __VA_ARGS__)           \
+            default: matched = false;                                                                                      \
+        } else matched = false;                                                                                            \
+    } while (0)
+
 // ---------------------------------------------------------------- launch helpers
 __host__ __device__ static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 #define GB_LAUNCHED() (G.launches++)
+// grid of a grid-stride kernel: one CTA per `threads` items, at most `per_sm` CTAs per SM, at least one
+static inline int grid_for(int64_t n, int threads = 256, int per_sm = 16) {
+    const int64_t g = std::min<int64_t>(ceil_div(n, threads), (int64_t)G.num_sms * per_sm);
+    return (int)std::max<int64_t>(1, g);
+}
+// one 8-byte count from the device (synchronises the compute stream)
+GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err);

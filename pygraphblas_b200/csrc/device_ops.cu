@@ -86,8 +86,7 @@ GrB_Info dev_build_rowptr32(Csr &c, std::string *err) {
     DevBuf<uint32_t> rp32;
     GB_TRY(rp32.alloc((size_t)c.nrows + 1, err));
     const int64_t n = c.nrows + 1;
-    const int blocks = (int)std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 8);
-    narrow_rowptr_kernel<<<blocks, 256, 0, G.stream>>>(c.rowptr, rp32, n); GB_LAUNCHED();
+    narrow_rowptr_kernel<<<grid_for(n, 256, 8), 256, 0, G.stream>>>(c.rowptr, rp32, n); GB_LAUNCHED();
     CU_TRY(cudaGetLastError(), err);
     c.rowptr32 = std::move(rp32);
     return GrB_SUCCESS;
@@ -121,10 +120,6 @@ __global__ void permute_kernel(const uint32_t *perm, const uint32_t *rowid, cons
             default: ((uint64_t *)tval)[k] = ((const uint64_t *)val)[p]; break;
         }
     }
-}
-
-static inline int grid_for(int64_t n, int threads = 256) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, threads), (int64_t)G.num_sms * 16));
 }
 
 // T = A' as CSR.  A stable LSD radix sort of the entries by column keeps, inside
@@ -167,6 +162,12 @@ GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int fro
     GB_TRY(out.alloc((size_t)n * tc_size(to_code) + 16, err));
     if (n > 0) { cast_kernel<<<grid_for(n), 256, 0, G.stream>>>(out, to_code, in, from_code, n); GB_LAUNCHED(); }
     CU_TRY(cudaGetLastError(), err);
+    return GrB_SUCCESS;
+}
+
+GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
+    CU_TRY(cudaMemcpyAsync(h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
+    CU_TRY(cudaStreamSynchronize(G.stream), err);
     return GrB_SUCCESS;
 }
 

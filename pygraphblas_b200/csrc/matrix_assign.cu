@@ -19,8 +19,6 @@
 #include <vector>
 #include "../../include/b200grb_compat.h"
 
-static inline int agrid(int64_t n, int threads = 256) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, threads), (int64_t)G.num_sms * 16)); }
-
 GrB_Info index_list(const GrB_Index *I, GrB_Index ni, uint64_t dim, bool *all, std::vector<uint64_t> &out, std::string *err, const char *fn);   // vector_ops.cu
 extern "C" GrB_Info GrB_Matrix_dup(GrB_Matrix *C, const GrB_Matrix A);
 extern "C" GrB_Info GrB_Matrix_free(GrB_Matrix *A);
@@ -39,11 +37,6 @@ template <typename T> static GrB_Info upload(const std::vector<T> &h, DevBuf<T> 
     GB_TRY(d.alloc(h.size(), err));
     if (!h.empty()) CU_TRY(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);          // h is a caller-owned temporary
-    return GrB_SUCCESS;
-}
-static GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
-    CU_TRY(cudaMemcpyAsync(h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
-    CU_TRY(cudaStreamSynchronize(G.stream), err);
     return GrB_SUCCESS;
 }
 
@@ -70,7 +63,7 @@ static GrB_Info region_build(Region &R, const GrB_Index *I, GrB_Index ni, const 
         DevBuf<uint64_t> d; GB_TRY(upload(s, d, err));
         GB_TRY(R.rowflag.alloc((size_t)nrows, err));
         CU_TRY(cudaMemsetAsync(R.rowflag, 0, (size_t)nrows, G.stream), err);
-        if (!s.empty()) { flag_kernel<<<agrid((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.rowflag); GB_LAUNCHED(); }
+        if (!s.empty()) { flag_kernel<<<grid_for((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.rowflag); GB_LAUNCHED(); }
     }
     if (!R.all_cols) {
         std::vector<uint64_t> s(R.J); std::sort(s.begin(), s.end()); s.erase(std::unique(s.begin(), s.end()), s.end());
@@ -80,7 +73,7 @@ static GrB_Info region_build(Region &R, const GrB_Index *I, GrB_Index ni, const 
         DevBuf<uint64_t> d; GB_TRY(upload(s, d, err));
         GB_TRY(R.colflag.alloc((size_t)ncols, err));
         CU_TRY(cudaMemsetAsync(R.colflag, 0, (size_t)ncols, G.stream), err);
-        if (!s.empty()) { flag_kernel<<<agrid((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.colflag); GB_LAUNCHED(); }
+        if (!s.empty()) { flag_kernel<<<grid_for((int64_t)s.size()), 256, 0, G.stream>>>(d, (int64_t)s.size(), R.colflag); GB_LAUNCHED(); }
     }
     return GrB_SUCCESS;
 }
@@ -101,12 +94,12 @@ __global__ void fill_entries_kernel(const int64_t *rowptr, int64_t nrows, const 
 static GrB_Info region_filled(const Region &R, int64_t nrows, int64_t ncols, int tc, Sc x, Csr &T, std::string *err) {
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
     GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
-    fill_count_kernel<<<agrid(nrows + 1), 256, 0, G.stream>>>(R.rowflag, nrows, R.nj_distinct, T.rowptr); GB_LAUNCHED();
+    fill_count_kernel<<<grid_for(nrows + 1), 256, 0, G.stream>>>(R.rowflag, nrows, R.nj_distinct, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     T.nnz = R.ni_distinct * R.nj_distinct;
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(tc) + 16, err));
-    if (T.nnz > 0) { fill_entries_kernel<<<agrid(nrows * 32), 256, 0, G.stream>>>(T.rowptr, nrows, R.jsorted, T.col, T.val, tc, x); GB_LAUNCHED(); }
+    if (T.nnz > 0) { fill_entries_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(T.rowptr, nrows, R.jsorted, T.col, T.val, tc, x); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
@@ -138,13 +131,13 @@ __global__ void outside_fill_kernel(const int64_t *ptr, const uint32_t *col, con
 static GrB_Info csr_outside_region(const Csr &c, size_t vsize, const Region &R, Csr &out, std::string *err) {
     out = Csr(); out.nrows = c.nrows; out.ncols = c.ncols;
     GB_TRY(out.rowptr.alloc((size_t)c.nrows + 1, err));
-    outside_count_kernel<<<agrid(c.nrows + 1), 256, 0, G.stream>>>(c.rowptr, c.col, c.nrows, R.rowflag, R.colflag, out.rowptr); GB_LAUNCHED();
+    outside_count_kernel<<<grid_for(c.nrows + 1), 256, 0, G.stream>>>(c.rowptr, c.col, c.nrows, R.rowflag, R.colflag, out.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(out.rowptr, c.nrows + 1, err));
     GB_TRY(read_i64(out.rowptr + c.nrows, &out.nnz, err));
     GB_TRY(out.col.alloc((size_t)out.nnz, err));
     GB_TRY(out.val.alloc((size_t)out.nnz * vsize + 16, err));
     if (out.nnz > 0) {
-        outside_fill_kernel<<<agrid(c.nrows), 256, 0, G.stream>>>(c.rowptr, c.col, (const uint8_t *)c.val, (int)vsize, c.nrows, R.rowflag, R.colflag,
+        outside_fill_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr, c.col, (const uint8_t *)c.val, (int)vsize, c.nrows, R.rowflag, R.colflag,
                                                                   out.rowptr, out.col, (uint8_t *)out.val); GB_LAUNCHED();
     }
     GB_TRY(dev_build_rowptr32(out, err));
@@ -306,15 +299,15 @@ extern "C" GrB_Info GrB_Matrix_extract(GrB_Matrix C, const GrB_Matrix Mask, cons
     }
     Csr T; T.nrows = (int64_t)tn; T.ncols = (int64_t)tm;
     GB_TRY(T.rowptr.alloc((size_t)tn + 1, err));
-    extract_count_kernel<<<agrid((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), T.rowptr); GB_LAUNCHED();
+    extract_count_kernel<<<grid_for((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)tn + 1, err));
     GB_TRY(read_i64(T.rowptr + tn, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (T.nnz > 0) {
-        extract_fill_kernel<<<agrid((int64_t)tn), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jsv, d_jsq,
+        extract_fill_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jsv, d_jsq,
                                                                     (int64_t)Jv.size(), T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
-        if (need_sort) { rows_insertion_sort_kernel<<<agrid((int64_t)tn), 256, 0, G.stream>>>(T.rowptr, (int64_t)tn, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
+        if (need_sort) { rows_insertion_sort_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(T.rowptr, (int64_t)tn, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
     }
     GB_TRY(dev_build_rowptr32(T, err));
     d_rows.reset(); d_jsv.reset(); d_jsq.reset();
@@ -353,12 +346,12 @@ extern "C" GrB_Info GxB_Matrix_diag(GrB_Matrix C, const GrB_Vector v, int64_t k,
     const size_t vsize = v->type->size;
     Csr T; T.nrows = T.ncols = (int64_t)dim;
     GB_TRY(T.rowptr.alloc((size_t)dim + 1, err));
-    diag_build_kernel<<<agrid((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, T.rowptr); GB_LAUNCHED();
+    diag_build_kernel<<<grid_for((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)dim + 1, err));
     GB_TRY(read_i64(T.rowptr + dim, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
-    if (T.nnz > 0) { diag_fill_kernel<<<agrid((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
+    if (T.nnz > 0) { diag_fill_kernel<<<grid_for((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     DescFlags plain{};
     return matrix_writeback(C, nullptr, nullptr, plain, std::move(T), v->type->code, false, err);
@@ -393,7 +386,7 @@ extern "C" GrB_Info GxB_Vector_diag(GrB_Vector v, const GrB_Matrix A, int64_t k,
     GB_TRY(oval.alloc((size_t)len * vsize + 16, err));
     GB_TRY(opres.alloc((size_t)len, err));
     CU_TRY(cudaMemsetAsync(oval, 0, (size_t)len * vsize, G.stream), err);
-    if (len > 0) { diag_extract_kernel<<<agrid(len), 256, 0, G.stream>>>(A->dev.rowptr, A->dev.col, (const uint8_t *)A->dev.val, (int)vsize, nr, nc, k, len, (uint8_t *)oval, opres); GB_LAUNCHED(); }
+    if (len > 0) { diag_extract_kernel<<<grid_for(len), 256, 0, G.stream>>>(A->dev.rowptr, A->dev.col, (const uint8_t *)A->dev.val, (int)vsize, nr, nc, k, len, (uint8_t *)oval, opres); GB_LAUNCHED(); }
     DescFlags plain{};
     return vector_write(v, nullptr, nullptr, plain, oval, opres, A->type->code, false, nullptr, std::move(oval), std::move(opres));
 }
@@ -445,13 +438,13 @@ extern "C" GrB_Info GrB_Matrix_kronecker_BinaryOp(GrB_Matrix C, const GrB_Matrix
     const int ztc = op->ztype->code;
     Csr T; T.nrows = (int64_t)(am * bm); T.ncols = (int64_t)(an * bn);
     GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    kron_count_kernel<<<agrid(T.nrows + 1), 256, 0, G.stream>>>(a.rowptr, b.rowptr, (int64_t)am, (int64_t)bm, T.rowptr); GB_LAUNCHED();
+    kron_count_kernel<<<grid_for(T.nrows + 1), 256, 0, G.stream>>>(a.rowptr, b.rowptr, (int64_t)am, (int64_t)bm, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(ztc) + 16, err));
     if (T.nnz > 0) {
-        kron_fill_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, a.val, A->type->code, b.rowptr, b.col, b.val, B->type->code, (int64_t)am, (int64_t)bm,
+        kron_fill_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, a.val, A->type->code, b.rowptr, b.col, b.val, B->type->code, (int64_t)am, (int64_t)bm,
                                                               (int64_t)bn, op->opcode, op->xtype->code, op->ytype->code, ztc, T.rowptr, T.col, T.val); GB_LAUNCHED();
     }
     GB_TRY(dev_build_rowptr32(T, err));
@@ -489,8 +482,8 @@ static GrB_Info slice_vector(const Csr &a, GrB_Type type, int along, uint64_t in
     CU_TRY(cudaMemsetAsync(val, 0, (size_t)n * vsize, G.stream), err);
     CU_TRY(cudaMemsetAsync(pres, 0, (size_t)n, G.stream), err);
     if (a.nnz > 0) {
-        if (along == 0) row_to_dense_kernel<<<agrid(4096), 256, 0, G.stream>>>(a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, (int64_t)index, (uint8_t *)val, pres);
-        else col_to_dense_kernel<<<agrid(a.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, a.nrows, (uint32_t)index, (uint8_t *)val, pres);
+        if (along == 0) row_to_dense_kernel<<<grid_for(4096), 256, 0, G.stream>>>(a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, (int64_t)index, (uint8_t *)val, pres);
+        else col_to_dense_kernel<<<grid_for(a.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, a.nrows, (uint32_t)index, (uint8_t *)val, pres);
         GB_LAUNCHED();
     }
     GB_TRY(GrB_Vector_new(out, type, (GrB_Index)n));
@@ -524,19 +517,19 @@ static GrB_Info vector_as_slice_csr(GrB_Vector v, int along, uint64_t index, int
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
     DevBuf<int64_t> pos;
     GB_TRY(pos.alloc((size_t)n + 1, err));
-    vec_flags_kernel<<<agrid(n + 1), 256, 0, G.stream>>>(v->dpres, n, pos); GB_LAUNCHED();
+    vec_flags_kernel<<<grid_for(n + 1), 256, 0, G.stream>>>(v->dpres, n, pos); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(pos, n + 1, err));
     GB_TRY(read_i64(pos + n, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (along == 0) {
         GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
-        row_only_ptr_kernel<<<agrid(nrows + 1), 256, 0, G.stream>>>(nrows, (int64_t)index, T.nnz, T.rowptr); GB_LAUNCHED();
-        if (T.nnz > 0) { vec_to_row_kernel<<<agrid(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, pos, 0, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
+        row_only_ptr_kernel<<<grid_for(nrows + 1), 256, 0, G.stream>>>(nrows, (int64_t)index, T.nnz, T.rowptr); GB_LAUNCHED();
+        if (T.nnz > 0) { vec_to_row_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, pos, 0, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
         pos.reset();
     } else {
         T.rowptr = std::move(pos);       // one entry per present position: the scan IS the row pointer
-        if (T.nnz > 0) { vec_to_col_kernel<<<agrid(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, T.rowptr, (uint32_t)index, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
+        if (T.nnz > 0) { vec_to_col_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, T.rowptr, (uint32_t)index, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
     }
     GB_TRY(dev_build_rowptr32(T, err));
     CU_TRY(cudaGetLastError(), err);
@@ -678,14 +671,14 @@ extern "C" GrB_Info GrB_Matrix_assign(GrB_Matrix C, const GrB_Matrix Mask, const
     }
     Csr T; T.nrows = (int64_t)C->nrows; T.ncols = (int64_t)C->ncols;
     GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    massign_count_kernel<<<agrid(T.nrows + 1), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, j_repeats ? d_jmap.get() : nullptr, T.rowptr); GB_LAUNCHED();
+    massign_count_kernel<<<grid_for(T.nrows + 1), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, j_repeats ? d_jmap.get() : nullptr, T.rowptr); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (T.nnz > 0) {
-        massign_fill_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jmap, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
-        if (need_sort) { rows_insertion_sort_kernel<<<agrid(T.nrows), 256, 0, G.stream>>>(T.rowptr, T.nrows, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
+        massign_fill_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jmap, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
+        if (need_sort) { rows_insertion_sort_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(T.rowptr, T.nrows, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
     }
     GB_TRY(dev_build_rowptr32(T, err));
     d_rowsrc.reset(); d_jmap.reset();

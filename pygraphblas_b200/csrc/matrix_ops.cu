@@ -18,13 +18,6 @@
 #include <vector>
 #include "../../include/b200grb_compat.h"
 
-static inline int wgrid(int64_t rows) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(rows * 32, 256), (int64_t)G.num_sms * 16)); }
-static inline int egrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 16)); }
-static GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
-    CU_TRY(cudaMemcpyAsync(h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
-    CU_TRY(cudaStreamSynchronize(G.stream), err);
-    return GrB_SUCCESS;
-}
 #define GB_MAT_OK(A, fn) do { if (!(A)) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL matrix", fn); \
     if (!gb_valid_matrix(A)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid matrix handle", fn); } while (0)
 #define GB_VEC_OK(v, fn) do { if (!(v)) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL vector", fn); \
@@ -131,13 +124,13 @@ extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const
     GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
     a.o_ptr = T.rowptr;
-    select_kernel<false><<<wgrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    select_kernel<false><<<grid_for(T.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * A->type->size + 16, err));
     a.o_col = T.col; a.o_val = T.val;
-    if (T.nnz > 0) { select_kernel<true><<<wgrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    if (T.nnz > 0) { select_kernel<true><<<grid_for(T.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }
@@ -166,7 +159,7 @@ extern "C" GrB_Info GxB_Vector_select(GrB_Vector w, const GrB_Vector mask, const
     GB_TRY(tval.alloc(bytes + 16, &w->err));
     GB_TRY(tpres.alloc((size_t)u->n, &w->err));
     CU_TRY(cudaMemcpyAsync(tval, u->dval, bytes, cudaMemcpyDeviceToDevice, G.stream), &w->err);
-    vec_select_kernel<<<egrid(a.nrows), 256, 0, G.stream>>>(a, u->dpres, tpres); GB_LAUNCHED();
+    vec_select_kernel<<<grid_for(a.nrows), 256, 0, G.stream>>>(a, u->dpres, tpres); GB_LAUNCHED();
     return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, std::move(tval), std::move(tpres));
 }
 
@@ -194,7 +187,7 @@ static GrB_Info mat_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     Csr T; GB_TRY(new_pattern_like(*src, (size_t)tc_size(ztc), T, err));
     ApplyArgs a{};
     a.nnz = src->nnz; a.aval = src->val; a.atc = A->type->code; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar; a.tval = T.val;
-    if (a.nnz > 0) { mat_apply_kernel<<<egrid(a.nnz), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    if (a.nnz > 0) { mat_apply_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), ztc, false, err);
 }
@@ -286,7 +279,7 @@ static GrB_Info mat_reduce_vector(GrB_Vector w, const GrB_Vector mask, const GrB
     GB_TRY(tval.alloc((size_t)rows * tc_size(a.mtc) + 16, &w->err));
     GB_TRY(tpres.alloc((size_t)rows, &w->err));
     a.tval = tval; a.tpres = tpres;
-    row_reduce_kernel<<<wgrid(a.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    row_reduce_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     return vector_write(w, mask, accum, f, a.tval, a.tpres, a.mtc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Matrix_reduce_Monoid(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Monoid monoid, const GrB_Matrix A, const GrB_Descriptor desc) {
@@ -356,13 +349,13 @@ static GrB_Info mat_ewise(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
     a.o_ptr = T.rowptr;
-    merge_rows_kernel<false><<<egrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    merge_rows_kernel<false><<<grid_for(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(a.ztc) + 16, err));
     a.o_col = T.col; a.o_val = T.val;
-    if (T.nnz > 0) { merge_rows_kernel<true><<<egrid(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    if (T.nnz > 0) { merge_rows_kernel<true><<<grid_for(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), a.ztc, false, err);
 }

@@ -36,19 +36,15 @@ static Tunables g_tun; static bool g_tun_loaded = false;
 static void tunables_load() {
     Tunables t;
     auto geti = [](const char *k, int d) { const char *e = getenv(k); return e ? atoi(e) : d; };
-    t.spmv_items = geti("B200GRB_SPMV_ITEMS", 8);
     t.spmv_run = geti("B200GRB_SPMV_RUN", -1);
     t.spmv_hot_kb = geti("B200GRB_SPMV_HOT", -1);
     t.no_pull = getenv("B200GRB_NO_PULL") != nullptr; t.no_push = getenv("B200GRB_NO_PUSH") != nullptr;
-    t.force_push = getenv("B200GRB_FORCE_PUSH") != nullptr; t.spmv_debug = getenv("B200GRB_SPMV_DEBUG") != nullptr;
-    t.spmv_pipe = geti("B200GRB_SPMV_PIPE", 0) != 0;
+    t.force_push = getenv("B200GRB_FORCE_PUSH") != nullptr;
     t.spmv_cluster = geti("B200GRB_SPMV_CLUSTER", Tunables().spmv_cluster);
     t.spmv_hot_repl_kb = std::max(0, geti("B200GRB_SPMV_HOT_REPL", Tunables().spmv_hot_repl_kb));
     t.spgemm_trace = getenv("B200GRB_SPGEMM_TRACE") != nullptr;
     t.stream_blk_log2 = std::min(12, std::max(7, geti("B200GRB_STREAM_BLK", 7)));
-    t.spgemm_v = geti("B200GRB_SPGEMM_V", 0);
     t.mxv_inplace = geti("B200GRB_MXV_INPLACE", 1);
-    t.spgemm_esc = geti("B200GRB_SPGEMM_ESC", 1) != 0;
     g_tun = t; g_tun_loaded = true;
 }
 const Tunables &tunables() { if (!g_tun_loaded) tunables_load(); return g_tun; }

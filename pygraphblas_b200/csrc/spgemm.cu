@@ -4,9 +4,10 @@
 // (Matrix.mxm, `@`, `@=`, `**`).  Gustavson row-wise formulation, three methods:
 //
 //   unmasked    per-row flop count -> rows binned by flops -> symbolic pass (distinct
-//               columns per row) -> scan -> numeric pass.  Small / medium rows use a hash
-//               table in shared memory (atomicCAS probing), rows beyond the shared-memory
-//               budget a dense accumulator in HBM owned by a persistent CTA.  Rows come out
+//               columns per row) -> scan -> numeric pass.  Small / medium rows count their
+//               columns in a shared-memory hash table (atomicCAS probing) and form their
+//               values by expand-sort-compress in shared memory; rows beyond the shared-memory
+//               budget use a dense accumulator in HBM owned by a persistent CTA.  Rows come out
 //               sorted (in-smem bitonic sort / ordered bitmap sweep).
 //   masked      C<M> = A*B with a non-complemented mask: the mask row M(i,:) is loaded into
 //               the table first, products are accumulated only where they hit it, so both
@@ -22,18 +23,9 @@
 #include <limits>
 #include <type_traits>
 
-static inline int grid_for(int64_t n, int threads = 256) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, threads), (int64_t)G.num_sms * 16));
-}
-
 static constexpr uint32_t EMPTY_KEY = 0xFFFFFFFFu;
 
 // ------------------------------------------------------------------ device helpers
-template <typename T> __device__ __forceinline__ T gload(const T *p) {
-    if constexpr (sizeof(T) == 1) { const unsigned char v = __ldg(reinterpret_cast<const unsigned char *>(p)); return reinterpret_cast<const T &>(v); }
-    else return __ldg(p);
-}
-
 // storage word of an accumulator slot: 32-bit for types up to 4 bytes, 64-bit otherwise
 template <typename ZT> struct SlotWord { typedef typename std::conditional<sizeof(ZT) == 8, unsigned long long, unsigned int>::type W; };
 template <typename ZT> __host__ __device__ __forceinline__ typename SlotWord<ZT>::W pack_slot(ZT v) {
@@ -139,7 +131,7 @@ __global__ void flops_kernel(const uint32_t *a_ptr, const uint32_t *a_col, const
     if (lane == 0 && mine) atomicAdd(total, mine);
 }
 
-// bins: 0 = nothing to do, 1 = warp/smem hash, 2 = CTA/smem hash, 3 = dense accumulator
+// bins: 0 = nothing to do, 1 = warp per row (shared memory), 2 = CTA per row (shared memory), 3 = dense accumulator
 struct BinLimits { int64_t small_max, medium_max; };
 __global__ void bin_count_kernel(const int64_t *work, int64_t nrows, BinLimits lim, unsigned int *counts) {
     for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
@@ -176,8 +168,8 @@ template <bool WARP> __device__ void bitonic_sort_u64(unsigned long long *a, int
     }
 }
 
-// ------------------------------------------------------------------ unmasked: shared-memory hash
-// One row per group (a warp, or the whole CTA).  Symbolic: count distinct columns.
+// ------------------------------------------------------------------ unmasked, symbolic pass: shared-memory hash
+// One row per group (a warp, or the whole CTA): count its distinct columns.
 template <bool WARP>
 __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
     extern __shared__ unsigned char smem_raw[];
@@ -235,77 +227,6 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
     if (active && tid == 0) p.c_cnt[p.rows[idx]] = s_count[gid];
 }
 
-// Numeric: packed[s] = (column << 32 | slot), vals[s] = accumulator.  After the products are in,
-// the packed array is bitonic-sorted (empty keys sort last) and the first nnz entries written out.
-template <typename XT, typename ZT, int ADD, int MUL, bool WARP>
-__global__ void __launch_bounds__(256) hash_numeric_kernel(const GemmArgs p) {
-    typedef typename SlotWord<ZT>::W W;
-    extern __shared__ unsigned char smem_raw[];
-    const int add = ADD >= 0 ? ADD : p.add_op;
-    const int mul = MUL >= 0 ? MUL : p.mul_op;
-    const int gsize = WARP ? 32 : blockDim.x;
-    const int gid = WARP ? (threadIdx.x >> 5) : 0;
-    const int tid = WARP ? (threadIdx.x & 31) : threadIdx.x;
-    const int groups = WARP ? (blockDim.x >> 5) : 1;
-    unsigned long long *packed = reinterpret_cast<unsigned long long *>(smem_raw) + (size_t)gid * p.table;
-    W *vals = reinterpret_cast<W *>(smem_raw + (size_t)groups * p.table * 8) + (size_t)gid * p.table;
-    const int64_t idx = (int64_t)blockIdx.x * groups + gid;
-    const bool active = idx < p.nbin;
-    const uint32_t tmask = (uint32_t)p.table - 1;
-    const int hshift = __clz(p.table) + 1;                            // 32 - log2(table)
-    const W ident = pack_slot<ZT>(accum_init<ZT>(add));
-    for (int s = tid; s < p.table; s += gsize) { packed[s] = ((unsigned long long)EMPTY_KEY << 32) | (unsigned)s; vals[s] = ident; }
-    group_sync<WARP>();
-    const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
-    int64_t row = 0;
-    if (active) {
-        row = p.rows[idx];
-        const uint32_t as = p.a_ptr[row], ae = p.a_ptr[row + 1];
-        auto insert = [&](uint32_t j, ZT prod) {
-            uint32_t s = hash_col(j, hshift);
-            while (true) {
-                uint32_t *kp = reinterpret_cast<uint32_t *>(&packed[s]) + 1;   // high word = key
-                const uint32_t seen = atomicCAS(kp, EMPTY_KEY, j);
-                if (seen == EMPTY_KEY || seen == j) break;
-                s = (s + 1) & tmask;
-            }
-            atomic_combine<ZT>(&vals[s], prod, add);
-        };
-        if (WARP) {
-            for (uint32_t pa = as + tid; pa < ae; pa += 32) {
-                const uint32_t k = p.a_col[pa];
-                const XT av = p.need_a ? gload<XT>(aval + pa) : (XT)1;
-                for (uint32_t pb = p.b_ptr[k]; pb < p.b_ptr[k + 1]; ++pb) {
-                    const XT bv = p.need_b ? gload<XT>(bval + pb) : (XT)1;
-                    insert(__ldg(p.b_col + pb), MulApply<XT, ZT>::f(mul, av, bv));
-                }
-            }
-        } else {
-            const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-            for (uint32_t pa = as + warp; pa < ae; pa += nwarps) {
-                const uint32_t k = p.a_col[pa];
-                const XT av = p.need_a ? gload<XT>(aval + pa) : (XT)1;
-                for (uint32_t pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
-                    const XT bv = p.need_b ? gload<XT>(bval + pb) : (XT)1;
-                    insert(__ldg(p.b_col + pb), MulApply<XT, ZT>::f(mul, av, bv));
-                }
-            }
-        }
-    }
-    group_sync<WARP>();
-    bitonic_sort_u64<WARP>(packed, p.table, tid, gsize);
-    if (active) {
-        const int64_t base = p.c_ptr[row];
-        const int n = (int)(p.c_ptr[row + 1] - base);
-        ZT *cval = static_cast<ZT *>(p.c_val);
-        for (int k = tid; k < n; k += gsize) {
-            const unsigned long long e = packed[k];
-            p.c_col[base + k] = (uint32_t)(e >> 32);
-            cval[base + k] = unpack_slot<ZT>(vals[(uint32_t)e]);
-        }
-    }
-}
-
 // ------------------------------------------------------------------ unmasked: dense accumulator in HBM
 // Persistent CTAs pull rows from a queue; each owns a bitmap (+ value array) over all columns.
 // The ordered sweep of the bitmap yields the row already sorted.
@@ -329,13 +250,12 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int *s_warp, int *tot
 }
 
 // ------------------------------------------------------------------ unmasked, numeric pass: expand - sort - compress (ESC)
-// The numeric pass of the two shared-memory bins without a hash table.  The products of a row are EXPANDED into shared memory in
-// their Gustavson order (key = column << 32 | position, the value stays at its position), the keys are SORTED by a bitonic
-// network over the next power of two of the row's OWN product count (the hash path sorts its whole table -- 256 or 4096 slots --
-// whatever the row holds), and equal columns are COMPRESSED by folding their values in position order.  No atomics and no table
-// to clear; a floating-point PLUS monoid gives the same bit pattern on every run (the hash path adds in arrival order).  One
-// warp per row of the small bin (<= 128 products), one CTA per row of the medium bin (<= 2048).  The row's output count comes
-// from the symbolic pass (c_ptr), as for the hash kernels.
+// The numeric pass of the two shared-memory bins.  The products of a row are EXPANDED into shared memory in their Gustavson order
+// (key = column << 32 | position, the value stays at its position), the keys are SORTED by a bitonic network over the next
+// power of two of the row's own product count, and equal columns are COMPRESSED by folding their values in position order.  No
+// atomics and no table to clear; a floating-point PLUS monoid gives the same bit pattern on every run.  One warp per row of the
+// small bin (<= 128 products), one CTA per row of the medium bin (<= 2048).  The row's output count comes from the symbolic
+// pass (c_ptr).
 static constexpr int ESC_SMALL = 128, ESC_MEDIUM = 2048;
 static constexpr size_t ESC_SMEM_SMALL = (size_t)8 * ESC_SMALL * 16;                       // 8 warps x (keys 8 B + value words 8 B)
 static constexpr size_t ESC_SMEM_MEDIUM = (size_t)ESC_MEDIUM * 16 + 3 * 256 * 4 + 256 * 8;   // + offsets, starts, lengths, A values of a chunk
@@ -794,15 +714,6 @@ static GrB_Info read_counts(const unsigned int *d, unsigned int *h, int n, std::
     CU_TRY(cudaStreamSynchronize(G.stream), err);
     return GrB_SUCCESS;
 }
-static GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
-    CU_TRY(cudaMemcpyAsync(h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
-    CU_TRY(cudaStreamSynchronize(G.stream), err);
-    return GrB_SUCCESS;
-}
-
-static bool op_uses_x(int op) { return !(op == OP_SECOND || op == OP_PAIR); }
-static bool op_uses_y(int op) { return !(op == OP_FIRST || op == OP_PAIR || op == OP_ANY); }
-
 static constexpr int SMALL_TABLE = 256, SMALL_FLOPS = 128;      // warp per row
 static constexpr int MEDIUM_TABLE = 4096, MEDIUM_FLOPS = 2048;  // CTA per row
 static constexpr int MIDSMALL_TABLE = 1024;                       // masked: CTA per chunk, mask rows up to 512 entries
@@ -819,31 +730,8 @@ static constexpr int MIDSMALL_TABLE = 1024;                       // masked: CTA
             else if (xt == TC_INT64 && add == OP_PLUS && mul == OP_TIMES) { KERNEL(int64_t, int64_t, OP_PLUS, OP_TIMES); done_ = true; } \
             else if (xt == TC_UINT32 && add == OP_PLUS && mul == OP_PAIR) { KERNEL(uint32_t, uint32_t, OP_PLUS, OP_PAIR); done_ = true; } \
             else if (xt == TC_BOOL && add == OP_LOR && mul == OP_LAND) { KERNEL(bool, bool, OP_LOR, OP_LAND); done_ = true; } \
-            else switch (xt) {                                                                                 \
-                case TC_BOOL: KERNEL(bool, bool, -1, -1); done_ = true; break;                                 \
-                case TC_INT8: KERNEL(int8_t, int8_t, -1, -1); done_ = true; break;                             \
-                case TC_INT16: KERNEL(int16_t, int16_t, -1, -1); done_ = true; break;                          \
-                case TC_INT32: KERNEL(int32_t, int32_t, -1, -1); done_ = true; break;                          \
-                case TC_INT64: KERNEL(int64_t, int64_t, -1, -1); done_ = true; break;                          \
-                case TC_UINT8: KERNEL(uint8_t, uint8_t, -1, -1); done_ = true; break;                          \
-                case TC_UINT16: KERNEL(uint16_t, uint16_t, -1, -1); done_ = true; break;                       \
-                case TC_UINT32: KERNEL(uint32_t, uint32_t, -1, -1); done_ = true; break;                       \
-                case TC_UINT64: KERNEL(uint64_t, uint64_t, -1, -1); done_ = true; break;                       \
-                case TC_FP32: KERNEL(float, float, -1, -1); done_ = true; break;                               \
-                case TC_FP64: KERNEL(double, double, -1, -1); done_ = true; break;                             \
-            }                                                                                                  \
-        } else if (zt == TC_BOOL) switch (xt) {                                                                \
-            case TC_INT8: KERNEL(int8_t, bool, -1, -1); done_ = true; break;                                   \
-            case TC_INT16: KERNEL(int16_t, bool, -1, -1); done_ = true; break;                                 \
-            case TC_INT32: KERNEL(int32_t, bool, -1, -1); done_ = true; break;                                 \
-            case TC_INT64: KERNEL(int64_t, bool, -1, -1); done_ = true; break;                                 \
-            case TC_UINT8: KERNEL(uint8_t, bool, -1, -1); done_ = true; break;                                 \
-            case TC_UINT16: KERNEL(uint16_t, bool, -1, -1); done_ = true; break;                               \
-            case TC_UINT32: KERNEL(uint32_t, bool, -1, -1); done_ = true; break;                               \
-            case TC_UINT64: KERNEL(uint64_t, bool, -1, -1); done_ = true; break;                               \
-            case TC_FP32: KERNEL(float, bool, -1, -1); done_ = true; break;                                    \
-            case TC_FP64: KERNEL(double, bool, -1, -1); done_ = true; break;                                   \
         }                                                                                                      \
+        if (!done_) GB_FOR_DOMAINS(xt, zt, done_, KERNEL(XT_, ZT_, -1, -1));                                   \
         if (!done_) return gb_fail(GrB_DOMAIN_MISMATCH, err, "mxm: unsupported semiring domains (x=%d, z=%d)", xt, zt); \
     } while (0)
 
@@ -864,7 +752,6 @@ static GrB_Info make_bins(const int64_t *work, int64_t nrows, BinLimits lim, Row
     return GrB_SUCCESS;
 }
 
-static size_t numeric_smem(int table, int groups, size_t wsize) { return (size_t)groups * table * (8 + wsize); }
 static size_t masked_smem(int table, int groups, size_t wsize) {
     const size_t per = (size_t)table * 8 + (size_t)(table / 2) * wsize + (size_t)(table / 2);
     return (size_t)groups * ((per + 15) & ~(size_t)15);
@@ -921,25 +808,16 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     GB_TRY(T.col.alloc((size_t)nnz, err));
     GB_TRY(T.val.alloc((size_t)nnz * tc_size(zt) + 16, err));
     g.c_ptr = T.rowptr; g.c_col = T.col; g.c_val = T.val;
-    // ---- numeric (shared-memory bins: expand-sort-compress unless B200GRB_SPGEMM_ESC=0 selects the hash kernels)
-    const bool esc = tunables().spgemm_esc;
+    // ---- numeric (shared-memory bins: expand-sort-compress)
     if (bins.count[1]) {
-        g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1]; g.table = SMALL_TABLE;
-        const size_t sm = numeric_smem(SMALL_TABLE, 8, wsize);
-#define K_SMALL(XT, ZT, A_, M_) hash_numeric_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(g.nbin, 8), 256, sm, G.stream>>>(g)
+        g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1];
 #define K_ESC_SMALL(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
-        if (esc) GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); else GB_FOR_SEMIRING(xt, zt, add, mul, K_SMALL, err);
-        GB_LAUNCHED(); gb_kernel_used(esc ? "esc-small" : "hash-small");
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); GB_LAUNCHED(); gb_kernel_used("esc-small");
     }
     if (bins.count[2]) {
-        g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
-        const size_t sm = numeric_smem(MEDIUM_TABLE, 1, wsize);
-#define K_MEDIUM(XT, ZT, A_, M_) do { \
-        cudaFuncSetAttribute(hash_numeric_kernel<XT, ZT, A_, M_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); \
-        hash_numeric_kernel<XT, ZT, A_, M_, false><<<(unsigned)g.nbin, 256, sm, G.stream>>>(g); } while (0)
+        g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2];
 #define K_ESC_MEDIUM(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, false><<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
-        if (esc) GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); else GB_FOR_SEMIRING(xt, zt, add, mul, K_MEDIUM, err);
-        GB_LAUNCHED(); gb_kernel_used(esc ? "esc-medium" : "hash-medium");
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); GB_LAUNCHED(); gb_kernel_used("esc-medium");
     }
     if (bins.count[3]) {
         g.rows = bins.rows + bins.offset[3]; g.nbin = bins.count[3]; g.queue = queue + 1;
@@ -1198,7 +1076,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
                        (unsigned long long)C->nrows, (unsigned long long)C->ncols);
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "GrB_mxm: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
     const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
-    const bool need_a = op_uses_x(mul), need_b = op_uses_y(mul);
+    const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
     GbBurble burble("GrB_mxm");
     G.last_kernel.clear();
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed

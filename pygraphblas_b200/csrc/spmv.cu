@@ -13,7 +13,7 @@
 //   nnz >= 4096                 -> run kernel (spmv_run*.cu): 256-entry runs per warp on a cached run plan,
 //                                  compile-time semirings (+ shared-memory hot-column table), run-time
 //                                  operator codes, dense or sparse u
-//   otherwise                   -> tile kernel below: the nnz range is cut into tiles of SPMV_THREADS * items
+//   otherwise                   -> tile kernel below: the nnz range is cut into tiles of SPMV_TILE = 2048
 //                                  entries, one CTA per tile, item-centric segmented reduction; rows that straddle
 //                                  tiles leave head / tail partials that a fix-up kernel combines in a fixed order.
 // Every path is nnz-split (R-MAT hub rows cannot serialise a warp) and deterministic for a given matrix.
@@ -22,13 +22,10 @@
 //   + ncols*sizeof(u) + nrows*(sizeof(t) + 1).
 #include "spmv_args.cuh"
 
-// build with -DB200GRB_PHASE_TIMERS=1 and run with B200GRB_SPMV_DEBUG=1 to get per-phase cycle counts of the tile kernel
-#ifndef B200GRB_PHASE_TIMERS
-#define B200GRB_PHASE_TIMERS 0
-#endif
-static constexpr bool SPMV_PHASE_TIMERS = B200GRB_PHASE_TIMERS != 0;
 static constexpr int SPMV_THREADS = 256;
 static constexpr int SPMV_WARPS = SPMV_THREADS / 32;
+static constexpr int SPMV_PER_THREAD = 8;                         // entries per thread of the tile kernel
+static constexpr int SPMV_TILE = SPMV_THREADS * SPMV_PER_THREAD;
 
 struct SpmvArgs {
     const uint32_t *rowptr; const uint32_t *col; const void *aval;
@@ -38,8 +35,7 @@ struct SpmvArgs {
     void *head_val; uint8_t *head_has; void *tail_val; uint8_t *tail_has; int32_t *tail_row;
     int add_op, mul_op;
     int flip;      // 0: z = mul(a, u) (mxv)   1: z = mul(u, a) (vxm)   (run-time-operator kernels only)
-    int tile;      // entries per tile = SPMV_THREADS * items per thread
-    unsigned long long *dbg;   // optional per-phase cycle counters (B200GRB_SPMV_DEBUG), nullptr in production
+    int tile;      // entries per tile (SPMV_TILE)
 };
 
 // ---- plan: tile_row[t] = row holding entry t*tile (tile_row[0] = 0, tile_row[ntiles] = nrows)
@@ -54,15 +50,14 @@ __global__ void spmv_plan_kernel(const uint32_t *rowptr, int64_t nrows, int64_t 
     tile_row[t] = (uint32_t)(lo - 1);
 }
 
-static GrB_Info spmv_plan(Csr &c, int tile, std::string *err) {
-    if (c.tile.row && c.tile.size == tile) return GrB_SUCCESS;
+static GrB_Info spmv_plan(Csr &c, std::string *err) {
+    if (c.tile.row) return GrB_SUCCESS;
     if (!c.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "mxv: matrices with >= 2^32 entries are not supported");
-    c.tile = TilePlan();
     TilePlan p;
-    p.ntiles = ceil_div(c.nnz, tile); p.size = tile;
+    p.ntiles = ceil_div(c.nnz, SPMV_TILE);
     GB_TRY(p.row.alloc((size_t)p.ntiles + 1, err));
     const int64_t n = p.ntiles + 1;
-    spmv_plan_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, G.stream>>>(c.rowptr32, c.nrows, p.ntiles, tile, p.row); GB_LAUNCHED();
+    spmv_plan_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, G.stream>>>(c.rowptr32, c.nrows, p.ntiles, SPMV_TILE, p.row); GB_LAUNCHED();
     CU_TRY(cudaGetLastError(), err);
     c.tile = std::move(p);
     return GrB_SUCCESS;
@@ -100,8 +95,6 @@ __device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32
     const XT *uval = static_cast<const XT *>(p.uval);
     ZT *tval = static_cast<ZT *>(p.tval);
 
-    long long t0 = 0, t1 = 0, t2 = 0, t3 = 0;
-    if (SPMV_PHASE_TIMERS && p.dbg && tid == 0) t0 = clock64();
     const uint32_t r0 = p.tile_row[tile];
     const uint32_t r1 = (uint32_t)min((int64_t)p.tile_row[tile + 1], p.nrows - 1);
     uint32_t pre_rs = 0, pre_re = 0;                                      // row pointers of this thread's first row
@@ -121,7 +114,6 @@ __device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32
         }
     }
     sync();                                                               // head marks are clear
-    if (SPMV_PHASE_TIMERS && p.dbg && tid == 0) t1 = clock64();
 
     // ---- (2) rows of the tile: empty ones are final, the others mark their first entry
     {
@@ -142,7 +134,6 @@ __device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32
         else prod[j] = p.flip ? MulApply<XT, ZT>::f(mul, uu, av) : MulApply<XT, ZT>::f(mul, av, uu);
     }
     sync();                                                               // head marks are complete
-    if (SPMV_PHASE_TIMERS && p.dbg && tid == 0) t2 = clock64();
 
     // ---- (3a) fold this thread's items between row marks
     int32_t h[IT];
@@ -188,7 +179,6 @@ __device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32
     }
     if (lane == 0) { s_wv[warp] = x.v; s_wflag[warp] = x.has | (stop << 1); }
     sync();
-    if (SPMV_PHASE_TIMERS && p.dbg && tid == 0) t3 = clock64();
     Part<ZT> carry{(ZT)0, 0}; int carry_stop = 0;                         // what the following warps add to a row open at this warp's end
     for (int w = SPMV_WARPS - 1; w > warp; --w) {
         Part<ZT> y; y.v = s_wv[w]; const int f = s_wflag[w]; y.has = f & 1;
@@ -207,12 +197,6 @@ __device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32
     }
     if (tid == 0 && h[0] < 0) {                                           // the tile starts inside a row of an earlier tile
         static_cast<ZT *>(p.head_val)[tile] = x.v; p.head_has[tile] = (uint8_t)x.has;
-    }
-    if (SPMV_PHASE_TIMERS && p.dbg && tid == 0) {
-        const long long t4 = clock64();
-        atomicAdd(&p.dbg[0], (unsigned long long)(t1 - t0)); atomicAdd(&p.dbg[1], (unsigned long long)(t2 - t1));
-        atomicAdd(&p.dbg[2], (unsigned long long)(t3 - t2)); atomicAdd(&p.dbg[3], (unsigned long long)(t4 - t3));
-        atomicAdd(&p.dbg[4], 1ull);
     }
 }
 
@@ -279,87 +263,40 @@ __global__ void clear_presence_kernel(uint8_t *p, int64_t n) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) p[k] = 0;
 }
 
-static int g_items_fast = 8, g_items_generic = 8;     // entries per thread (tunable: B200GRB_SPMV_ITEMS)
-
-template <typename XT, typename ZT, int ADD, int MUL, bool SPARSE, int IT>
+template <typename XT, typename ZT, int ADD, int MUL, bool SPARSE>
 static void spmv_launch(const SpmvArgs &a) {
-    spmv_tile_kernel<XT, ZT, ADD, MUL, SPARSE, IT><<<(unsigned)a.ntiles, SPMV_THREADS, 0, G.stream>>>(a); GB_LAUNCHED();
+    spmv_tile_kernel<XT, ZT, ADD, MUL, SPARSE, SPMV_PER_THREAD><<<(unsigned)a.ntiles, SPMV_THREADS, 0, G.stream>>>(a); GB_LAUNCHED();
     spmv_fixup_kernel<ZT, ADD><<<(unsigned)ceil_div(a.ntiles * 32, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
 }
 
-// compile-time specialised semirings (BASELINE.json north_star: PLUS_TIMES, LOR_LAND, MIN_PLUS,
-// PLUS_SECOND; plus PLUS_PAIR / ANY_PAIR / PLUS_FIRST / MIN_FIRST / MIN_SECOND which the reference's
-// demos use) for dense u; everything else runs the same kernel with run-time operator codes.
-template <typename T> static bool spmv_fast(int add, int mul, int items, const SpmvArgs &a) {
-#define GB_FAST(A, M) if (add == A && mul == M) { if (items == 16) spmv_launch<T, T, A, M, false, 16>(a); else if (items == 4) spmv_launch<T, T, A, M, false, 4>(a); else spmv_launch<T, T, A, M, false, 8>(a); return true; }
-    GB_FAST(OP_PLUS, OP_TIMES) GB_FAST(OP_MIN, OP_PLUS) GB_FAST(OP_PLUS, OP_SECOND) GB_FAST(OP_PLUS, OP_FIRST)
-    GB_FAST(OP_PLUS, OP_PAIR) GB_FAST(OP_MIN, OP_FIRST) GB_FAST(OP_MIN, OP_SECOND)
+// compile-time specialised semirings (spmv_common.cuh: BASELINE.json north_star PLUS_TIMES, LOR_LAND, MIN_PLUS, PLUS_SECOND,
+// and the ones the reference's demos use) for dense u; everything else runs the same kernel with run-time operator codes.
+template <typename T> static bool spmv_fast(int add, int mul, const SpmvArgs &a) {
+#define GB_FAST(A, M) if (add == A && mul == M) { spmv_launch<T, T, A, M, false>(a); return true; }
+    GB_SPMV_FAST_PAIRS(T, GB_FAST)
 #undef GB_FAST
     return false;
-}
-static bool spmv_fast_bool(int add, int mul, int items, const SpmvArgs &a) {
-#define GB_FAST(A, M) if (add == A && mul == M) { if (items == 16) spmv_launch<bool, bool, A, M, false, 16>(a); else if (items == 4) spmv_launch<bool, bool, A, M, false, 4>(a); else spmv_launch<bool, bool, A, M, false, 8>(a); return true; }
-    GB_FAST(OP_LOR, OP_LAND) GB_FAST(OP_ANY, OP_PAIR) GB_FAST(OP_LOR, OP_PAIR) GB_FAST(OP_LOR, OP_SECOND) GB_FAST(OP_LOR, OP_FIRST)
-#undef GB_FAST
-    return false;
-}
-
-// the tile size a call will use (so that the plan can be built first)
-static bool spmv_is_fast(int xt, int zt, int add, int mul, bool sparse_u) {
-    if (sparse_u || xt != zt) return false;
-    const bool num = (add == OP_PLUS && (mul == OP_TIMES || mul == OP_SECOND || mul == OP_FIRST || mul == OP_PAIR)) ||
-                     (add == OP_MIN && (mul == OP_PLUS || mul == OP_FIRST || mul == OP_SECOND));
-    const bool boo = (add == OP_LOR && (mul == OP_LAND || mul == OP_PAIR || mul == OP_SECOND || mul == OP_FIRST)) || (add == OP_ANY && mul == OP_PAIR);
-    switch (xt) {
-        case TC_FP32: case TC_FP64: case TC_INT32: case TC_INT64: case TC_UINT32: case TC_UINT64: return num;
-        case TC_BOOL: return boo;
-        default: return false;
-    }
 }
 
 static GrB_Info spmv_dispatch(int xt, int zt, int add, int mul, bool sparse_u, const SpmvArgs &a, std::string *err) {
     if (spmv_is_fast(xt, zt, add, mul, sparse_u)) {
-        const int items = a.tile / SPMV_THREADS;
+        bool ok = false;
         switch (xt) {
-            case TC_FP32:  if (spmv_fast<float>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_FP64:  if (spmv_fast<double>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_INT32: if (spmv_fast<int32_t>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_INT64: if (spmv_fast<int64_t>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_UINT32: if (spmv_fast<uint32_t>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_UINT64: if (spmv_fast<uint64_t>(add, mul, items, a)) return GrB_SUCCESS; break;
-            case TC_BOOL:  if (spmv_fast_bool(add, mul, items, a)) return GrB_SUCCESS; break;
+            case TC_FP32:  ok = spmv_fast<float>(add, mul, a); break;
+            case TC_FP64:  ok = spmv_fast<double>(add, mul, a); break;
+            case TC_INT32: ok = spmv_fast<int32_t>(add, mul, a); break;
+            case TC_INT64: ok = spmv_fast<int64_t>(add, mul, a); break;
+            case TC_UINT32: ok = spmv_fast<uint32_t>(add, mul, a); break;
+            case TC_UINT64: ok = spmv_fast<uint64_t>(add, mul, a); break;
+            case TC_BOOL:  ok = spmv_fast<bool>(add, mul, a); break;
             default: break;
         }
-        return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
+        return ok ? GrB_SUCCESS : gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
     }
-#define GB_GEN2(XT_, ZT_) do { if (sparse_u) spmv_launch<XT_, ZT_, -1, -1, true, 8>(a); else spmv_launch<XT_, ZT_, -1, -1, false, 8>(a); return GrB_SUCCESS; } while (0)
-    if (xt == zt) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_GEN2(T, T);
-            GB_GEN(TC_BOOL, bool) GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    } else if (zt == TC_BOOL) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_GEN2(T, bool);
-            GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    }
-#undef GB_GEN2
-    return gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
+    bool ok;
+    GB_FOR_DOMAINS(xt, zt, ok, if (sparse_u) spmv_launch<XT_, ZT_, -1, -1, true>(a); else spmv_launch<XT_, ZT_, -1, -1, false>(a));
+    return ok ? GrB_SUCCESS : gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
 }
-
-static inline int grid_for(int64_t n, int threads = 256) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, threads), (int64_t)G.num_sms * 16));
-}
-
-static bool op_uses_x(int op) { return !(op == OP_SECOND || op == OP_PAIR); }
-static bool op_uses_y(int op) { return !(op == OP_FIRST || op == OP_PAIR || op == OP_ANY); }
 
 // w<mask> = accum(w, A' (+).(x) u) with `flip` selecting mul(u,a) (vxm) and `use_transpose`
 // selecting the cached CSR of A' (so that the kernel always pulls along CSR rows).
@@ -397,17 +334,15 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     if (flip && (mul == OP_FIRST || mul == OP_SECOND)) { kmul = mul == OP_FIRST ? OP_SECOND : OP_FIRST; kflip = false; }
     if (flip && (mul == OP_TIMES || mul == OP_PLUS || mul == OP_MIN || mul == OP_MAX || mul == OP_PAIR || mul == OP_LAND || mul == OP_LOR ||
                  mul == OP_LXOR || mul == OP_EQ || mul == OP_NE || mul == OP_ISEQ || mul == OP_ISNE)) kflip = false;     // commutative
-    const bool need_a = kflip ? op_uses_y(kmul) : op_uses_x(kmul);
-    const bool need_u = kflip ? op_uses_x(kmul) : op_uses_y(kmul);
+    const bool need_a = kflip ? mul_reads_y(kmul) : mul_reads_x(kmul);
+    const bool need_u = kflip ? mul_reads_x(kmul) : mul_reads_y(kmul);
     const bool sparse_u = u->dpres != nullptr;
     const bool fast_sr = !kflip && spmv_is_fast(xt, zt, add, kmul, false);      // a compile-time specialised semiring
     const bool fast = fast_sr && !sparse_u;
     const Tunables &tn = tunables();
     std::string hot_note;                    // the burble line names the cluster; it is printed when `burble` is destroyed
     GbBurble burble(fn);
-    g_items_fast = (tn.spmv_items == 16 || tn.spmv_items == 4) ? tn.spmv_items : 8;
-    const int tile = SPMV_THREADS * (fast ? g_items_fast : g_items_generic);
-    GB_TRY(spmv_plan(c, tile, err));
+    GB_TRY(spmv_plan(c, err));
 
     DevBuf<void> a_cast, u_cast;
     const void *aval = c.val, *uval = u->dval;
@@ -500,7 +435,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
             hot.want_cluster = 1;
             while (hot.want_cluster < 16 && hot.want_cluster * 2 <= tn.spmv_cluster) hot.want_cluster *= 2;
             hot.want_repl = (uint32_t)(((size_t)tn.spmv_hot_repl_kb << 10) / tc_size(xt));
-            kernel_name = tc_size(xt) <= 4 && tn.spmv_pipe ? "run+hot-table (TMA-staged, pipelined)" : "run+hot-table (TMA-staged)";
+            kernel_name = "run+hot-table (TMA-staged)";
         } else {
             CU_TRY(cudaMemsetAsync(tval, 0, (size_t)n * zsz, G.stream), err);
             if (sparse_u) CU_TRY(cudaMemsetAsync(tpres, 0, (size_t)n, G.stream), err);     // presence follows u: written row by row
@@ -514,28 +449,20 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
         kernel_name = "empty";
     } else {
-        kernel_name = !fast ? "tile (run-time operators)" : g_items_fast == 4 ? "tile (specialised, 4 items)"
-                    : g_items_fast == 16 ? "tile (specialised, 16 items)" : "tile (specialised, 8 items)";
+        kernel_name = fast ? "tile (specialised, 8 items)" : "tile (run-time operators)";
         SpmvArgs a{};
         a.rowptr = c.rowptr32; a.col = c.col; a.aval = aval; a.tile_row = c.tile.row; a.ntiles = c.tile.ntiles;
         a.nrows = c.nrows; a.nnz = c.nnz; a.uval = uval; a.upres = u->dpres; a.tval = tval; a.tpres = tpres;
-        a.add_op = add; a.mul_op = kmul; a.flip = kflip; a.tile = tile;
+        a.add_op = add; a.mul_op = kmul; a.flip = kflip; a.tile = SPMV_TILE;
         const size_t nt = (size_t)c.tile.ntiles;
-        DevBuf<void> head_val, tail_val; DevBuf<uint8_t> head_has, tail_has; DevBuf<int32_t> tail_row; DevBuf<unsigned long long> dbg;
+        DevBuf<void> head_val, tail_val; DevBuf<uint8_t> head_has, tail_has; DevBuf<int32_t> tail_row;
         GB_TRY(head_val.alloc(nt * zsz + 16, err));
         GB_TRY(tail_val.alloc(nt * zsz + 16, err));
         GB_TRY(head_has.alloc(nt, err));
         GB_TRY(tail_has.alloc(nt, err));
         GB_TRY(tail_row.alloc(nt, err));
         a.head_val = head_val; a.tail_val = tail_val; a.head_has = head_has; a.tail_has = tail_has; a.tail_row = tail_row;
-        if (SPMV_PHASE_TIMERS && tn.spmv_debug) { GB_TRY(dbg.alloc(8, err)); a.dbg = dbg; CU_TRY(cudaMemsetAsync(a.dbg, 0, 64, G.stream), err); }
         GB_TRY(spmv_dispatch(xt, zt, add, kmul, sparse_u, a, err));
-        if (a.dbg) {
-            unsigned long long h[5];
-            cudaMemcpyAsync(h, a.dbg, 40, cudaMemcpyDeviceToHost, G.stream); cudaStreamSynchronize(G.stream);
-            if (h[4]) fprintf(stderr, "[spmv phases, avg cycles per tile] load+issue %.0f | rows+gather %.0f | fold+scan %.0f | carry+store %.0f | tiles %llu\n",
-                              (double)h[0] / h[4], (double)h[1] / h[4], (double)h[2] / h[4], (double)h[3] / h[4], h[4]);
-        }
     }
     gb_kernel_used(kernel_name);
     if (in_place) gb_kernel_used("mxv=in-place");

@@ -35,11 +35,6 @@ template <typename T> __device__ __forceinline__ void load4(const T *p, T *out) 
     }
 }
 
-template <typename T> __device__ __forceinline__ T gload(const T *p) {
-    if constexpr (sizeof(T) == 1) { const unsigned char v = __ldg(reinterpret_cast<const unsigned char *>(p)); return reinterpret_cast<const T &>(v); }
-    else return __ldg(p);
-}
-
 template <typename T> __device__ __forceinline__ T shfl_xor_t(T v, int o) {
     if constexpr (sizeof(T) == 8) { long long x = reinterpret_cast<long long &>(v); x = __shfl_xor_sync(0xffffffffu, x, o); return reinterpret_cast<T &>(x); }
     else if constexpr (sizeof(T) == 4) { int x = reinterpret_cast<int &>(v); x = __shfl_xor_sync(0xffffffffu, x, o); return reinterpret_cast<T &>(x); }
@@ -61,16 +56,29 @@ template <typename ZT> __device__ __forceinline__ Part<ZT> part_join(int add, Pa
     return r;
 }
 
-// which operands a multiply reads (compile-time for the specialised semirings)
-__host__ __device__ constexpr bool mul_reads_x(int op) { return !(op == OP_SECOND || op == OP_PAIR); }
-__host__ __device__ constexpr bool mul_reads_y(int op) { return !(op == OP_FIRST || op == OP_PAIR || op == OP_ANY); }
-
 template <typename T> __device__ __forceinline__ T shfl_idx_t(T v, int src) {
     if constexpr (sizeof(T) == 8) { long long x = reinterpret_cast<long long &>(v); x = __shfl_sync(0xffffffffu, x, src); return reinterpret_cast<T &>(x); }
     else if constexpr (sizeof(T) == 4) { int x = reinterpret_cast<int &>(v); x = __shfl_sync(0xffffffffu, x, src); return reinterpret_cast<T &>(x); }
     else { int x = (int)v; x = __shfl_sync(0xffffffffu, x, src); return (T)x; }
 }
-static inline int hgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 32)); }
+
+// ---- the semirings with compile-time kernels (tile and run kernels; dense u, x = z): F(ADD, MUL) for each.  The numeric list
+//      serves FP32, FP64, INT32, INT64, UINT32 and UINT64, the BOOL list BOOL; every other semiring runs with operator codes.
+#define GB_SPMV_FAST_NUM(F) F(OP_PLUS, OP_TIMES) F(OP_MIN, OP_PLUS) F(OP_PLUS, OP_SECOND) F(OP_PLUS, OP_FIRST) \
+                            F(OP_PLUS, OP_PAIR) F(OP_MIN, OP_FIRST) F(OP_MIN, OP_SECOND)
+#define GB_SPMV_FAST_BOOL(F) F(OP_LOR, OP_LAND) F(OP_ANY, OP_PAIR) F(OP_LOR, OP_PAIR) F(OP_LOR, OP_SECOND) F(OP_LOR, OP_FIRST)
+// F(ADD, MUL) for the specialised semirings of value type T (a statement inside a template over T)
+#define GB_SPMV_FAST_PAIRS(T, F) if constexpr (std::is_same<T, bool>::value) { GB_SPMV_FAST_BOOL(F) } else { GB_SPMV_FAST_NUM(F) }
+static inline bool spmv_is_fast(int xt, int zt, int add, int mul, bool sparse_u) {
+    if (sparse_u || xt != zt) return false;
+#define GB_IS(A, M) || (add == A && mul == M)
+    switch (xt) {
+        case TC_FP32: case TC_FP64: case TC_INT32: case TC_INT64: case TC_UINT32: case TC_UINT64: return false GB_SPMV_FAST_NUM(GB_IS);
+        case TC_BOOL: return false GB_SPMV_FAST_BOOL(GB_IS);
+        default: return false;
+    }
+#undef GB_IS
+}
 
 // ---- run kernels (spmv_run.cuh, spmv_run*.cu)
 struct RunArgs;

@@ -141,29 +141,12 @@ __global__ void __launch_bounds__(1024) spmv_pull_long_kernel(const PullArgs p) 
     }
 }
 GrB_Info spmv_masked_pull_dispatch(int xt, int zt, const PullArgs &a, std::string *err) {
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nrows, 256), (int64_t)G.num_sms * 8));
-    const int lgrid = (int)std::max<int64_t>(1, std::min<int64_t>(a.long_cap, (int64_t)G.num_sms * 2));
-#define GB_PULL(XT_, ZT_) do { spmv_masked_pull_kernel<XT_, ZT_><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED(); \
-        if (a.has_long) { spmv_pull_long_kernel<XT_, ZT_><<<lgrid, 1024, 0, G.stream>>>(a); GB_LAUNCHED(); } return GrB_SUCCESS; } while (0)
-    if (xt == zt) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_PULL(T, T);
-            GB_GEN(TC_BOOL, bool) GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    } else if (zt == TC_BOOL) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_PULL(T, bool);
-            GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    }
-#undef GB_PULL
-    return gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
+    const int grid = grid_for(a.nrows, 256, 8), lgrid = grid_for(a.long_cap, 1, 2);
+    bool ok;
+    GB_FOR_DOMAINS(xt, zt, ok,
+        spmv_masked_pull_kernel<XT_, ZT_><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED();
+        if (a.has_long) { spmv_pull_long_kernel<XT_, ZT_><<<lgrid, 1024, 0, G.stream>>>(a); GB_LAUNCHED(); });
+    return ok ? GrB_SUCCESS : gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
 }
 
 
@@ -239,11 +222,9 @@ __global__ void __launch_bounds__(256) push_kernel(const PushArgs a, int64_t cou
 }
 template <typename XT, typename ZT> static void push_launch(const PushArgs &a, int64_t count, int64_t chunk_bound) {
     const ZT init = a.add_op == OP_LAND ? (ZT)1 : (ZT)0;
-    const int g0 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nout, 256), (int64_t)G.num_sms * 16));
-    push_init_kernel<ZT><<<g0, 256, 0, G.stream>>>(static_cast<ZT *>(a.tval), a.tpres, a.nout, init); GB_LAUNCHED();
+    push_init_kernel<ZT><<<grid_for(a.nout), 256, 0, G.stream>>>(static_cast<ZT *>(a.tval), a.tpres, a.nout, init); GB_LAUNCHED();
     if (count > 0) {
-        const int g1 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(chunk_bound * 32, 256), (int64_t)G.num_sms * 16));
-        push_kernel<XT, ZT><<<g1, 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
+        push_kernel<XT, ZT><<<grid_for(chunk_bound * 32), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
     }
 }
 GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bool *done, std::string *err) {
@@ -255,8 +236,7 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     GB_TRY(counters.alloc(4, err));
     a.counters = counters;
     CU_TRY(cudaMemsetAsync(a.counters, 0, 32, G.stream), err);
-    const int g = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nin, 256 * 4), (int64_t)G.num_sms * 8));
-    push_stats_kernel<<<g, 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    push_stats_kernel<<<grid_for(a.nin, 256 * 4, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     unsigned long long h[2] = {0, 0};
     CU_TRY(cudaMemcpyAsync(h, a.counters, 16, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
@@ -266,39 +246,17 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     GB_TRY(list.alloc((size_t)count + 1, err));
     a.list = list;
     if (count > 0) {
-        const int gf = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(a.nin, 256), (int64_t)G.num_sms * 16));
-        push_frontier_kernel<<<gf, 256, 0, G.stream>>>(a); GB_LAUNCHED();
+        push_frontier_kernel<<<grid_for(a.nin), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     }
     GB_TRY(chunk_scan.alloc((size_t)count + 2, err));
     a.chunk_scan = chunk_scan;
     if (count > 0) {
-        const int g2 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count + 1, 256), (int64_t)G.num_sms * 16));
-        push_chunks_kernel<<<g2, 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
+        push_chunks_kernel<<<grid_for(count + 1), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
         GB_TRY(dev_exclusive_scan(a.chunk_scan, count + 1, err));
     } else CU_TRY(cudaMemsetAsync(a.chunk_scan, 0, 16, G.stream), err);
     const int64_t chunk_bound = edges / PUSH_CHUNK + count + 1;
-    bool ok = true;
-#define GB_PUSH(XT_, ZT_) do { push_launch<XT_, ZT_>(a, count, chunk_bound); } while (0)
-    if (xt == zt) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_PUSH(T, T); break;
-            GB_GEN(TC_BOOL, bool) GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-            default: ok = false;
-        }
-    } else {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_PUSH(T, bool); break;
-            GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-            default: ok = false;
-        }
-    }
-#undef GB_PUSH
+    bool ok;
+    GB_FOR_DOMAINS(xt, zt, ok, push_launch<XT_, ZT_>(a, count, chunk_bound));
     CU_TRY(cudaGetLastError(), err);
     *done = ok;
     return GrB_SUCCESS;

@@ -44,7 +44,6 @@ __global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzro
         tail_row[k] = tr; tail_last[k] = tl;
     }
 }
-static inline int rgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 16)); }
 
 GrB_Info spmv_run_plan(Csr &c, std::string *err) {
     if (c.run.headw) return GrB_SUCCESS;
@@ -63,19 +62,19 @@ GrB_Info spmv_run_plan(Csr &c, std::string *err) {
     GB_TRY(p.tail_last.alloc((size_t)p.nruns, err));
     CU_TRY(cudaMemsetAsync(p.headw, 0, ((size_t)nwords + 8) * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(flag + c.nrows, 0, 8, G.stream), err);
-    plan_nonempty_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, c.nrows, flag, p.pres_tmpl); GB_LAUNCHED();
+    plan_nonempty_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr32, c.nrows, flag, p.pres_tmpl); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(flag, c.nrows + 1, err));
     int64_t nz = 0;
     CU_TRY(cudaMemcpyAsync(&nz, flag + c.nrows, 8, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
     p.nnzrows = nz;
     GB_TRY(p.nzrow.alloc((size_t)nz, err));
-    plan_rows_kernel<<<rgrid(c.nrows), 256, 0, G.stream>>>(c.rowptr32, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
+    plan_rows_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr32, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
     CU_TRY(cudaMemsetAsync(cnt + p.nruns, 0, 8, G.stream), err);
     plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, p.lane, cnt); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
-    plan_base_kernel<<<rgrid(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
-    plan_tails_kernel<<<rgrid(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, c.rowptr32, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
+    plan_base_kernel<<<grid_for(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
+    plan_tails_kernel<<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, c.rowptr32, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
     flag.reset(); cnt.reset();
     // per-call scratch lives with the plan: partials of the rows that straddle runs (8 bytes covers every type)
     GB_TRY(p.ws_head.alloc((size_t)p.nruns * 8 + 16, err));
@@ -132,15 +131,15 @@ GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
     CU_TRY(cudaMemsetAsync(deg, 0, (size_t)n * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(inv, 0xff, (size_t)n * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(stats, 0, 24, G.stream), err);
-    hot_count_kernel<<<hgrid(c.nnz), 256, 0, G.stream>>>(c.col, c.nnz, deg); GB_LAUNCHED();
-    hot_iota_kernel<<<hgrid(n), 256, 0, G.stream>>>(ids, n); GB_LAUNCHED();
+    hot_count_kernel<<<grid_for(c.nnz, 256, 32), 256, 0, G.stream>>>(c.col, c.nnz, deg); GB_LAUNCHED();
+    hot_iota_kernel<<<grid_for(n, 256, 32), 256, 0, G.stream>>>(ids, n); GB_LAUNCHED();
     size_t tmp_bytes = 0;     // stable sort: equal degrees keep ascending column order (deterministic plan)
     CU_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, deg.get(), deg_sorted.get(), ids.get(), perm.get(), n, 0, 32, G.stream), err);
     DevBuf<void> tmp; GB_TRY(tmp.alloc(tmp_bytes, err));
     CU_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp.get(), tmp_bytes, deg.get(), deg_sorted.get(), ids.get(), perm.get(), n, 0, 32, G.stream), err);
     G.launches += 8;
     const int64_t topk = std::min<int64_t>(n, HOT_EXT);
-    hot_invert_kernel<<<hgrid(topk), 256, 0, G.stream>>>(perm, deg_sorted, topk, inv, stats); GB_LAUNCHED();
+    hot_invert_kernel<<<grid_for(topk, 256, 32), 256, 0, G.stream>>>(perm, deg_sorted, topk, inv, stats); GB_LAUNCHED();
     unsigned long long h[3] = {0, 0, 0};
     CU_TRY(cudaMemcpyAsync(h, stats, 24, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
@@ -152,7 +151,7 @@ GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
         GB_TRY(p.col.alloc((size_t)c.nnz, err));
         GB_TRY(p.ws_uhot.alloc(((size_t)p.henc + 256) * 8 + 16, err));      // + the unused tail of the last slices (< 16 per CTA)
         CU_TRY(cudaMemcpyAsync(p.perm, perm, (size_t)p.henc * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-        hot_encode_kernel<<<hgrid(c.nnz), 256, 0, G.stream>>>(c.col, inv, c.nnz, p.henc, p.col); GB_LAUNCHED();
+        hot_encode_kernel<<<grid_for(c.nnz, 256, 32), 256, 0, G.stream>>>(c.col, inv, c.nnz, p.henc, p.col); GB_LAUNCHED();
     }
     CU_TRY(cudaGetLastError(), err);
     c.hot = std::move(p);
@@ -189,13 +188,6 @@ void spmv_hot2_prep(const Hot2Args &h) {
     GB_LAUNCHED();
 }
 
-template <typename T> static bool spmv_run_fast(int add, int mul, const RunArgs &a, Hot2Args *hot, size_t table_limit) {
-#define GB_FAST(A, M) if (add == A && mul == M) { spmv_run_launch<T, T, A, M>(a, hot, table_limit); return true; }
-    GB_FAST(OP_PLUS, OP_TIMES) GB_FAST(OP_MIN, OP_PLUS) GB_FAST(OP_PLUS, OP_SECOND) GB_FAST(OP_PLUS, OP_FIRST)
-    GB_FAST(OP_PLUS, OP_PAIR) GB_FAST(OP_MIN, OP_FIRST) GB_FAST(OP_MIN, OP_SECOND)
-#undef GB_FAST
-    return false;
-}
 bool spmv_run_fast_int(int xt, int add, int mul, const RunArgs &a, Hot2Args *hot, size_t table_limit);
 bool spmv_run_dispatch(int xt, int add, int mul, const RunArgs &a, Hot2Args *hot, size_t table_limit) {
     switch (xt) {

@@ -208,7 +208,7 @@ template <typename XT> __device__ __forceinline__ XT ld_dsmem(uint32_t saddr, ui
 template <typename XT> __host__ __device__ constexpr int hot2_stage_bytes(bool need_a) { return RUN * 4 + (need_a ? RUN * (int)sizeof(XT) : 0); }
 constexpr int HOT2_WARPS = 32;
 
-template <typename XT, typename ZT, int ADD, int MUL, bool PIPE>
+template <typename XT, typename ZT, int ADD, int MUL>
 __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const RunArgs p, const Hot2Args h) {
     constexpr bool NEED_A = mul_reads_x(MUL);
     constexpr int STAGE = hot2_stage_bytes<XT>(NEED_A);
@@ -264,12 +264,10 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         if (col < henc) return gload<XT>(urest + col);
         return gload<XT>(uval + (col - henc));
     };
-    // Software pipeline over the warp's runs: the words of run r+1 are copied out of the stage and its gathers of u
-    // are ISSUED before run r is multiplied, folded and stored, so the gather latency sits under a run's worth of
-    // arithmetic instead of in front of it (and the bulk copy of run r+2 is in flight under both).
+    // One run at a time: its words are copied out of the stage (which frees it for the bulk copy of the warp's next run)
+    // and its gathers of u issued, then it is multiplied, folded and stored.
     uint32_t parity = 0;
-    RunLane<XT> cur, nxt;
-    int64_t cur_run = -1;
+    RunLane<XT> cur;
     auto fetch = [&](int64_t r, RunLane<XT> &L) {
         mbar_wait(bar, parity); parity ^= 1u;
         const int64_t q = r * RUN + lane * 8;
@@ -311,19 +309,7 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         if (lane == 0 && never == 0u && r + stride < p.nruns) issue(r + stride);
         spmv_run_gather<XT, MUL, false>(p, r, lane, nvalid, c, L, gather);
     };
-    if constexpr (sizeof(XT) > 4 || !PIPE) {
-        // one run at a time (8-byte values: two runs in flight do not fit in 64 registers per thread)
-        for (; run < p.nruns; run += stride) { fetch(run, cur); spmv_run_fold<XT, ZT, ADD, MUL, false>(p, run, lane, cur); }
-        (void)nxt; (void)cur_run;
-    } else {
-        if (run < p.nruns) { fetch(run, cur); cur_run = run; run += stride; }
-        while (cur_run >= 0) {
-            const bool more = run < p.nruns;
-            if (more) fetch(run, nxt);
-            spmv_run_fold<XT, ZT, ADD, MUL, false>(p, cur_run, lane, cur);
-            if (more) { cur = nxt; cur_run = run; run += stride; } else cur_run = -1;
-        }
-    }
+    for (; run < p.nruns; run += stride) { fetch(run, cur); spmv_run_fold<XT, ZT, ADD, MUL, false>(p, run, lane, cur); }
     cluster_sync_all();                       // no peer reads this CTA's table any more
 }
 
@@ -392,10 +378,10 @@ template <typename Kernel> static int hot2_max_clusters(Kernel kernel, int C, si
     return n;
 }
 
-template <typename XT, typename ZT, int ADD, int MUL, bool PIPE>
+template <typename XT, typename ZT, int ADD, int MUL>
 static void hot2_launch(const RunArgs &a, Hot2Args &h, size_t table_limit) {
     constexpr bool NEED_A = mul_reads_x(MUL);
-    auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL, PIPE>;
+    auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL>;
     const uint32_t cap = hot2_table_entries<XT>(NEED_A, h.henc, table_limit);
     const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(NEED_A) + (HOT2_WARPS + 1) * 8 + 8;
     const size_t smem_max = fixed + (size_t)cap * sizeof(XT);
@@ -428,8 +414,7 @@ template <typename XT, typename ZT, int ADD, int MUL>
 static void spmv_run_launch(const RunArgs &a, Hot2Args *hot, size_t table_limit) {
     if constexpr (ADD >= 0) {
         if (hot && !a.upres) {
-            if (sizeof(XT) <= 4 && tunables().spmv_pipe) hot2_launch<XT, ZT, ADD, MUL, true>(a, *hot, table_limit);
-            else hot2_launch<XT, ZT, ADD, MUL, false>(a, *hot, table_limit);
+            hot2_launch<XT, ZT, ADD, MUL>(a, *hot, table_limit);
             spmv_run_fixup_kernel<ZT, ADD, false><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
             return;
         }
@@ -441,4 +426,12 @@ static void spmv_run_launch(const RunArgs &a, Hot2Args *hot, size_t table_limit)
     }
     spmv_run_kernel<XT, ZT, ADD, MUL, false><<<(unsigned)ceil_div(a.nruns, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     spmv_run_fixup_kernel<ZT, ADD, false><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+}
+
+// the run kernels of the specialised semiring (add, mul) on T (spmv_common.cuh); false when it is not one
+template <typename T> static bool spmv_run_fast(int add, int mul, const RunArgs &a, Hot2Args *hot, size_t table_limit) {
+#define GB_FAST(A, M) if (add == A && mul == M) { spmv_run_launch<T, T, A, M>(a, hot, table_limit); return true; }
+    GB_SPMV_FAST_PAIRS(T, GB_FAST)
+#undef GB_FAST
+    return false;
 }

@@ -2,24 +2,7 @@
 #include "spmv_run.cuh"
 
 bool spmv_run_generic(int xt, int zt, const RunArgs &a) {
-#define GB_RUNGEN(XT_, ZT_) do { spmv_run_launch<XT_, ZT_, -1, -1>(a, nullptr, 0); return true; } while (0)
-    if (xt == zt) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_RUNGEN(T, T);
-            GB_GEN(TC_BOOL, bool) GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    } else if (zt == TC_BOOL) {
-        switch (xt) {
-#define GB_GEN(TC, T) case TC: GB_RUNGEN(T, bool);
-            GB_GEN(TC_INT8, int8_t) GB_GEN(TC_INT16, int16_t) GB_GEN(TC_INT32, int32_t) GB_GEN(TC_INT64, int64_t)
-            GB_GEN(TC_UINT8, uint8_t) GB_GEN(TC_UINT16, uint16_t) GB_GEN(TC_UINT32, uint32_t) GB_GEN(TC_UINT64, uint64_t)
-            GB_GEN(TC_FP32, float) GB_GEN(TC_FP64, double)
-#undef GB_GEN
-        }
-    }
-#undef GB_RUNGEN
-    return false;
+    bool ok;
+    GB_FOR_DOMAINS(xt, zt, ok, spmv_run_launch<XT_, ZT_, -1, -1>(a, nullptr, 0));
+    return ok;
 }

@@ -20,7 +20,6 @@
 #include <vector>
 #include "../../include/b200grb_compat.h"
 
-static inline int vgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)G.num_sms * 16)); }
 
 // ------------------------------------------------------------------ write-back:  w<mask> = accum(w, t)
 struct VecFinalizeArgs {
@@ -98,7 +97,7 @@ template <typename T> static void launch_finalize_typed(const VecFinalizeArgs &g
     a.n = g.n; a.wval = (const T *)g.wval; a.wpres = g.wpres; a.w_exists = g.w_exists; a.tval = (const T *)g.tval; a.tpres = g.tpres;
     a.mval = g.mval; a.mpres = g.mpres; a.mtc = g.mtc; a.has_mask = g.has_mask; a.mask_comp = g.mask_comp; a.mask_struct = g.mask_struct;
     a.replace = g.replace; a.accum_op = g.accum_op; a.oval = (T *)g.oval; a.opres = g.opres;
-    vec_finalize_typed_kernel<T><<<vgrid(g.n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    vec_finalize_typed_kernel<T><<<grid_for(g.n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
 }
 static bool finalize_typed(const VecFinalizeArgs &g) {
     // one type throughout, whole-vector write, per-position T, accumulator (if any) of that type with a same-type result
@@ -168,7 +167,7 @@ GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp ac
     const bool out_full = (w_full && !(mask && f.replace) && (accum != nullptr || (region != nullptr && tpres == nullptr))) ||
                           (tpres == nullptr && !mask && !region);
     if (!out_full) { GB_TRY(opres.alloc((size_t)n, err)); fa.opres = opres; }
-    if (!finalize_typed(fa)) { vec_finalize_kernel<<<vgrid(n), 256, 0, G.stream>>>(fa); GB_LAUNCHED(); }
+    if (!finalize_typed(fa)) { vec_finalize_kernel<<<grid_for(n), 256, 0, G.stream>>>(fa); GB_LAUNCHED(); }
     own_val.reset(); own_pres.reset();
     vector_adopt_device(w, oval.release(), opres.release());
     CU_TRY(cudaGetLastError(), err);
@@ -234,7 +233,7 @@ static GrB_Info vec_ewise(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     const bool t_full = mode == EW_ADD ? (!u->dpres || !v->dpres) : (!u->dpres && !v->dpres);
     if (!t_full) GB_TRY(tpres.alloc((size_t)n, &w->err));
     a.tval = tval; a.tpres = tpres;
-    vec_ewise_kernel<<<vgrid(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, a.ztc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Vector_eWiseAdd_BinaryOp(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_BinaryOp op,
@@ -288,7 +287,7 @@ static GrB_Info vec_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     GB_TRY(tval.alloc((size_t)n * tc_size(ztc) + 16, &w->err));
     if (u->dpres) GB_TRY(tpres.alloc((size_t)n, &w->err));
     a.tval = tval; a.tpres = tpres;
-    vec_ewise_kernel<<<vgrid(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, ztc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Vector_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_UnaryOp op, const GrB_Vector u, const GrB_Descriptor desc) {
@@ -386,7 +385,7 @@ static GrB_Info vec_assign_scalar(GrB_Vector w, const GrB_Vector mask, const GrB
         if (!idx.empty()) {
             DevBuf<uint64_t> didx;
             GB_TRY(upload_indices(idx, didx, &w->err));
-            region_mark_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), region); GB_LAUNCHED();
+            region_mark_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), region); GB_LAUNCHED();
         }
     }
     return vector_write(w, mask, accum, desc_flags(desc), tval, nullptr, wtc, true, region, std::move(tval));
@@ -421,7 +420,7 @@ extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const
     if (!idx.empty()) {
         DevBuf<uint64_t> didx;
         GB_TRY(upload_indices(idx, didx, &w->err));
-        vec_scatter_u_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres, region); GB_LAUNCHED();
+        vec_scatter_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres, region); GB_LAUNCHED();
     }
     return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, region, std::move(tval), std::move(tpres));
 }
@@ -465,7 +464,7 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
     if (!idx.empty()) {
         DevBuf<uint64_t> didx;
         GB_TRY(upload_indices(idx, didx, &w->err));
-        vec_gather_u_kernel<<<vgrid((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres); GB_LAUNCHED();
+        vec_gather_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres); GB_LAUNCHED();
     }
     return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, nullptr, std::move(tval), std::move(tpres));
 }
@@ -501,7 +500,7 @@ __global__ void __launch_bounds__(256) vec_reduce_kernel(const ReduceArgs a) {
 GrB_Info dev_reduce_values(const void *val, const uint8_t *pres, int vtc, int64_t n, int op, int mtc, Sc *out, bool *has, std::string *err) {
     out->u = 0; *has = false;
     if (n <= 0) return GrB_SUCCESS;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256 * 8), (int64_t)G.num_sms * 8));
+    const int grid = grid_for(n, 256 * 8, 8);
     ReduceArgs a{};
     a.n = n; a.val = val; a.pres = pres; a.vtc = vtc; a.op = op; a.mtc = mtc;
     DevBuf<Sc> part; DevBuf<uint8_t> part_has;

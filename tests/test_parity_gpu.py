@@ -318,14 +318,13 @@ def test_rmat_masked_mxm_large_ST1_and_valued_mask():
     assert np.array_equal(Bp, R2.indptr) and np.array_equal(Bj, R2.indices) and np.array_equal(Bx, R2.data.astype(np.int64))
 
 
-@pytest.mark.parametrize("mode", [{}, {"B200GRB_SPMV_HOT": "64"}, {"B200GRB_SPMV_HOT": "0"}, {"B200GRB_SPMV_RUN": "0"}, {"B200GRB_SPMV_RUN": "0", "B200GRB_SPMV_ITEMS": "16"},
-                                  {"B200GRB_SPMV_RUN": "0", "B200GRB_SPMV_ITEMS": "4"}])
+@pytest.mark.parametrize("mode", [{}, {"B200GRB_SPMV_HOT": "64"}, {"B200GRB_SPMV_HOT": "0"}, {"B200GRB_SPMV_RUN": "0"}])
 def test_large_spmv_all_kernel_variants(mode):
     """Large dense-u SpMV through every kernel variant (hot-table run kernel with TMA-staged runs at two table
-    sizes, plain run kernel, tile kernel with 8 / 16 / 4 entries per thread): exact against the oracle on
-    small-integer data, for specialised and run-time semirings."""
+    sizes, plain run kernel, tile kernel): exact against the oracle on small-integer data, for specialised and
+    run-time semirings."""
     import os
-    old = {k: os.environ.get(k) for k in ("B200GRB_SPMV_ITEMS", "B200GRB_SPMV_HOT", "B200GRB_HOT_GROUPS", "B200GRB_SPMV_RUN")}
+    old = {k: os.environ.get(k) for k in ("B200GRB_SPMV_HOT", "B200GRB_SPMV_RUN")}
     os.environ.update(mode)
     gb.lib.B200_reload_tunables()                 # the switches are read at GrB_init and on request only
     try:
@@ -390,7 +389,7 @@ def test_large_spmv_sparse_u(dens):
 
 
 def test_rmat_unmasked_spgemm_matches_scipy():
-    """configs[3] secondary: unmasked A (+.second) A, all three row bins (hash / hash / dense accumulator)."""
+    """configs[3] secondary: unmasked A (+.second) A, all three row bins (ESC / ESC / dense accumulator)."""
     n, indptr, indices = _rmat(12)
     rng = np.random.default_rng(4)
     vals = rng.integers(1, 5, len(indices)).astype(np.float32)
@@ -408,10 +407,10 @@ def test_rmat_unmasked_spgemm_matches_scipy():
 
 
 @pytest.mark.parametrize("typ,sr", [(FP32, "PLUS_TIMES"), (FP64, "PLUS_SECOND"), (INT64, "PLUS_TIMES"), (FP32, "MIN_PLUS"), (BOOL, "LOR_LAND"), (UINT8, "MAX_FIRST")])
-def test_unmasked_spgemm_esc_equals_hash_and_scipy(typ, sr, monkeypatch):
-    """The expand-sort-compress numeric kernels (small bin: a warp per row, medium bin: a CTA per row) against the hash kernels they
-    replace (B200GRB_SPGEMM_ESC=0) -- pattern and every value, bit for bit (quarter-valued inputs: every fold order gives the same
-    sum) -- and, for PLUS_TIMES, against scipy.  The graph has rows in all three bins."""
+def test_unmasked_spgemm_esc_equals_model_and_scipy(typ, sr):
+    """The expand-sort-compress numeric kernels (small bin: a warp per row, medium bin: a CTA per row) against the oracle --
+    pattern and every value, bit for bit (quarter-valued inputs: every fold order gives the same sum) -- and, for PLUS_TIMES,
+    against scipy.  The graph has rows in all three bins."""
     n, indptr, indices = _rmat(12)
     rng = np.random.default_rng(8)
     if typ in (FP32, FP64):
@@ -421,20 +420,18 @@ def test_unmasked_spgemm_esc_equals_hash_and_scipy(typ, sr, monkeypatch):
     else:
         vals = rng.integers(1, 4, len(indices)).astype(typ.dtype)
     A = Matrix.from_csr(indptr, indices, vals, n, n, typ)
-    semiring = getattr(typ, sr)
-    out = {}
-    for esc in ("1", "0"):
-        monkeypatch.setenv("B200GRB_SPGEMM_ESC", esc)
-        gb.lib.B200_reload_tunables()
-        out[esc] = A.mxm(A, semiring=semiring).to_csr()
-    monkeypatch.delenv("B200GRB_SPGEMM_ESC")
-    gb.lib.B200_reload_tunables()
-    for a, b in zip(out["1"], out["0"]):
-        assert np.array_equal(a, b)
+    C = A.mxm(A, semiring=getattr(typ, sr))
+    assert {"esc-small", "esc-medium", "spa"} <= set(gb.ffi.string(gb.lib.B200_debug_last_kernel()).decode().split(";"))
+    rows = np.repeat(np.arange(n), np.diff(indptr))
+    Ao = orc.SpMat(typ.name, n, n, rows, indices, vals)
+    ref = orc.mxm(orc.SpMat(typ.name, n, n), None, None, (*sr.split("_"), typ.name), Ao, Ao, "")
+    ci, cj, cx = C.to_arrays()
+    assert np.array_equal(ci, ref.I) and np.array_equal(cj, ref.J)
+    assert cx.dtype == ref.X.dtype and np.array_equal(cx.view(np.uint8), ref.X.view(np.uint8))
     if sr == "PLUS_TIMES":
         S = sp.csr_matrix((vals.astype(np.float64), indices, indptr), shape=(n, n))
         R = (S @ S).tocsr(); R.sort_indices()
-        Cp, Cj, Cx = out["1"]
+        Cp, Cj, Cx = C.to_csr()
         assert np.array_equal(Cp, R.indptr) and np.array_equal(Cj, R.indices) and np.array_equal(Cx.astype(np.float64), R.data)
 
 

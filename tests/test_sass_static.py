@@ -52,7 +52,7 @@ def hot2_sass(sass_text):
 
 
 def test_every_hot2_instantiation_keeps_the_stage_guard(hot2_sass):
-    assert len(hot2_sass) >= 20                       # FP32 / FP64 / integer / BOOL semirings x {plain, pipelined}
+    assert len(hot2_sass) == 47                       # the specialised semirings: 7 on each of the 6 numeric types, 5 on BOOL
     for name, ops in hot2_sass.items():
         waits = [i for i, o in enumerate(ops) if o.startswith("SYNCS.PHASECHK")]
         copies = [i for i, o in enumerate(ops) if o.startswith("UBLKCP")]

@@ -170,15 +170,11 @@ def spmv_route(S, sr, vxm, env, sparse_u=False, upres=None, masked=False):
             henc, cover = _hot_stats(key)
             hot = henc >= 16 and (hot_kb >= 0 or cover >= 0.25)
         if hot:
-            pipe = orc.DTYPES[typ]().itemsize <= 4 and int(env.get("B200GRB_SPMV_PIPE", 0)) != 0
-            return "run+hot-table (TMA-staged, pipelined)" if pipe else "run+hot-table (TMA-staged)"
+            return "run+hot-table (TMA-staged)"
         return "run (sparse u)" if sparse_u else "run"
     if c.nnz == 0:
         return "empty"
-    if not fast:
-        return "tile (run-time operators)"
-    items = int(env.get("B200GRB_SPMV_ITEMS", 8))
-    return f"tile (specialised, {items if items in (4, 16) else 8} items)"
+    return "tile (specialised, 8 items)" if fast else "tile (run-time operators)"
 
 
 def flops_per_row(SA, SB):
@@ -221,12 +217,11 @@ def gemm_route(SA, SB, SM, desc, env):
     if SM is None and "C" in desc:
         return []
     f = flops_per_row(SA, Bt)
-    esc = int(env.get("B200GRB_SPGEMM_ESC", 1)) != 0
     out = []
     if ((f > 0) & (f <= 128)).any():
-        out.append("esc-small" if esc else "hash-small")
+        out.append("esc-small")
     if ((f > 128) & (f <= 2048)).any():
-        out.append("esc-medium" if esc else "hash-medium")
+        out.append("esc-medium")
     if (f > 2048).any():
         out.append("spa")
     return out
@@ -423,10 +418,10 @@ def tile_pattern(items, tail):
 
 
 @pytest.mark.parametrize("tail", [-1, 0, 1])
-@pytest.mark.parametrize("items", [4, 8, 16])
+@pytest.mark.parametrize("items", [8])
 def test_tile_boundaries(items, tail):
     S = tile_pattern(items, tail)
-    env = {"B200GRB_SPMV_RUN": 0, "B200GRB_SPMV_ITEMS": items}
+    env = {"B200GRB_SPMV_RUN": 0}
     routes = run_spmv(S, f"tile-{items}-{tail}", env)
     assert f"tile (specialised, {items} items)" in routes and "tile (run-time operators)" in routes, routes
     side(f"tile-{items}-nnz{tail:+d}")
@@ -509,8 +504,6 @@ HOT_CASES = {
     "nnz-below": ((1 << 16), (1 << 20) - 1, {}, "run"),
     "ncols-below": ((1 << 16) - 1, (1 << 20) + 1, {}, "run"),
     "table-64": ((1 << 16), (1 << 20) + 1, {"B200GRB_SPMV_HOT": 64}, "hot"),
-    "pipe": ((1 << 16), (1 << 20) + 1, {"B200GRB_SPMV_PIPE": 1}, "hot"),
-    "pipe-table-64": ((1 << 16), (1 << 20) + 1, {"B200GRB_SPMV_PIPE": 1, "B200GRB_SPMV_HOT": 64}, "hot"),
     "cover-below": ((1 << 20), (1 << 20) + 1, {}, "run"),
     "cover-below-forced": ((1 << 20), (1 << 20) + 1, {"B200GRB_SPMV_HOT": 128}, "hot"),
 }
@@ -647,19 +640,17 @@ def unmasked_operands():
     return SA, SB
 
 
-@pytest.mark.parametrize("esc", [1, 0])
-def test_unmasked_flops_bins(esc):
+def test_unmasked_flops_bins():
     SA, SB = unmasked_operands()
-    routes = run_gemm(SA, SB, None, "", f"unmasked-esc{esc}", {"B200GRB_SPGEMM_ESC": esc})
-    want = ["esc-small" if esc else "hash-small", "esc-medium" if esc else "hash-medium", "spa"]
-    assert all(r == want for r in routes), routes
-    side(f"unmasked-bins-esc{esc}")
+    routes = run_gemm(SA, SB, None, "", "unmasked")
+    assert all(r == ["esc-small", "esc-medium", "spa"] for r in routes), routes
+    side("unmasked-bins")
 
 
 @pytest.mark.parametrize("ncols", [1, 31, 32, 33, 4097])
 def test_spa_widths(ncols):
     """The dense accumulator keeps ceil(ncols / 32) bit words: widths that are not a multiple of 32.  Row 0 has 2048
-    products (hash / ESC), row 1 2049 (spa)."""
+    products (ESC), row 1 2049 (spa)."""
     per = min(ncols, 64)
     k0, r0 = divmod(2048, per)
     blens = [per] * k0 + ([r0] if r0 else []) + [1]
@@ -1039,14 +1030,14 @@ def test_plans_dropped_when_matrix_changes(path):
     side(f"seq-{path}")
 
 
-def test_alternating_semirings_rebuild_tile_plan():
-    """Specialised (4 items) and run-time-operator (8 items) semirings alternate on one matrix: the tile plan is rebuilt
-    for every call."""
-    S = tile_pattern(4, 1)
-    env = {"B200GRB_SPMV_RUN": 0, "B200GRB_SPMV_ITEMS": 4}
+def test_alternating_semirings_share_tile_plan():
+    """Specialised and run-time-operator semirings alternate on one matrix: every call reuses the one cached tile plan,
+    and every result equals the model."""
+    S = tile_pattern(8, 1)
+    env = {"B200GRB_SPMV_RUN": 0}
     srs = [("PLUS", "TIMES", "INT32"), ("MAX", "TIMES", "INT32")] * 3 + [("PLUS", "TIMES", "FP64"), ("MAX", "MINUS", "FP64")] * 2
     routes = run_spmv(S, "alternate", env, srs=srs, forms=("mxv",))
-    assert routes == {"tile (specialised, 4 items)", "tile (run-time operators)"}, routes
+    assert routes == {"tile (specialised, 8 items)", "tile (run-time operators)"}, routes
     side("seq-alternate")
 
 
@@ -1110,16 +1101,15 @@ def test_mxv_in_place_sequences(inplace):
 
 
 # ------------------------------------------------------------------ every entry, variant and boundary side was reached
-ALL_ENTRIES = {"tile (specialised, 4 items)", "tile (specialised, 8 items)", "tile (specialised, 16 items)", "tile (run-time operators)",
-               "run", "run (sparse u)", "run+hot-table (TMA-staged)", "run+hot-table (TMA-staged, pipelined)", "pull", "push",
-               "esc-small", "esc-medium", "hash-small", "hash-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot",
+ALL_ENTRIES = {"tile (specialised, 8 items)", "tile (run-time operators)", "run", "run (sparse u)", "run+hot-table (TMA-staged)",
+               "pull", "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot",
                "filter=exact", "filter=bloom", "mxv=in-place"}
 ALL_SIDES = (
-    {f"tile-{i}-nnz{t:+d}" for i in (4, 8, 16) for t in (-1, 0, 1)} | {"tile-nrows=1", "tile-ncols=1", "tile-last-entry"}
+    {f"tile-8-nnz{t:+d}" for t in (-1, 0, 1)} | {"tile-nrows=1", "tile-ncols=1", "tile-last-entry"}
     | {f"run-nnz{t:+d}" for t in (-1, 0, 1)} | {"run-threshold-below", "run-threshold-at"}
     | {f"hot-{c}" for c in HOT_CASES} | {f"push-{k}" for k in ("edges-at", "edges-over", "count-at", "count-over")}
     | {f"pull-{m}" for m in PULL_MASKS}
-    | {"unmasked-bins-esc1", "unmasked-bins-esc0"} | {f"spa-ncols-{n}" for n in (1, 31, 32, 33, 4097)}
+    | {"unmasked-bins"} | {f"spa-ncols-{n}" for n in (1, 31, 32, 33, 4097)}
     | {f"masked-{s}" for s in ("warp-limit", "mask-128-129", "mask-512-513", "mask-2048-2049", "chunks-1-2", "chunks-3-4",
                                "a-batch-256", "a-batch-1024", "long-b-rows", "b-past-end", "blk7", "blk12", "mask-empty", "a-empty",
                                "b-empty")}

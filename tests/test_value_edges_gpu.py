@@ -90,14 +90,10 @@ def rmat17():
 
 # SpMV paths: pattern, the switches, the expected kernel, the semirings it serves
 SPMV = {
-    "tile-4": dict(shape="small", env={"B200GRB_SPMV_ITEMS": 4}, kernel="tile (specialised, 4 items)", only=spmv_specialised),
     "tile-8": dict(shape="small", env={}, kernel="tile", only=None),
-    "tile-16": dict(shape="small", env={"B200GRB_SPMV_ITEMS": 16}, kernel="tile (specialised, 16 items)", only=spmv_specialised),
     "run": dict(shape="run", env={}, kernel="run", only=None),
     "run-sparse-u": dict(shape="run", env={}, kernel="run (sparse u)", only=None, sparse_u=True),
     "hot": dict(shape="rmat", env={"B200GRB_SPMV_HOT": 128}, kernel="run+hot-table (TMA-staged)", only=spmv_specialised),
-    "hot-pipe": dict(shape="rmat", env={"B200GRB_SPMV_HOT": 128, "B200GRB_SPMV_PIPE": 1}, kernel="run+hot-table (TMA-staged, pipelined)",
-                     only=spmv_specialised),
     "pull": dict(shape="pull", env={}, kernel="pull", only=lambda a, m, t: a in ("LOR", "LAND", "ANY"), mask=True),
     "push": dict(shape="pull", env={"B200GRB_FORCE_PUSH": 1}, kernel="push", only=lambda a, m, t: a in ("LOR", "LAND", "ANY"),
                  mask=True, sparse_u=True),
@@ -126,10 +122,8 @@ def _spmv_expect(path, cfg, typ, add, mul, vxm):
     k = cfg["kernel"]
     if path == "tile-8":
         return None                                            # specialised (8 items) or run-time operators: checked by prefix
-    if path.startswith("hot") and mul == ("SECOND" if vxm else "FIRST"):
+    if path == "hot" and mul == ("SECOND" if vxm else "FIRST"):
         return "run"                                           # the multiply ignores u: no gathers for the hot table to serve
-    if path == "hot-pipe" and orc.DTYPES[typ]().itemsize > 4:
-        return "run+hot-table (TMA-staged)"                   # the pipelined kernel serves types of up to 4 bytes
     return k
 
 
@@ -182,7 +176,7 @@ def run_spmv_path(path, typ):
 
 
 @pytest.mark.parametrize("typ", ALL_T)
-@pytest.mark.parametrize("path", ["tile-4", "tile-8", "tile-16", "run", "run-sparse-u", "pull", "push"])   # SPMV_CASES
+@pytest.mark.parametrize("path", ["tile-8", "run", "run-sparse-u", "pull", "push"])   # SPMV_CASES
 def test_spmv_edges(path, typ):
     if not semirings(typ, SPMV[path]["only"]):
         pytest.skip(f"no specialised SpMV kernel on {typ}")
@@ -190,7 +184,7 @@ def test_spmv_edges(path, typ):
 
 
 @pytest.mark.parametrize("typ", HOT_T)
-@pytest.mark.parametrize("path", ["hot", "hot-pipe"])
+@pytest.mark.parametrize("path", ["hot"])
 def test_spmv_hot_table_edges(path, typ):
     """R-MAT scale 17: edge values land at hot and cold columns of u and inside hub rows that span many runs, whose
     partials the fix-up kernel folds."""
@@ -200,9 +194,9 @@ def test_spmv_hot_table_edges(path, typ):
 # ------------------------------------------------------------------ SpGEMM
 # path: (A, B, mask patterns, descriptor, switches, expected kernels)
 def _gemm_patterns(path):
-    if path in ("esc-small", "hash-small"):
+    if path == "esc-small":
         return pattern(21, 200, 200, 6), pattern(22, 200, 200, 6), None, ""
-    if path in ("esc-medium", "hash-medium"):
+    if path == "esc-medium":
         return pattern(23, 150, 300, 30), pattern(24, 300, 300, 30), None, ""
     if path == "spa":
         return pattern(25, 64, 400, 60), pattern(26, 400, 3000, 60), None, ""
@@ -228,9 +222,7 @@ def _gemm_patterns(path):
 
 
 GEMM = {
-    "esc-small": ({}, ["esc-small"]), "hash-small": ({"B200GRB_SPGEMM_ESC": 0}, ["hash-small"]),
-    "esc-medium": ({}, ["esc-medium"]), "hash-medium": ({"B200GRB_SPGEMM_ESC": 0}, ["hash-medium"]),
-    "spa": ({}, ["spa"]), "masked-warp": ({}, ["masked-warp"]),
+    "esc-small": ({}, ["esc-small"]), "esc-medium": ({}, ["esc-medium"]), "spa": ({}, ["spa"]), "masked-warp": ({}, ["masked-warp"]),
     "stream-S": ({}, ["stream-S"]), "stream-M": ({}, ["stream-M"]), "stream-L": ({}, ["stream-L"]),
     "split": ({}, ["stream-S", "stream-L"]), "dot": ({}, ["dot"]), "st1-transpose": ({}, ["masked-warp"]),
 }
@@ -391,7 +383,7 @@ def _general_values(rng, typ, n, scale):
     return x.astype(dt)
 
 
-BOUND_SPMV = ["tile-8", "run", "run-sparse-u", "hot", "hot-pipe"]
+BOUND_SPMV = ["tile-8", "run", "run-sparse-u", "hot"]
 
 
 @pytest.mark.parametrize("scale", ["normal", "subnormal"])
@@ -447,14 +439,13 @@ def test_fp_sums_within_error_bound(path, typ, scale):
 
 
 # ------------------------------------------------------------------ every path of the table was reached
-ALL_PATHS = {"tile (specialised, 4 items)", "tile (specialised, 8 items)", "tile (specialised, 16 items)", "tile (run-time operators)",
-             "run", "run (sparse u)", "run+hot-table (TMA-staged)", "run+hot-table (TMA-staged, pipelined)", "pull", "push",
-             "esc-small", "esc-medium", "hash-small", "hash-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot"}
+ALL_PATHS = {"tile (specialised, 8 items)", "tile (run-time operators)", "run", "run (sparse u)", "run+hot-table (TMA-staged)", "pull",
+             "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot"}
 
 
-SPMV_CASES = ["tile-4", "tile-8", "tile-16", "run", "run-sparse-u", "pull", "push"]
+SPMV_CASES = ["tile-8", "run", "run-sparse-u", "pull", "push"]
 MIXED_PATHS = ["tile-8", "run", "esc-small", "spa", "masked-warp", "stream-L", "dot"]
-FULL_COUNT = (len(SPMV_CASES) * len(ALL_T) + 2 * len(HOT_T) + len(GEMM) * len(ALL_T) + len(MIXED_PATHS) * len(MIXED)
+FULL_COUNT = (len(SPMV_CASES) * len(ALL_T) + len(HOT_T) + len(GEMM) * len(ALL_T) + len(MIXED_PATHS) * len(MIXED)
               + (len(BOUND_SPMV) + len(GEMM)) * len(FP_T) * 2)
 
 

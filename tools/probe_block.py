@@ -20,10 +20,8 @@ w = Vector.sparse(FP32, lb)
 sp_ = gb.ffi.new("void**"); gb.lib.B200_get_stream(sp_)
 stream = torch.cuda.ExternalStream(int(gb.ffi.cast("uintptr_t", sp_[0])))
 print(f"block of a {world}-way partition: {lb} rows, {len(lidx)} entries")
-for label, env in (("default", {}), ("plain run kernel", {"B200GRB_SPMV_HOT": "0"}), ("table 32KB", {"B200GRB_SPMV_HOT": "32"}), ("table 64KB", {"B200GRB_SPMV_HOT": "64"}),
-                   ("table 128KB pipelined", {"B200GRB_SPMV_HOT": "128", "B200GRB_SPMV_PIPE": "1"})):
-    for k in ("B200GRB_SPMV_HOT", "B200GRB_SPMV_PIPE"):
-        os.environ.pop(k, None)
+for label, env in (("default", {}), ("plain run kernel", {"B200GRB_SPMV_HOT": "0"}), ("table 32KB", {"B200GRB_SPMV_HOT": "32"}), ("table 64KB", {"B200GRB_SPMV_HOT": "64"})):
+    os.environ.pop("B200GRB_SPMV_HOT", None)
     os.environ.update(env); gb.lib.B200_reload_tunables()
     for _ in range(10):
         A.mxv(u, semiring=FP32.PLUS_TIMES, out=w)

@@ -34,9 +34,12 @@ enum OpCode : int {
     OP_TIMES, OP_DIV, OP_RDIV, OP_POW, OP_ISEQ, OP_ISNE, OP_ISGT, OP_ISLT, OP_ISGE, OP_ISLE,
     OP_LOR, OP_LAND, OP_LXOR, OP_BOR, OP_BAND, OP_BXOR, OP_BXNOR,
     OP_EQ, OP_NE, OP_GT, OP_LT, OP_GE, OP_LE,   // z = BOOL
+    // positional (z = INT32 / INT64, an index of x or y; never handed to a kernel: positional.cu rewrites the call)
+    OP_FIRSTI, OP_FIRSTI1, OP_FIRSTJ, OP_FIRSTJ1, OP_SECONDI, OP_SECONDI1, OP_SECONDJ, OP_SECONDJ1,
     OP_USER, OP_COUNT
 };
 static inline bool op_is_cmp(int op) { return op >= OP_EQ && op <= OP_LE; }
+static inline bool op_is_positional(int op) { return op >= OP_FIRSTI && op <= OP_SECONDJ1; }
 
 // ---------------------------------------------------------------- opaque objects
 struct GB_Type_opaque { int magic; int code; size_t size; const char *name; };
@@ -57,8 +60,10 @@ enum UnaryCode : int {
     UOP_TANH, UOP_ACOSH, UOP_ASINH, UOP_ATANH, UOP_SIGNUM, UOP_CEIL, UOP_FLOOR, UOP_ROUND, UOP_TRUNC, UOP_EXP2,
     UOP_EXPM1, UOP_LOG10, UOP_LOG1P, UOP_LGAMMA, UOP_TGAMMA, UOP_ERF, UOP_ERFC,
     UOP_ISINF, UOP_ISNAN, UOP_ISFINITE,      // z = BOOL
+    UOP_POSITIONI, UOP_POSITIONI1, UOP_POSITIONJ, UOP_POSITIONJ1,      // z = INT32 / INT64, the row or column of the entry
     UOP_COUNT
 };
+static inline bool uop_is_positional(int op) { return op >= UOP_POSITIONI && op <= UOP_POSITIONJ1; }
 
 // device memory (stream-ordered pool on G.stream)
 GrB_Info dmalloc(void **p, size_t bytes, std::string *err);
@@ -281,12 +286,40 @@ GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp ac
                       const void *tval, const uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region,
                       DevBuf<void> &&own_val = DevBuf<void>(), DevBuf<uint8_t> &&own_pres = DevBuf<uint8_t>());
 
+// positional operators (positional.cu).  What a positional operator returns, decoded: the index of the first or the second
+// operand (`second`), its row or its column (`col`), plus `off` (0, or 1 for the ...1 forms)
+struct PosOp { bool second, col; int64_t off; };
+static inline PosOp pos_binop(int op) { const int d = op - OP_FIRSTI; return PosOp{(d >> 2) != 0, ((d >> 1) & 1) != 0, (int64_t)(d & 1)}; }
+static inline PosOp pos_unop(int op) { const int d = op - UOP_POSITIONI; return PosOp{false, (d >> 1) != 0, (int64_t)(d & 1)}; }
+// A positional operator as accumulator, or in an operation that has no positional form: refused before anything is read
+GrB_Info gb_refuse_positional_accum(const GrB_BinaryOp accum, const char *fn);
+// A positional semiring with a user-defined monoid or accumulator: GrB_INVALID_VALUE, like every other call with a user-defined
+// operator, and before the hypersparse dispatch and the device check (the rewrite would hand them to the write-back)
+GrB_Info gb_refuse_user_with_positional(const GrB_Semiring s, const GrB_BinaryOp accum, const char *fn);
+GrB_Info gb_refuse_positional(const GrB_BinaryOp op, const char *fn);
+GrB_Info gb_refuse_positional(const GrB_Semiring s, const char *fn);
+static inline GrB_Info gb_refuse_positional(const GrB_Monoid, const char *) { return GrB_SUCCESS; }   // no monoid is positional
+// out[p] (type tc = INT32 / INT64, n positions) = v(p) folded cnt[p] times with the monoid `add`: v(p) = (zero ? 0 : ids[p] or p)
+// + off, truncated like a C cast.  cnt NULL: v(p) itself (one product per position).  ids NULL: the position is the index.
+GrB_Info pos_vector_values(void *out, int tc, const int64_t *cnt, int add, int64_t n, bool zero, const uint64_t *ids, int64_t off,
+                           std::string *err);
+// the same over the entries of a CSR: v(e) = the column (by_col) or the row of entry e, through ids when given
+GrB_Info pos_csr_values(void *out, int tc, const int64_t *cnt, int add, const Csr &c, bool by_col, const uint64_t *ids, int64_t off,
+                        std::string *err);
+// GrB_mxv / GrB_vxm / GrB_mxm with a positional multiply (spmv.cu / spgemm.cu).  ids_*: the original index of every position of
+// a compact (hypersparse) operand, in device memory; NULL when the positions are the indices
+GrB_Info positional_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                        const GrB_Vector u, const DescFlags &f, bool vxm, const uint64_t *ids_in, const uint64_t *ids_out);
+GrB_Info positional_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                        const GrB_Matrix B, const DescFlags &f, const uint64_t *ids_m, const uint64_t *ids_k, const uint64_t *ids_n);
+
 // kernels (device_ops.cu / spmv.cu / spgemm.cu)
 GrB_Info dev_build_rowptr32(Csr &c, std::string *err);
 GrB_Info dev_exclusive_scan(int64_t *data, int64_t n, std::string *err);
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err);
 GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int from_code, int64_t n, std::string *err);
 GrB_Info dev_count_present(const uint8_t *pres, int64_t n, int64_t *count, std::string *err);
+GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err);     // host list -> device (vector_ops.cu)
 
 // ---------------------------------------------------------------- scalar carrier
 // A value of any builtin type held in 64 bits: BOOL/UINT* in .u, INT* in .i, FP* in .d

@@ -99,7 +99,13 @@ GrB_Info hyper_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum
     if (r == GrB_SUCCESS) r = compact_vector(u, in_ids, &uc);
     if (r == GrB_SUCCESS) r = compact_vector(w, out_ids, &wc);
     if (r == GrB_SUCCESS && mask) r = compact_vector(mask, out_ids, &mc);
-    if (r == GrB_SUCCESS) r = vxm ? GrB_vxm(wc, mc, accum, s, uc, Ac, desc) : GrB_mxv(wc, mc, accum, s, Ac, uc, desc);
+    if (r == GrB_SUCCESS && op_is_positional(s->mul->opcode)) {
+        // a positional multiply returns original indices, not compact ranks: the id lists go to the device
+        DevBuf<uint64_t> din, dout;
+        r = upload_indices(in_ids, din, &w->err);
+        if (r == GrB_SUCCESS) r = upload_indices(out_ids, dout, &w->err);
+        if (r == GrB_SUCCESS) r = positional_mxv(wc, mc, accum, s, Ac, uc, f, vxm, din, dout);
+    } else if (r == GrB_SUCCESS) r = vxm ? GrB_vxm(wc, mc, accum, s, uc, Ac, desc) : GrB_mxv(wc, mc, accum, s, Ac, uc, desc);
     if (r == GrB_SUCCESS) r = expand_vector(w, wc, out_ids);
     else if (wc) w->err = wc->err;
     GrB_Matrix_free(&Ac); GrB_Vector_free(&uc); GrB_Vector_free(&wc); GrB_Vector_free(&mc);
@@ -134,7 +140,13 @@ GrB_Info hyper_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
     // C may alias A or B: the compact C is a separate object either way, the result replaces C at the end
     if (r == GrB_SUCCESS) r = compact_matrix(C, ms, ns, &Cc);
     if (r == GrB_SUCCESS && Mask) r = compact_matrix(Mask, ms, ns, &Mc);
-    if (r == GrB_SUCCESS) r = GrB_mxm(Cc, Mc, accum, s, Ac, Bc, desc);
+    if (r == GrB_SUCCESS && op_is_positional(s->mul->opcode)) {
+        DevBuf<uint64_t> dm, dk, dn;
+        r = upload_indices(ms, dm, &C->err);
+        if (r == GrB_SUCCESS) r = upload_indices(ks, dk, &C->err);
+        if (r == GrB_SUCCESS) r = upload_indices(ns, dn, &C->err);
+        if (r == GrB_SUCCESS) r = positional_mxm(Cc, Mc, accum, s, Ac, Bc, f, dm, dk, dn);
+    } else if (r == GrB_SUCCESS) r = GrB_mxm(Cc, Mc, accum, s, Ac, Bc, desc);
     if (r == GrB_SUCCESS) r = expand_matrix(C, Cc, ms, ns);
     else if (Cc) C->err = Cc->err;
     GrB_Matrix_free(&Ac); GrB_Matrix_free(&Bc); GrB_Matrix_free(&Cc); GrB_Matrix_free(&Mc);

@@ -189,6 +189,7 @@ static GrB_Info matrix_assign_scalar(GrB_Matrix C, const GrB_Matrix Mask, const 
     if (!C) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL argument", fn);
     if (!gb_valid_matrix(C) || (Mask && !gb_valid_matrix(Mask))) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid object", fn);
     std::string *err = &C->err;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, err, "%s: user-defined accumulators are host function pointers and cannot run on the GPU", fn);
     if (Mask && (Mask->nrows != C->nrows || Mask->ncols != C->ncols)) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: the mask must have C's dimensions", fn);
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
@@ -271,6 +272,7 @@ extern "C" GrB_Info GrB_Matrix_extract(GrB_Matrix C, const GrB_Matrix Mask, cons
     if (!C || !A) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL argument", fn);
     if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || (Mask && !gb_valid_matrix(Mask))) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid object", fn);
     std::string *err = &C->err;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, err, "%s: user-defined accumulators cannot run on the GPU", fn);
     const DescFlags f = desc_flags(desc);
     const uint64_t an = f.tran0 ? A->ncols : A->nrows, am = f.tran0 ? A->nrows : A->ncols;
@@ -423,7 +425,9 @@ extern "C" GrB_Info GrB_Matrix_kronecker_BinaryOp(GrB_Matrix C, const GrB_Matrix
     if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || !gb_valid_matrix(B) || (Mask && !gb_valid_matrix(Mask)) || op->magic != GB_MAGIC)
         return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid object", fn);
     std::string *err = &C->err;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER)) return gb_fail(GrB_INVALID_VALUE, err, "%s: user-defined operators cannot run on the GPU", fn);
+    GB_TRY(gb_refuse_positional(op, fn));
     const DescFlags f = desc_flags(desc);
     const uint64_t am = f.tran0 ? A->ncols : A->nrows, an = f.tran0 ? A->nrows : A->ncols;
     const uint64_t bm = f.tran1 ? B->ncols : B->nrows, bn = f.tran1 ? B->nrows : B->ncols;
@@ -636,6 +640,7 @@ extern "C" GrB_Info GrB_Matrix_assign(GrB_Matrix C, const GrB_Matrix Mask, const
     if (!C || !A) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL argument", fn);
     if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || (Mask && !gb_valid_matrix(Mask))) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid object", fn);
     std::string *err = &C->err;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, err, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (Mask && (Mask->nrows != C->nrows || Mask->ncols != C->ncols)) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: the mask must have C's dimensions", fn);
     const DescFlags f = desc_flags(desc);

@@ -110,6 +110,7 @@ extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const
     const char *fn = "GxB_Matrix_select";
     GB_MAT_OK(C, fn); GB_MAT_OK(A, fn);
     if (Mask) GB_MAT_OK(Mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     std::string *err = &C->err;
     const DescFlags f = desc_flags(desc);
@@ -146,6 +147,7 @@ extern "C" GrB_Info GxB_Vector_select(GrB_Vector w, const GrB_Vector mask, const
     const char *fn = "GxB_Vector_select";
     GB_VEC_OK(w, fn); GB_VEC_OK(u, fn);
     if (mask) GB_VEC_OK(mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (w->n != u->n || (mask && mask->n != w->n)) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: dimensions do not match", fn);
     SelectArgs a{};
@@ -177,6 +179,7 @@ static GrB_Info mat_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
                           const GrB_Matrix A, const GrB_Descriptor desc, const char *fn) {
     GB_MAT_OK(C, fn); GB_MAT_OK(A, fn);
     if (Mask) GB_MAT_OK(Mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     std::string *err = &C->err;
     const DescFlags f = desc_flags(desc);
@@ -187,7 +190,11 @@ static GrB_Info mat_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     Csr T; GB_TRY(new_pattern_like(*src, (size_t)tc_size(ztc), T, err));
     ApplyArgs a{};
     a.nnz = src->nnz; a.aval = src->val; a.atc = A->type->code; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar; a.tval = T.val;
-    if (a.nnz > 0) { mat_apply_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    if (mode == AP_UNARY ? uop_is_positional(opcode) : op_is_positional(opcode)) {
+        // POSITIONI / J, and FIRSTI ... SECONDJ1 bound to a scalar (the scalar is ignored): the row or column of each entry of op(A)
+        const PosOp p = mode == AP_UNARY ? pos_unop(opcode) : pos_binop(opcode);
+        GB_TRY(pos_csr_values(T.val, ztc, nullptr, OP_ANY, *src, p.col, nullptr, p.off, err));
+    } else if (a.nnz > 0) { mat_apply_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), ztc, false, err);
 }
@@ -227,6 +234,7 @@ static GrB_Info mat_reduce_scalar(void *c, int ctc, const GrB_BinaryOp accum, co
     GB_MAT_OK(A, fn);
     if (monoid->magic != GB_MAGIC) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid monoid", fn);
     const GrB_BinaryOp op = monoid->op;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER)) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined operators cannot run on the GPU", fn);
     GB_TRY(matrix_ensure_device(A));
     const int mtc = op->ztype->code;
@@ -267,7 +275,9 @@ static GrB_Info mat_reduce_vector(GrB_Vector w, const GrB_Vector mask, const GrB
     if (mask) GB_VEC_OK(mask, fn);
     if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL operator", fn);
     if (op->magic != GB_MAGIC) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid operator", fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER)) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined operators cannot run on the GPU", fn);
+    GB_TRY(gb_refuse_positional(op, fn));
     const DescFlags f = desc_flags(desc);
     const uint64_t rows = f.tran0 ? A->ncols : A->nrows;
     if (w->n != rows || (mask && mask->n != rows)) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: dimensions do not match", fn);
@@ -332,7 +342,9 @@ static GrB_Info mat_ewise(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     if (Mask) GB_MAT_OK(Mask, fn);
     if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL operator", fn);
     if (op->magic != GB_MAGIC || (accum && accum->magic != GB_MAGIC)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid operator", fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER)) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined operators cannot run on the GPU", fn);
+    GB_TRY(gb_refuse_positional(op, fn));
     std::string *err = &C->err;
     const DescFlags f = desc_flags(desc);
     const uint64_t an = f.tran0 ? A->ncols : A->nrows, am = f.tran0 ? A->nrows : A->ncols;
@@ -362,6 +374,7 @@ static GrB_Info mat_ewise(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
 #define GB_MAT_EWISE(NAME, KIND, OPEXPR, MULT) \
     extern "C" GrB_Info NAME(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const KIND op, const GrB_Matrix A, const GrB_Matrix B, const GrB_Descriptor desc) { \
         GB_LOCK; GB_CHECK_INIT; if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, #NAME ": NULL operator"); \
+        GB_TRY(gb_refuse_positional(op, #NAME)); \
         return mat_ewise(C, Mask, accum, OPEXPR, A, B, desc, MULT, #NAME); }
 GB_MAT_EWISE(GrB_Matrix_eWiseAdd_BinaryOp, GrB_BinaryOp, op, 0)
 GB_MAT_EWISE(GrB_Matrix_eWiseAdd_Monoid, GrB_Monoid, op->op, 0)

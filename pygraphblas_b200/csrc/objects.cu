@@ -795,6 +795,7 @@ static GrB_Info check_dup_op(GrB_BinaryOp dup, std::string *err) {
     if (!dup) return GrB_SUCCESS;
     if (!valid_binop(dup)) return gb_fail(GrB_UNINITIALIZED_OBJECT, err, "build: bad dup operator");
     if (dup->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, err, "build: user-defined dup operators (host function pointers) are not supported");
+    GB_TRY(gb_refuse_positional(dup, "build"));
     if (op_is_cmp(dup->opcode) && dup->xtype->code != TC_BOOL) return gb_fail(GrB_DOMAIN_MISMATCH, err, "build: dup operator must have one domain");
     return GrB_SUCCESS;
 }

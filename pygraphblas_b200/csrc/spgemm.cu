@@ -1056,33 +1056,17 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     return GrB_SUCCESS;
 }
 
-extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring semiring,
-                            const GrB_Matrix A, const GrB_Matrix B, const GrB_Descriptor desc) {
-    GB_LOCK; GB_CHECK_INIT;
-    if (!C || !semiring || !A || !B) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_mxm: NULL argument");
-    if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || !gb_valid_matrix(B) || (Mask && !gb_valid_matrix(Mask)) || semiring->magic != GB_MAGIC)
-        return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GrB_mxm: invalid object");
-    std::string *err = &C->err;
-    if (gb_hyper_matrix(A) || gb_hyper_matrix(B) || gb_hyper_matrix(C)) return hyper_mxm(C, Mask, accum, semiring, A, B, desc);
-    const DescFlags f = desc_flags(desc);
-    const GrB_BinaryOp mulop = semiring->mul, addop = semiring->add->op;
-    if (mulop->opcode == OP_USER || addop->opcode == OP_USER || (accum && accum->opcode == OP_USER))
-        return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: user-defined operators are host function pointers and cannot run on the GPU (no CPU fallback)");
-    const uint64_t am = f.tran0 ? A->ncols : A->nrows, ak = f.tran0 ? A->nrows : A->ncols;
-    const uint64_t bk = f.tran1 ? B->ncols : B->nrows, bn = f.tran1 ? B->nrows : B->ncols;
-    if (ak != bk || C->nrows != am || C->ncols != bn || (Mask && (Mask->nrows != am || Mask->ncols != bn)))
-        return gb_fail(GrB_DIMENSION_MISMATCH, err, "GrB_mxm: dimensions do not match (op(A) %llux%llu, op(B) %llux%llu, C %llux%llu)",
-                       (unsigned long long)am, (unsigned long long)ak, (unsigned long long)bk, (unsigned long long)bn,
-                       (unsigned long long)C->nrows, (unsigned long long)C->ncols);
-    if (!G.have_device) return gb_fail(GrB_PANIC, err, "GrB_mxm: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
-    const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
-    const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
-    GbBurble burble("GrB_mxm");
-    G.last_kernel.clear();
-    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
+// Values one operand gets in place of its own (the inner form of a positional multiply): side 1 = each entry of op(A) its column
+// index, side 2 = each entry of op(B) its row index; through ids (hypersparse operands) when given, plus off, of type tc
+struct MxmPos { int side = 0; int tc = 0; int64_t off = 0; const uint64_t *ids = nullptr; };
 
+// T = op(A) (+).(x) op(B), masked by Mask when it is not complemented (*masked tells the write-back)
+static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, int zt, int add, int mul, const GrB_Matrix A, const GrB_Matrix B,
+                            const MxmPos &pos, Csr &T, bool *masked, std::string *err) {
+    const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
     // masked methods apply to non-complemented masks
     const bool use_mask = Mask && !f.mask_comp;
+    *masked = use_mask;
     if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
     GB_TRY(matrix_ensure_device(B));
     // C<M> = A*B': small problems intersect rows of A and B directly (no transpose); large ones
@@ -1097,15 +1081,93 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
 
     DevBuf<void> a_cast, b_cast;
     const void *aval = a.val, *bval = b.val;
-    if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
-    if (need_b && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
+    if (pos.side == 1) {
+        GB_TRY(a_cast.alloc((size_t)a.nnz * tc_size(pos.tc) + 16, err));
+        GB_TRY(pos_csr_values(a_cast, pos.tc, nullptr, OP_ANY, a, /*by_col=*/true, pos.ids, pos.off, err));
+        aval = a_cast;
+    } else if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
+    if (pos.side == 2) {
+        // op(B)'s row index: the row of b, or its column when b is B itself standing for B' (the dot method)
+        GB_TRY(b_cast.alloc((size_t)b.nnz * tc_size(pos.tc) + 16, err));
+        GB_TRY(pos_csr_values(b_cast, pos.tc, nullptr, OP_ANY, b, /*by_col=*/f.tran1 && dot, pos.ids, pos.off, err));
+        bval = b_cast;
+    } else if (need_b && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
 
-    Csr T; GrB_Info r;
+    GrB_Info r;
     if (use_mask) r = spgemm_masked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, Mask->dev, Mask->type->code, f.mask_struct, dot, T, err);
     else r = spgemm_unmasked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, T, err);
     a_cast.reset(); b_cast.reset();
-    if (r != GrB_SUCCESS) return r;
-    return matrix_writeback(C, Mask, accum, f, std::move(T), zt, use_mask, err);
+    return r;
+}
+
+extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring semiring,
+                            const GrB_Matrix A, const GrB_Matrix B, const GrB_Descriptor desc) {
+    GB_LOCK; GB_CHECK_INIT;
+    if (!C || !semiring || !A || !B) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_mxm: NULL argument");
+    if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || !gb_valid_matrix(B) || (Mask && !gb_valid_matrix(Mask)) || semiring->magic != GB_MAGIC)
+        return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GrB_mxm: invalid object");
+    std::string *err = &C->err;
+    GB_TRY(gb_refuse_positional_accum(accum, "GrB_mxm"));
+    GB_TRY(gb_refuse_user_with_positional(semiring, accum, "GrB_mxm"));
+    if (gb_hyper_matrix(A) || gb_hyper_matrix(B) || gb_hyper_matrix(C)) return hyper_mxm(C, Mask, accum, semiring, A, B, desc);
+    const DescFlags f = desc_flags(desc);
+    const GrB_BinaryOp mulop = semiring->mul, addop = semiring->add->op;
+    if (mulop->opcode == OP_USER || addop->opcode == OP_USER || (accum && accum->opcode == OP_USER))
+        return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: user-defined operators are host function pointers and cannot run on the GPU (no CPU fallback)");
+    const uint64_t am = f.tran0 ? A->ncols : A->nrows, ak = f.tran0 ? A->nrows : A->ncols;
+    const uint64_t bk = f.tran1 ? B->ncols : B->nrows, bn = f.tran1 ? B->nrows : B->ncols;
+    if (ak != bk || C->nrows != am || C->ncols != bn || (Mask && (Mask->nrows != am || Mask->ncols != bn)))
+        return gb_fail(GrB_DIMENSION_MISMATCH, err, "GrB_mxm: dimensions do not match (op(A) %llux%llu, op(B) %llux%llu, C %llux%llu)",
+                       (unsigned long long)am, (unsigned long long)ak, (unsigned long long)bk, (unsigned long long)bn,
+                       (unsigned long long)C->nrows, (unsigned long long)C->ncols);
+    if (!G.have_device) return gb_fail(GrB_PANIC, err, "GrB_mxm: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
+    if (op_is_positional(mulop->opcode)) return positional_mxm(C, Mask, accum, semiring, A, B, f, nullptr, nullptr, nullptr);
+    const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
+    GbBurble burble("GrB_mxm");
+    G.last_kernel.clear();
+    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
+    Csr T; bool masked = false;
+    GB_TRY(mxm_product(Mask, f, xt, zt, add, mul, A, B, MxmPos(), T, &masked, err));
+    return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);
+}
+
+// C<Mask> = accum(C, op(A) (+).(x) op(B)) with a positional multiply (DESIGN.md section 3.5).  FIRSTJ / SECONDI give the inner index
+// k: the values of op(A) become their column index and the call runs on (+).FIRST, or those of op(B) their row index with
+// (+).SECOND, whichever operand has fewer entries.  FIRSTI / SECONDJ give the row i / column j of C: (+).PAIR in INT64 counts the
+// products of every entry under the same mask, and one kernel turns each count into the fold of that many copies of i or j.
+GrB_Info positional_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                        const GrB_Matrix B, const DescFlags &f, const uint64_t *ids_m, const uint64_t *ids_k, const uint64_t *ids_n) {
+    std::string *err = &C->err;
+    const PosOp p = pos_binop(s->mul->opcode);
+    const int zt = s->add->op->ztype->code, add = s->add->op->opcode;
+    GbBurble burble("GrB_mxm");
+    G.last_kernel.clear();
+    if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
+    Csr T; bool masked = false;
+    if (p.second != p.col) {
+        // ---- inner form: product = k (+ off)
+        GB_TRY(matrix_ensure_device(A)); GB_TRY(matrix_ensure_device(B));
+        MxmPos pos; pos.tc = zt; pos.off = p.off; pos.ids = ids_k;
+        pos.side = A->dev.nnz <= B->dev.nnz ? 1 : 2;
+        const int mul = pos.side == 1 ? OP_FIRST : OP_SECOND;
+        GB_TRY(mxm_product(Mask, f, zt, zt, add, mul, A, B, pos, T, &masked, err));
+        gb_kernel_used("positional=inner");
+        gb_kernel_used(pos.side == 1 ? "positional-operand=A" : "positional-operand=B");
+        return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);
+    }
+    // ---- count form: product = i (FIRSTI) or j (SECONDJ), + off
+    const bool idem = add == OP_MIN || add == OP_MAX || add == OP_ANY;       // the count is not needed, only the pattern
+    GB_TRY(mxm_product(Mask, f, TC_INT64, TC_INT64, idem ? OP_ANY : OP_PLUS, OP_PAIR, A, B, MxmPos(), T, &masked, err));
+    if (!T.rowptr && T.nnz == 0) {      // an empty product may come without arrays
+        GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
+        CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
+    }
+    DevBuf<void> v;
+    GB_TRY(v.alloc((size_t)T.nnz * tc_size(zt) + 16, err));
+    GB_TRY(pos_csr_values(v, zt, (const int64_t *)T.val.get(), add, T, /*by_col=*/p.second, p.second ? ids_n : ids_m, p.off, err));
+    T.val = std::move(v);
+    gb_kernel_used("positional=count");
+    return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);
 }
 
 // C<M> = accum(C, A')  -- used by the reference around the hot path (Matrix.transpose,
@@ -1116,6 +1178,7 @@ extern "C" GrB_Info GrB_transpose(GrB_Matrix C, const GrB_Matrix Mask, const GrB
     if (!gb_valid_matrix(C) || !gb_valid_matrix(A) || (Mask && !gb_valid_matrix(Mask))) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GrB_transpose: invalid object");
     std::string *err = &C->err;
     const DescFlags f = desc_flags(desc);
+    GB_TRY(gb_refuse_positional_accum(accum, "GrB_transpose"));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, err, "GrB_transpose: user-defined accumulators cannot run on the GPU");
     const uint64_t tn = f.tran0 ? A->nrows : A->ncols, tm = f.tran0 ? A->ncols : A->nrows;
     if (C->nrows != tn || C->ncols != tm || (Mask && (Mask->nrows != tn || Mask->ncols != tm)))

@@ -485,28 +485,102 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     return vector_write(w, mask, accum, f, tval, tpres, zt, /*t_scalar=*/false, /*region=*/nullptr, std::move(t_val), std::move(t_pres));
 }
 
-static GrB_Info mxv_check(GrB_Vector w, const GrB_Vector mask, const GrB_Semiring s, const GrB_Matrix A, const GrB_Vector u, const char *fn) {
+// The value semiring the inner form runs on: the monoid of s, with FIRST (vxm) / SECOND (mxv) of the monoid's type
+static GB_Semiring_opaque value_semiring(const GrB_Semiring s, bool vxm) {
+    const bool i32 = s->add->op->ztype->code == TC_INT32;
+    const GrB_BinaryOp m = vxm ? (i32 ? GrB_FIRST_INT32 : GrB_FIRST_INT64) : (i32 ? GrB_SECOND_INT32 : GrB_SECOND_INT64);
+    return GB_Semiring_opaque{GB_MAGIC, s->add, m, s->name, true};
+}
+
+// w<mask> = accum(w, op(A) (+).(x) u) with a positional multiply (DESIGN.md section 3.5).  FIRSTJ / SECONDI give the inner index k:
+// u's values are replaced by k (a dense iota of the monoid type, u's presence kept) and the call runs on (+).SECOND (mxv) or
+// (+).FIRST (vxm), with A's plans as they are.  FIRSTI / SECONDJ give the output position (or 0): the number of products per
+// position comes from (+).PAIR in INT64 under the same mask, and one kernel turns it into the fold of that many copies.
+GrB_Info positional_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                        const GrB_Vector u, const DescFlags &f, bool vxm, const uint64_t *ids_in, const uint64_t *ids_out) {
+    const char *fn = vxm ? "GrB_vxm" : "GrB_mxv";
+    const bool use_transpose = vxm ? !f.tran1 : f.tran0;
+    std::string *err = &w->err;
+    const PosOp p = pos_binop(s->mul->opcode);
+    const int zt = s->add->op->ztype->code, add = s->add->op->opcode;
+    const uint64_t out_n = use_transpose ? A->ncols : A->nrows, in_n = use_transpose ? A->nrows : A->ncols;
+    if (u->n != in_n || w->n != out_n || (mask && mask->n != out_n))
+        return mxv_core(w, mask, accum, s, A, u, f, use_transpose, vxm, fn);           // reports the mismatch
+    if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
+    if (!mask && f.mask_comp) return mxv_core(w, mask, accum, s, A, u, f, use_transpose, vxm, fn);   // w<!NULL>: no product
+    if (p.second != p.col) {
+        // ---- inner form: product = k (+ off)
+        GB_TRY(vector_ensure_device(u));
+        DevBuf<void> iota; DevBuf<uint8_t> pres;
+        GB_TRY(iota.alloc((size_t)in_n * tc_size(zt) + 16, err));
+        GB_TRY(pos_vector_values(iota, zt, nullptr, OP_ANY, (int64_t)in_n, false, ids_in, p.off, err));
+        const uint8_t *upres = u->dpres;
+        if (upres && w == u) {      // T may be formed in w's buffers: the kernels must not read the presence they write
+            GB_TRY(pres.alloc((size_t)in_n, err));
+            CU_TRY(cudaMemcpyAsync(pres, upres, (size_t)in_n, cudaMemcpyDeviceToDevice, G.stream), err);
+            upres = pres;
+        }
+        GB_Vector_opaque k{};      // u with the values k: borrows its buffers, never freed through the vector
+        k.magic = GB_MAGIC; k.type = s->add->op->ztype; k.n = in_n; k.host_valid = false;
+        k.dval = iota; k.dpres = (uint8_t *)upres; k.dev_valid = true; k.dev_nvals = u->dev_nvals; k.borrowed = true;
+        GB_Semiring_opaque sr = value_semiring(s, vxm);
+        GB_TRY(mxv_core(w, mask, accum, &sr, A, &k, f, use_transpose, vxm, fn));
+        vector_mark_used(u);
+        gb_kernel_used("positional=inner");
+        return GrB_SUCCESS;
+    }
+    // ---- count form: product = the output position (mxv FIRSTI, vxm SECONDJ) or 0 (mxv SECONDJ, vxm FIRSTI), + off
+    const bool zero = vxm ? !p.second : p.second;
+    GrB_Vector t = nullptr;
+    GB_TRY(GrB_Vector_new(&t, GrB_INT64, out_n));
+    const bool idem = add == OP_MIN || add == OP_MAX || add == OP_ANY;     // the count is not needed, only the pattern
+    DescFlags fc = f; fc.replace = false;
+    GrB_Info r = mxv_core(t, mask, nullptr, idem ? GxB_ANY_PAIR_INT64 : GxB_PLUS_PAIR_INT64, A, u, fc, use_transpose, vxm, fn);
+    if (r == GrB_SUCCESS) r = vector_ensure_device(t);
+    // T = the values from the counts, with the counts' presence (its own copy: w may adopt T's buffers)
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    if (r == GrB_SUCCESS) r = tval.alloc((size_t)out_n * tc_size(zt) + 16, err);
+    if (r == GrB_SUCCESS) r = pos_vector_values(tval, zt, (const int64_t *)t->dval, add, (int64_t)out_n, zero, ids_out, p.off, err);
+    if (r == GrB_SUCCESS && t->dpres) {
+        r = tpres.alloc((size_t)out_n, err);
+        if (r == GrB_SUCCESS && cudaMemcpyAsync(tpres, t->dpres, (size_t)out_n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+            r = gb_fail(GrB_PANIC, err, "%s: copy of the count presence failed", fn);
+    }
+    if (r == GrB_SUCCESS) {
+        gb_kernel_used("positional=count");
+        void *tv = tval; uint8_t *tp = tpres;
+        r = vector_write(w, mask, accum, f, tv, tp, zt, false, nullptr, std::move(tval), std::move(tpres));
+    } else if (t->err.size()) *err = t->err;
+    GrB_Vector_free(&t);
+    return r;
+}
+
+static GrB_Info mxv_check(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A, const GrB_Vector u,
+                          const char *fn) {
     if (!w || !s || !A || !u) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL argument", fn);
     if (!gb_valid_vector(w) || !gb_valid_vector(u) || !gb_valid_matrix(A) || (mask && !gb_valid_vector(mask)) || s->magic != GB_MAGIC)
         return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid object", fn);
-    return GrB_SUCCESS;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
+    return gb_refuse_user_with_positional(s, accum, fn);
 }
 
 extern "C" GrB_Info GrB_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Semiring semiring,
                             const GrB_Matrix A, const GrB_Vector u, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
-    GB_TRY(mxv_check(w, mask, semiring, A, u, "GrB_mxv"));
+    GB_TRY(mxv_check(w, mask, accum, semiring, A, u, "GrB_mxv"));
     if (gb_hyper_matrix(A) || gb_hyper_vector(u) || gb_hyper_vector(w)) return hyper_mxv(w, mask, accum, semiring, A, u, desc, false);
     const DescFlags f = desc_flags(desc);
+    if (op_is_positional(semiring->mul->opcode)) return positional_mxv(w, mask, accum, semiring, A, u, f, false, nullptr, nullptr);
     return mxv_core(w, mask, accum, semiring, A, u, f, /*use_transpose=*/f.tran0, /*flip=*/false, "GrB_mxv");
 }
 
 extern "C" GrB_Info GrB_vxm(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Semiring semiring,
                             const GrB_Vector u, const GrB_Matrix A, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
-    GB_TRY(mxv_check(w, mask, semiring, A, u, "GrB_vxm"));
+    GB_TRY(mxv_check(w, mask, accum, semiring, A, u, "GrB_vxm"));
     if (gb_hyper_matrix(A) || gb_hyper_vector(u) || gb_hyper_vector(w)) return hyper_mxv(w, mask, accum, semiring, A, u, desc, true);
     const DescFlags f = desc_flags(desc);
+    if (op_is_positional(semiring->mul->opcode)) return positional_mxv(w, mask, accum, semiring, A, u, f, true, nullptr, nullptr);
     // w' = u'A  <=>  w = A'u: pull along the rows of A' (INP1 = TRAN cancels the transpose)
     return mxv_core(w, mask, accum, semiring, A, u, f, /*use_transpose=*/!f.tran1, /*flip=*/true, "GrB_vxm");
 }

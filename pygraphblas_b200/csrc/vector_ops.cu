@@ -211,6 +211,7 @@ __global__ void vec_ewise_kernel(const EwiseArgs a) {
 static GrB_Info binop_ok(const GrB_BinaryOp op, const GrB_BinaryOp accum, const char *fn) {
     if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: NULL operator", fn);
     if (op->magic != GB_MAGIC || (accum && accum->magic != GB_MAGIC)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid operator", fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER))
         return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined operators are host function pointers and cannot run on the GPU", fn);
     return GrB_SUCCESS;
@@ -221,6 +222,7 @@ static GrB_Info vec_ewise(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     GB_VEC_OK(w, fn); GB_VEC_OK(u, fn); GB_VEC_OK(v, fn);
     if (mask) GB_VEC_OK(mask, fn);
     GB_TRY(binop_ok(op, accum, fn));
+    GB_TRY(gb_refuse_positional(op, fn));
     if (u->n != v->n || w->n != u->n || (mask && mask->n != w->n)) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: dimensions do not match", fn);
     GB_NEED_DEVICE(w, fn);
     GB_TRY(vector_ensure_device(u)); GB_TRY(vector_ensure_device(v));
@@ -250,6 +252,7 @@ extern "C" GrB_Info GrB_Vector_eWiseAdd_Semiring(GrB_Vector w, const GrB_Vector 
                                                   const GrB_Vector u, const GrB_Vector v, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
     if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_Vector_eWiseAdd_Semiring: NULL semiring");
+    GB_TRY(gb_refuse_positional(op, "GrB_Vector_eWiseAdd_Semiring"));
     return vec_ewise(w, mask, accum, op->add->op, u, v, desc, EW_ADD, "GrB_Vector_eWiseAdd_Semiring");
 }
 extern "C" GrB_Info GrB_Vector_eWiseMult_BinaryOp(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_BinaryOp op,
@@ -267,6 +270,7 @@ extern "C" GrB_Info GrB_Vector_eWiseMult_Semiring(GrB_Vector w, const GrB_Vector
                                                    const GrB_Vector u, const GrB_Vector v, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
     if (!op) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_Vector_eWiseMult_Semiring: NULL semiring");
+    GB_TRY(gb_refuse_positional(op, "GrB_Vector_eWiseMult_Semiring"));
     return vec_ewise(w, mask, accum, op->mul, u, v, desc, EW_MULT, "GrB_Vector_eWiseMult_Semiring");
 }
 
@@ -275,6 +279,7 @@ static GrB_Info vec_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
                           const GrB_Vector u, const GrB_Descriptor desc, const char *fn) {
     GB_VEC_OK(w, fn); GB_VEC_OK(u, fn);
     if (mask) GB_VEC_OK(mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (w->n != u->n || (mask && mask->n != w->n)) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: dimensions do not match", fn);
     GB_NEED_DEVICE(w, fn);
@@ -287,7 +292,12 @@ static GrB_Info vec_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     GB_TRY(tval.alloc((size_t)n * tc_size(ztc) + 16, &w->err));
     if (u->dpres) GB_TRY(tpres.alloc((size_t)n, &w->err));
     a.tval = tval; a.tpres = tpres;
-    vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    if (mode == EW_UNARY ? uop_is_positional(opcode) : op_is_positional(opcode)) {
+        // a vector is a column: position k is (k, 0), so the row operators give k and the column ones 0; T keeps u's presence
+        const PosOp p = mode == EW_UNARY ? pos_unop(opcode) : pos_binop(opcode);
+        GB_TRY(pos_vector_values(tval, ztc, nullptr, OP_ANY, n, p.col, nullptr, p.off, &w->err));
+        if (u->dpres) CU_TRY(cudaMemcpyAsync(tpres, u->dpres, (size_t)n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
+    } else { vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, ztc, false, nullptr, std::move(tval), std::move(tpres));
 }
 extern "C" GrB_Info GrB_Vector_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_UnaryOp op, const GrB_Vector u, const GrB_Descriptor desc) {
@@ -333,7 +343,7 @@ GrB_Info index_list(const GrB_Index *I, GrB_Index ni, uint64_t dim, bool *all, s
     if (out.size() == dim) { bool iota = true; for (uint64_t k = 0; k < dim && iota; ++k) iota = out[k] == k; if (iota) { *all = true; out.clear(); } }
     return GrB_SUCCESS;
 }
-static GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err) {
+GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err) {
     GB_TRY(d.alloc(idx.size(), err));
     CU_TRY(cudaMemcpyAsync(d, idx.data(), idx.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);          // idx is a caller-owned temporary
@@ -365,6 +375,7 @@ static GrB_Info vec_assign_scalar(GrB_Vector w, const GrB_Vector mask, const GrB
                                   const GrB_Descriptor desc, const char *fn) {
     GB_VEC_OK(w, fn);
     if (mask) GB_VEC_OK(mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (mask && mask->n != w->n) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: mask dimension does not match", fn);
     bool all; std::vector<uint64_t> idx;
@@ -397,6 +408,7 @@ extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const
     const char *fn = "GrB_Vector_assign";
     GB_VEC_OK(w, fn); GB_VEC_OK(u, fn);
     if (mask) GB_VEC_OK(mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (mask && mask->n != w->n) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: mask dimension does not match", fn);
     bool all; std::vector<uint64_t> idx;
@@ -431,6 +443,7 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
     const char *fn = "GrB_Vector_extract";
     GB_VEC_OK(w, fn); GB_VEC_OK(u, fn);
     if (mask) GB_VEC_OK(mask, fn);
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (accum && accum->opcode == OP_USER) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined accumulators cannot run on the GPU", fn);
     if (mask && mask->n != w->n) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: mask dimension does not match", fn);
     if (I && I != GrB_ALL && ni == GxB_RANGE && I[0] <= I[1] && I[1] < u->n && I[1] - I[0] + 1 == w->n && w != u && G.have_device) {
@@ -523,6 +536,7 @@ static GrB_Info vec_reduce(void *c, int ctc, const GrB_BinaryOp accum, const GrB
     GB_VEC_OK(u, fn);
     if (monoid->magic != GB_MAGIC) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid monoid", fn);
     const GrB_BinaryOp op = monoid->op;
+    GB_TRY(gb_refuse_positional_accum(accum, fn));
     if (op->opcode == OP_USER || (accum && accum->opcode == OP_USER)) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: user-defined operators cannot run on the GPU", fn);
     GB_TRY(vector_ensure_device(u));
     const int mtc = op->ztype->code;

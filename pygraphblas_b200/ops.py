@@ -144,7 +144,8 @@ def get_bin_op(op, typ):
 
 _binop_re = re.compile(rf"^(?:GrB|GxB)_([A-Z0-9]+)_({_T})$")
 _monoid_res = (re.compile(rf"^GxB_([A-Z]+)_({_T})_MONOID$"), re.compile(rf"^GrB_([A-Z]+)_MONOID_({_T})$"))
-_semiring_re = re.compile(rf"^(?:GrB|GxB)_([A-Z]+)_([A-Z]+)_(?:SEMIRING_)?({_T})$")
+# the multiply may carry a digit: the positional semirings MIN_FIRSTI1 ... TIMES_SECONDJ1 (semiring.py:87-93 of the reference)
+_semiring_re = re.compile(rf"^(?:GrB|GxB)_([A-Z]+)_([A-Z][A-Z0-9]*)_(?:SEMIRING_)?({_T})$")
 _skip_binop_prefix = ("Matrix", "Vector", "Monoid", "DESC", "ONEB")
 
 binaryops, monoids, semirings, unaryops = {}, {}, {}, {}

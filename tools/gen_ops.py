@@ -56,6 +56,13 @@ for op in ["LOR", "LAND", "LXOR"]:
 add_binop("GrB_LXNOR", "EQ", "BOOL", "BOOL")
 for t in ALL:  # v2.0 name of PAIR; harmless extra
     add_binop(f"GrB_ONEB_{t}", "PAIR", t, t)
+# positional operators (SuiteSparse v4 names, INT32 / INT64 only): z is an index of where x / y sit, their values are never
+# read.  x = y = z = the index type, so that the object has no NULL type (the reference prints only the ztype).
+POSITIONAL = ["FIRSTI", "FIRSTI1", "FIRSTJ", "FIRSTJ1", "SECONDI", "SECONDI1", "SECONDJ", "SECONDJ1"]
+POS_T = ["INT32", "INT64"]
+for t in POS_T:
+    for op in POSITIONAL:
+        add_binop(f"GxB_{op}_{t}", op, t, t)
 
 monoids = []     # (symbol, op, type)
 monoid_sym = {}  # (op, type) -> canonical symbol
@@ -98,6 +105,9 @@ for t in FLOATS:
         unops.append((f"GxB_{op}_{t}", op, t, t))
     for op in ["ISINF", "ISNAN", "ISFINITE"]:
         unops.append((f"GxB_{op}_{t}", op, t, "BOOL"))
+for t in POS_T:
+    for op in ["POSITIONI", "POSITIONI1", "POSITIONJ", "POSITIONJ1"]:
+        unops.append((f"GxB_{op}_{t}", op, t, t))
 
 semirings = []   # (symbol, add op, add type, mul op, mul xtype)
 
@@ -131,6 +141,10 @@ for t in NONBOOL:
 for name, a, m in [("LOR_LAND", "LOR", "LAND"), ("LAND_LOR", "LAND", "LOR"),
                    ("LXOR_LAND", "LXOR", "LAND"), ("LXNOR_LOR", "EQ", "LOR")]:
     add_semiring(f"GrB_{name}_SEMIRING_BOOL", a, "BOOL", m, "BOOL")
+for t in POS_T:
+    for a in ["MIN", "MAX", "ANY", "PLUS", "TIMES"]:
+        for m in POSITIONAL:
+            add_semiring(f"GxB_{a}_{m}_{t}", a, t, m, t)
 
 
 def main():

@@ -204,6 +204,16 @@ GrB_Info B200_Matrix_import_CSR(GrB_Matrix *A, GrB_Type type, GrB_Index nrows, G
 /* Ap must hold nrows+1, Aj/Ax nvals entries; any pointer may be NULL to skip it.
  * Rows are sorted by column. */
 GrB_Info B200_Matrix_export_CSR(const GrB_Matrix A, int64_t *Ap, uint32_t *Aj, void *Ax, int where);
+/* dense matrix import: x[nrows*ncols] row-major values of `type`; present[nrows*ncols] bytes, entry (i,j) present where
+ * present[i*ncols+j] != 0, or NULL when every entry is present.  where = 0 or 1.  The matrix holds the dense form in HBM
+ * (GxB_SPARSITY_STATUS reports GxB_FULL without presence bytes, GxB_BITMAP with them); GrB_mxm with it as the
+ * untransposed B runs the dense-operand kernel, and every other operation sees its CSR, built on first use.
+ * nrows*ncols must be at most 2^31-1 (GrB_INVALID_VALUE otherwise). */
+GrB_Info B200_Matrix_import_dense(GrB_Matrix *A, GrB_Type type, GrB_Index nrows, GrB_Index ncols,
+                                  const void *x, const uint8_t *present, int where);
+/* dense matrix export of any matrix: x[nrows*ncols] row-major values (0 where absent), present[nrows*ncols] bytes (1 / 0);
+ * either pointer may be NULL to skip it.  where = 0 or 1; returns once the data is in place. */
+GrB_Info B200_Matrix_export_dense(const GrB_Matrix A, void *x, uint8_t *present, int where);
 /* dense import: every position present (present == NULL) or present[i] != 0 */
 GrB_Info B200_Vector_import_dense(GrB_Vector *v, GrB_Type type, GrB_Index n,
                                   const void *x, const uint8_t *present, int where);

@@ -91,6 +91,7 @@ public:
     template <typename U> explicit operator U *() const { return (U *)p_; }
     T *release() { T *q = p_; p_ = nullptr; return q; }
     void reset() { dfree(p_); p_ = nullptr; }
+    void adopt(T *p) { reset(); p_ = p; }     // takes a dmalloc block handed over as a raw pointer (vector_write's result)
 };
 
 // SpMV tile plan (spmv.cu): first row of every TILE-sized slice of the nnz range
@@ -150,6 +151,16 @@ struct Csr : CsrFields {
 // layout (always CSR by row / dense + presence) -- the API is format-agnostic, results do not depend on them
 struct GBObjOpts { double hyper = 0.0625; int format = 0 /* GxB_BY_ROW */; int sparsity = 15 /* GxB_AUTO_SPARSITY */; };
 
+// Dense device form of a matrix (DESIGN.md section 3.6): nrows x ncols values of the matrix type, row-major, and one presence byte
+// per entry (pres NULL: every entry present).  Only B200_Matrix_import_dense and the SpMM result of GrB_mxm create one.  While it
+// is held it is authoritative: the CSR and the host tuples beside it are caches built from it on demand, and any modification
+// drops it (matrix_invalidate_device).  nrows * ncols <= 2^31-1, so the flattened form is a legal vector.
+struct DenseForm {
+    DevBuf<void> val;
+    DevBuf<uint8_t> pres;
+    bool valid = false;
+};
+
 struct GB_Matrix_opaque {
     int magic; GrB_Type type; uint64_t nrows, ncols;
     GBObjOpts opts;
@@ -159,6 +170,7 @@ struct GB_Matrix_opaque {
     std::vector<uint64_t> pi, pj; std::vector<uint8_t> px;
     // device form (+ cached transpose)
     Csr dev, devT;
+    DenseForm dn;
     std::string err;
 };
 
@@ -254,6 +266,8 @@ GrB_Info matrix_ensure_device(GrB_Matrix A);
 GrB_Info matrix_ensure_transpose(GrB_Matrix A);     // builds A->devT on the device
 void matrix_invalidate_device(GrB_Matrix A);
 void matrix_adopt_device(GrB_Matrix A, Csr &&c);    // A takes ownership of c, host form dropped
+void matrix_adopt_dense(GrB_Matrix A, DevBuf<void> &&val, DevBuf<uint8_t> &&pres);   // A takes a dense form, every other form dropped
+bool matrix_known_empty(const GrB_Matrix A);        // A has no entries, as far as can be told without reading the device
 GrB_Info vector_ensure_host(GrB_Vector v);
 GrB_Info vector_ensure_device(GrB_Vector v);
 void vector_invalidate_device(GrB_Vector v);
@@ -320,6 +334,13 @@ GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err);
 GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int from_code, int64_t n, std::string *err);
 GrB_Info dev_count_present(const uint8_t *pres, int64_t n, int64_t *count, std::string *err);
 GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err);     // host list -> device (vector_ops.cu)
+// dense form <-> CSR (spmm.cu).  dense_to_csr compacts the present entries (pres NULL: all) into c, rowptr32 included;
+// csr_to_dense scatters c into fresh zero-filled values and presence bytes
+GrB_Info dense_to_csr(const void *val, const uint8_t *pres, int64_t nrows, int64_t ncols, size_t vsize, Csr &c, std::string *err);
+GrB_Info csr_to_dense(const Csr &c, size_t vsize, DevBuf<void> &val, DevBuf<uint8_t> &pres, std::string *err);
+// C<Mask> = accum(C, op(A) (+).(x) B) for a dense-form B, not transposed, and a builtin non-positional semiring (spmm.cu)
+GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                  const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
 
 // ---------------------------------------------------------------- scalar carrier
 // A value of any builtin type held in 64 bits: BOOL/UINT* in .u, INT* in .i, FP* in .d

@@ -119,7 +119,8 @@ extern "C" GrB_Info GrB_Vector_resize(GrB_Vector v, GrB_Index n) {
 extern "C" GrB_Info GxB_Matrix_memoryUsage(size_t *size, const GrB_Matrix A) {
     if (!size) return gb_fail(GrB_NULL_POINTER, nullptr, "GxB_Matrix_memoryUsage: NULL");
     if (!gb_valid_matrix(A)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GxB_Matrix_memoryUsage: invalid matrix");
-    *size = sizeof(*A) + A->hi.size() * (16 + A->type->size) + (A->dev.valid ? (size_t)A->dev.nnz * (4 + A->type->size) + ((size_t)A->dev.nrows + 1) * 12 : 0);
+    *size = sizeof(*A) + A->hi.size() * (16 + A->type->size) + (A->dev.valid ? (size_t)A->dev.nnz * (4 + A->type->size) + ((size_t)A->dev.nrows + 1) * 12 : 0)
+          + (A->dn.valid ? (size_t)(A->nrows * A->ncols) * (A->type->size + (A->dn.pres ? 1 : 0)) : 0);
     return GrB_SUCCESS;
 }
 extern "C" GrB_Info GxB_Vector_memoryUsage(size_t *size, const GrB_Vector v) {
@@ -190,8 +191,16 @@ extern "C" GrB_Info GxB_Matrix_Option_set(GrB_Matrix A, GxB_Option_Field field, 
 }
 extern "C" GrB_Info GxB_Matrix_Option_get(GrB_Matrix A, GxB_Option_Field field, ...) {
     if (!gb_valid_matrix(A)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GxB_Matrix_Option_get: invalid matrix");
-    // host-only tuple form (no HBM CSR yet, or dimensions beyond 2^31) reports HYPERSPARSE, tests/test_matrix.py:555,570
-    va_list ap; va_start(ap, field); const GrB_Info r = object_option_get(A->opts, field, !A->dev.valid, ap); va_end(ap); return r;
+    // host-only tuple form (no HBM CSR yet, or dimensions beyond 2^31) reports HYPERSPARSE, tests/test_matrix.py:555,570;
+    // a dense form reports FULL (no presence bytes) or BITMAP
+    va_list ap; va_start(ap, field);
+    GrB_Info r;
+    if (field == GxB_SPARSITY_STATUS && A->dn.valid) {
+        int *out = va_arg(ap, int *);
+        if (out) { *out = A->dn.pres ? GxB_BITMAP : GxB_FULL; r = GrB_SUCCESS; }
+        else r = gb_fail(GrB_NULL_POINTER, nullptr, "Option_get: NULL");
+    } else r = object_option_get(A->opts, field, !A->dev.valid, ap);
+    va_end(ap); return r;
 }
 extern "C" GrB_Info GxB_Vector_Option_set(GrB_Vector v, GxB_Option_Field field, ...) {
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GxB_Vector_Option_set: invalid vector");

@@ -427,7 +427,7 @@ bool gb_valid_matrix(const GrB_Matrix A) { return A && A->magic == GB_MAGIC; }
 bool gb_valid_vector(const GrB_Vector v) { return v && v->magic == GB_MAGIC; }
 static const uint64_t DEV_DIM_MAX = ((uint64_t)1 << 31) - 1;   // 32-bit column / row ids in HBM
 
-void matrix_invalidate_device(GrB_Matrix A) { A->dev = Csr(); A->devT = Csr(); }
+void matrix_invalidate_device(GrB_Matrix A) { A->dev = Csr(); A->devT = Csr(); A->dn = DenseForm(); }
 // copies still running on the copy streams must finish before the compute stream frees (or overwrites) the buffers
 static void vector_join_copies(GrB_Vector v) {
     if (v->h2d_pending) { cudaStreamWaitEvent(G.stream, v->ev_h2d, 0); v->h2d_pending = false; }
@@ -447,6 +447,17 @@ void matrix_adopt_device(GrB_Matrix A, Csr &&c) {
     A->hi.clear(); A->hj.clear(); A->hx.clear(); A->hi.shrink_to_fit(); A->hj.shrink_to_fit(); A->hx.shrink_to_fit();
     A->pi.clear(); A->pj.clear(); A->px.clear();
     A->host_valid = false;
+}
+void matrix_adopt_dense(GrB_Matrix A, DevBuf<void> &&val, DevBuf<uint8_t> &&pres) {
+    matrix_invalidate_device(A);
+    A->dn.val = std::move(val); A->dn.pres = std::move(pres); A->dn.valid = true;
+    A->hi.clear(); A->hj.clear(); A->hx.clear(); A->hi.shrink_to_fit(); A->hj.shrink_to_fit(); A->hx.shrink_to_fit();
+    A->pi.clear(); A->pj.clear(); A->px.clear();
+    A->host_valid = false;
+}
+bool matrix_known_empty(const GrB_Matrix A) {
+    if (A->host_valid) return A->hi.empty() && A->pi.empty();
+    return A->dev.valid ? A->dev.nnz == 0 : !A->dn.valid;
 }
 void vector_adopt_device(GrB_Vector v, void *vals, uint8_t *pres) {
     vector_invalidate_device(v);
@@ -512,8 +523,9 @@ static GrB_Info vector_flush_pending(GrB_Vector v) {
 
 GrB_Info matrix_ensure_host(GrB_Matrix A) {
     if (A->host_valid) return matrix_flush_pending(A);
-    // HBM CSR -> host COO
+    // HBM CSR -> host COO (a dense form goes through its CSR)
     const Csr &c = A->dev;
+    if (!c.valid && A->dn.valid) GB_TRY(matrix_ensure_device(A));
     if (!c.valid) { A->host_valid = true; return GrB_SUCCESS; }
     const size_t sz = A->type->size;
     std::vector<int64_t> rp((size_t)c.nrows + 1);
@@ -536,6 +548,13 @@ GrB_Info matrix_ensure_device(GrB_Matrix A) {
     if (!G.have_device) return gb_fail(GrB_PANIC, &A->err, "no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
     if (A->host_valid) GB_TRY(matrix_flush_pending(A));
     if (A->dev.valid) return GrB_SUCCESS;
+    if (A->dn.valid) {      // the CSR of a dense form, built once and cached beside it
+        Csr c;
+        GB_TRY(dense_to_csr(A->dn.val, A->dn.pres, (int64_t)A->nrows, (int64_t)A->ncols, A->type->size, c, &A->err));
+        c.valid = true;
+        A->dev = std::move(c);
+        return GrB_SUCCESS;
+    }
     if (A->nrows > DEV_DIM_MAX || A->ncols > DEV_DIM_MAX)
         return gb_fail(GrB_INVALID_VALUE, &A->err, "matrix dimensions %llu x %llu exceed the 2^31-1 limit of the HBM CSR layout",
                        (unsigned long long)A->nrows, (unsigned long long)A->ncols);
@@ -657,6 +676,10 @@ extern "C" GrB_Info GrB_Matrix_free(GrB_Matrix *A) {
 #define GB_VECTOR_OK(v, fn) do { if (!(v)) return gb_fail(GrB_NULL_POINTER, nullptr, fn ": NULL vector"); \
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, fn ": invalid vector handle"); } while (0)
 
+static GrB_Info copy_dev(void *dst, const void *src, size_t bytes, std::string *err) {
+    if (bytes) CU_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, G.stream), err);
+    return GrB_SUCCESS;
+}
 static GrB_Info csr_clone(const Csr &a, size_t vsize, Csr &c, std::string *err) {
     c = Csr(); c.nrows = a.nrows; c.ncols = a.ncols; c.nnz = a.nnz;
     GB_TRY(c.rowptr.alloc((size_t)a.nrows + 1, err));
@@ -678,7 +701,16 @@ extern "C" GrB_Info GrB_Matrix_dup(GrB_Matrix *C, const GrB_Matrix A) {
     GB_MATRIX_OK(A, "GrB_Matrix_dup");
     GB_Matrix_opaque *m = new GB_Matrix_opaque();
     m->magic = GB_MAGIC; m->type = A->type; m->nrows = A->nrows; m->ncols = A->ncols;
-    if (A->host_valid) {
+    if (A->dn.valid) {      // the dense form is copied (the caches beside it are rebuilt on demand)
+        m->host_valid = false;
+        const size_t n = (size_t)(A->nrows * A->ncols);
+        GrB_Info r = m->dn.val.alloc(n * A->type->size + 16, &A->err);
+        if (r == GrB_SUCCESS && A->dn.pres) r = m->dn.pres.alloc(n, &A->err);
+        if (r == GrB_SUCCESS) r = copy_dev(m->dn.val, A->dn.val, n * A->type->size, &A->err);
+        if (r == GrB_SUCCESS && A->dn.pres) r = copy_dev(m->dn.pres, A->dn.pres, n, &A->err);
+        if (r != GrB_SUCCESS) { delete m; return r; }
+        m->dn.valid = true;
+    } else if (A->host_valid) {
         GrB_Info r = matrix_flush_pending(A);
         if (r != GrB_SUCCESS) { delete m; return r; }
         m->hi = A->hi; m->hj = A->hj; m->hx = A->hx; m->host_valid = true;
@@ -707,7 +739,9 @@ extern "C" GrB_Info GrB_Matrix_nvals(GrB_Index *n, const GrB_Matrix A) {
     GB_LOCK;
     if (!n) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_Matrix_nvals: NULL"); GB_MATRIX_OK(A, "GrB_Matrix_nvals");
     if (A->host_valid) { GB_TRY(matrix_flush_pending(A)); *n = A->hi.size(); }
-    else { if (G.have_device) CU_TRY(cudaStreamSynchronize(G.stream), &A->err); *n = (GrB_Index)A->dev.nnz; }
+    else if (A->dev.valid) { if (G.have_device) CU_TRY(cudaStreamSynchronize(G.stream), &A->err); *n = (GrB_Index)A->dev.nnz; }
+    else if (A->dn.pres) { int64_t c = 0; GB_TRY(dev_count_present(A->dn.pres, (int64_t)(A->nrows * A->ncols), &c, &A->err)); *n = (GrB_Index)c; }
+    else *n = A->dn.valid ? A->nrows * A->ncols : 0;
     return GrB_SUCCESS;
 }
 extern "C" GrB_Info GxB_Matrix_type(GrB_Type *t, const GrB_Matrix A) {
@@ -730,7 +764,7 @@ extern "C" GrB_Info GrB_Matrix_error(const char **error, const GrB_Matrix A) {
 
 static GrB_Info matrix_host_writable(GrB_Matrix A) {
     GB_TRY(matrix_ensure_host(A));
-    if (A->dev.valid || A->devT.valid) matrix_invalidate_device(A);
+    if (A->dev.valid || A->devT.valid || A->dn.valid) matrix_invalidate_device(A);
     return GrB_SUCCESS;
 }
 
@@ -1100,6 +1134,55 @@ extern "C" GrB_Info B200_Matrix_export_CSR(const GrB_Matrix A, int64_t *Ap, uint
     if (Ap) GB_TRY(copy_out(Ap, c.rowptr, ((size_t)c.nrows + 1) * 8, where, &A->err));
     if (Aj) GB_TRY(copy_out(Aj, c.col, (size_t)c.nnz * 4, where, &A->err));
     if (Ax) GB_TRY(copy_out(Ax, c.val, (size_t)c.nnz * A->type->size, where, &A->err));
+    CU_TRY(cudaStreamSynchronize(G.stream), &A->err);
+    return GrB_SUCCESS;
+}
+
+// the dense layout of an nrows x ncols matrix: each dimension and the flattened length within 2^31-1
+static GrB_Info dense_shape_ok(GrB_Index nrows, GrB_Index ncols, int where, const char *fn) {
+    if (where != 0 && where != 1) return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: where must be 0 (host) or 1 (device)", fn);
+    if (nrows > DEV_DIM_MAX || ncols > DEV_DIM_MAX || (ncols && nrows > DEV_DIM_MAX / ncols))
+        return gb_fail(GrB_INVALID_VALUE, nullptr, "%s: %llu x %llu entries exceed the 2^31-1 limit of the dense form", fn,
+                       (unsigned long long)nrows, (unsigned long long)ncols);
+    return GrB_SUCCESS;
+}
+extern "C" GrB_Info B200_Matrix_import_dense(GrB_Matrix *A, GrB_Type type, GrB_Index nrows, GrB_Index ncols,
+                                              const void *x, const uint8_t *present, int where) {
+    GB_LOCK; GB_CHECK_INIT;
+    if (!A || !x) return gb_fail(GrB_NULL_POINTER, nullptr, "B200_Matrix_import_dense: NULL argument");
+    GB_TRY(dense_shape_ok(nrows, ncols, where, "B200_Matrix_import_dense"));
+    if (!G.have_device) return gb_fail(GrB_PANIC, nullptr, "no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
+    GB_TRY(GrB_Matrix_new(A, type, nrows, ncols));
+    GrB_Matrix m = *A;
+    const size_t n = (size_t)(nrows * ncols), sz = type->size;
+    DevBuf<void> val; DevBuf<uint8_t> pres;
+    GrB_Info r = val.alloc(n * sz + 16, &m->err);
+    if (r == GrB_SUCCESS && present) r = pres.alloc(n, &m->err);
+    if (r == GrB_SUCCESS) r = copy_in(val, x, n * sz, where, &m->err);
+    if (r == GrB_SUCCESS && present) r = copy_in(pres, present, n, where, &m->err);
+    if (r == GrB_SUCCESS && !where && cudaStreamSynchronize(G.stream) != cudaSuccess) r = GrB_PANIC;
+    if (r != GrB_SUCCESS) { val.reset(); pres.reset(); GrB_Matrix_free(A); return r; }
+    matrix_adopt_dense(m, std::move(val), std::move(pres));
+    return GrB_SUCCESS;
+}
+extern "C" GrB_Info B200_Matrix_export_dense(const GrB_Matrix A, void *x, uint8_t *present, int where) {
+    GB_LOCK; GB_MATRIX_OK(A, "B200_Matrix_export_dense");
+    GB_TRY(dense_shape_ok(A->nrows, A->ncols, where, "B200_Matrix_export_dense"));
+    if (!G.have_device) return gb_fail(GrB_PANIC, &A->err, "no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
+    const size_t n = (size_t)(A->nrows * A->ncols), sz = A->type->size;
+    DevBuf<void> sval; DevBuf<uint8_t> spres;      // the dense image of a CSR-only matrix (not kept: A stays as it is)
+    const void *val = A->dn.val; const uint8_t *pres = A->dn.pres;
+    if (!A->dn.valid) {
+        GB_TRY(matrix_ensure_device(A));
+        GB_TRY(csr_to_dense(A->dev, sz, sval, spres, &A->err));
+        val = sval; pres = spres;
+    }
+    if (x) GB_TRY(copy_out(x, val, n * sz, where, &A->err));
+    if (present) {
+        if (pres) GB_TRY(copy_out(present, pres, n, where, &A->err));
+        else if (where) { if (n) CU_TRY(cudaMemsetAsync(present, 1, n, G.stream), &A->err); }
+        else memset(present, 1, n);
+    }
     CU_TRY(cudaStreamSynchronize(G.stream), &A->err);
     return GrB_SUCCESS;
 }

@@ -1033,7 +1033,7 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
         }
         return GrB_SUCCESS;
     }
-    const bool c_empty = C->host_valid ? (C->hi.empty() && C->pi.empty()) : (C->dev.nnz == 0);
+    const bool c_empty = matrix_known_empty(C);
     // fast exits: the result is exactly T
     const bool plain = !accum && (!Mask || (t_already_masked && (f.replace || c_empty)));
     if (plain || (accum && !Mask && c_empty)) {
@@ -1126,6 +1126,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     GbBurble burble("GrB_mxm");
     G.last_kernel.clear();
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
+    if (B->dn.valid && !f.tran1) return spmm_mxm(C, Mask, accum, semiring, A, B, f, burble);         // dense X: DESIGN.md section 3.6
     Csr T; bool masked = false;
     GB_TRY(mxm_product(Mask, f, xt, zt, add, mul, A, B, MxmPos(), T, &masked, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);

@@ -86,6 +86,37 @@ class Matrix:
         return cls(m)
 
     @classmethod
+    def from_numpy(cls, x, present=None, typ=None):
+        """Dense import of a 2-D array straight into HBM (B200 extension `B200_Matrix_import_dense`).  `present`
+        (same shape, nonzero = present) marks the entries; None means every entry is present."""
+        x = np.asarray(x)
+        if x.ndim != 2:
+            raise ValueError("from_numpy expects a 2-D array")
+        typ = typ or types._dtype_lookup(x.dtype)
+        x = np.ascontiguousarray(x, dtype=typ.dtype)
+        p = NULL
+        if present is not None:
+            present = np.ascontiguousarray(present, dtype=np.uint8)
+            if present.shape != x.shape:
+                raise ValueError("present must have the shape of x")
+            p = ffi.cast("uint8_t*", present.ctypes.data)
+        m = ffi.new("GrB_Matrix*")
+        _check(lib.B200_Matrix_import_dense(m, typ.gb_type, x.shape[0], x.shape[1], ffi.cast("void*", x.ctypes.data), p, 0))
+        return cls(m)
+
+    def to_numpy(self, out=None, present_out=None):
+        """(values, present) dense 2-D host arrays of any matrix (B200 extension `B200_Matrix_export_dense`); absent
+        entries read 0.  `out` / `present_out` are C-contiguous arrays of the matrix's shape to fill."""
+        shape = (self.nrows, self.ncols)
+        x = np.empty(shape, self.type.dtype) if out is None else out
+        p = np.empty(shape, np.uint8) if present_out is None else present_out
+        for a, dt in ((x, self.type.dtype), (p, np.uint8)):
+            if a.shape != shape or a.dtype != dt or not a.flags.c_contiguous:
+                raise ValueError(f"output arrays must be C-contiguous {dt} of shape {shape}")
+        _check(lib.B200_Matrix_export_dense(self._matrix[0], ffi.cast("void*", x.ctypes.data), ffi.cast("uint8_t*", p.ctypes.data), 0))
+        return x, p
+
+    @classmethod
     def from_mm(cls, mm_file):
         """Create a matrix from a Matrix-Market file (matrix.py:377-409 of the reference), parsed in bulk."""
         from .io import mm_read

@@ -1,0 +1,190 @@
+#!/usr/bin/env python
+"""GrB_mxm with a dense right operand (the SpMM path, DESIGN.md section 3.6) on the R-MAT graph of bench.py, against
+
+    (b) k back-to-back GrB_mxv calls of the same semiring, one per column of X
+    (c) the CSR GrB_mxm on the same X imported as CSR (at --scale-csr only: at scale 22 it sorts nnz(A) * k products)
+
+for FP32 PLUS_TIMES and MAX_PLUS and k in {8, 32, 128}.  Device times from CUDA events on the library's stream, medians of
+--reps calls after --warmup, the arms alternated in one process.  Outputs are checked: bit-equal across the arms on
+quarter-valued inputs, and within 1e-6 relative of an fp64 scipy reference on random FP32 (PLUS_TIMES).  The byte model is
+
+    nnz(A) (4 + b_A) + (m + 1) 4 + n k (b_X [+ 1 with presence]) + m k (b_C + 1)
+
+and the share of it is over the data sheet's 3.35 TB/s.  --profile prints one torch.profiler split of a call instead.
+
+    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile]"""
+import argparse
+import os
+import subprocess
+import sys
+
+import numpy as np
+import scipy.sparse as sp
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch
+import pygraphblas_b200 as gb
+from pygraphblas_b200 import FP32, Matrix, Vector
+from bench import cached_graph
+
+HBM_BPS = 3.35e12
+KS = (8, 32, 128)
+
+
+def lib_stream():
+    sp_ = gb.ffi.new("void**")
+    gb.lib.B200_get_stream(sp_)
+    return torch.cuda.ExternalStream(int(gb.ffi.cast("uintptr_t", sp_[0])))
+
+
+def time_once(stream, f):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    f()
+    e1.record(stream)
+    gb.lib.B200_device_synchronize()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1)
+
+
+def alternate(stream, arms, reps, warmup):
+    """Median ms of each arm, the arms interleaved call by call."""
+    for f in arms.values():
+        for _ in range(warmup):
+            f()
+    ts = {k: [] for k in arms}
+    for _ in range(reps):
+        for k, f in arms.items():
+            ts[k].append(time_once(stream, f))
+    return {k: float(np.median(v)) for k, v in ts.items()}
+
+
+def last_kernel():
+    return gb.ffi.string(gb.lib.B200_debug_last_kernel()).decode()
+
+
+def byte_model(nnz, m, n, k, b=4):
+    return nnz * (4 + b) + (m + 1) * 4 + n * k * b + m * k * (b + 1)
+
+
+def graph(scale, quarter, seed=2):
+    n, indptr, indices = cached_graph(scale)
+    rng = np.random.default_rng(seed)
+    nnz = len(indices)
+    vals = (rng.integers(1, 9, nnz) / 4.0).astype(np.float32) if quarter else (rng.random(nnz, dtype=np.float32) + np.float32(0.5))
+    return n, indptr, indices, vals
+
+
+def xblock(n, k, quarter, seed=3):
+    rng = np.random.default_rng(seed + k)
+    return (rng.integers(-4, 5, (n, k)) / 4.0).astype(np.float32) if quarter else rng.random((n, k), dtype=np.float32)
+
+
+def run_scale(stream, scale, with_csr, reps, warmup, out):
+    for quarter in (True, False):
+        n, indptr, indices, vals = graph(scale, quarter)
+        nnz = len(indices)
+        A = Matrix.from_csr(indptr, indices, vals, n, n, FP32)
+        S64 = sp.csr_matrix((vals.astype(np.float64), indices, indptr), shape=(n, n)) if not quarter else None
+        for semi in (FP32.PLUS_TIMES, FP32.MAX_PLUS):
+            if not quarter and semi is not FP32.PLUS_TIMES:
+                continue
+            for k in KS:
+                x = xblock(n, k, quarter)
+                X = Matrix.from_numpy(x)
+                cols = [Vector.from_numpy(np.ascontiguousarray(x[:, j])) for j in range(k)]
+                ws = [Vector.sparse(FP32, n) for _ in range(k)]
+                C = Matrix.sparse(FP32, n, k)
+                arms = {"spmm": lambda: A.mxm(X, semiring=semi, out=C),
+                        "mxv": lambda: [A.mxv(cols[j], semiring=semi, out=ws[j]) for j in range(k)]}
+                Xc = None
+                if with_csr and k <= 32:
+                    Xc = Matrix.from_csr(np.arange(0, n * k + 1, k, dtype=np.int64), np.tile(np.arange(k, dtype=np.uint32), n), x.reshape(-1), n, k, FP32)
+                    Cc = Matrix.sparse(FP32, n, k)
+                    arms["csr-mxm"] = lambda: A.mxm(Xc, semiring=semi, out=Cc)
+                t = alternate(stream, arms, reps if k < 128 or not with_csr else max(3, reps // 2), warmup)
+                A.mxm(X, semiring=semi, out=C)
+                kern = last_kernel()
+                # outputs
+                got, pres = C.to_numpy()
+                got = np.where(pres.astype(bool), got, np.float32(0))
+                mxv = np.zeros((n, k), np.float32); mxv_p = np.zeros((n, k), np.uint8)
+                for j in range(k):
+                    v, p = ws[j].to_numpy()
+                    mxv[:, j], mxv_p[:, j] = np.where(p.astype(bool), v, 0), p
+                check = {"presence_equal_mxv": bool(np.array_equal(pres, mxv_p))}
+                if quarter:
+                    check["bits_equal_mxv"] = bool(np.array_equal(got.view(np.uint32), mxv.view(np.uint32)))
+                    if Xc is not None:
+                        cx, cp = Cc.to_numpy()
+                        check["bits_equal_csr_mxm"] = bool(np.array_equal(cp, pres) and np.array_equal(np.where(cp.astype(bool), cx, 0).view(np.uint32), got.view(np.uint32)))
+                else:
+                    want = S64 @ x.astype(np.float64)
+                    nz = pres.astype(bool)
+                    rel = np.abs(got[nz] - want[nz]) / np.maximum(np.abs(want[nz]), 1e-300)
+                    check["max_rel_err_fp64_spmm"] = float(rel.max()) if rel.size else 0.0
+                    rel_b = np.abs(mxv[nz] - want[nz]) / np.maximum(np.abs(want[nz]), 1e-300)
+                    check["max_rel_err_fp64_mxv"] = float(rel_b.max()) if rel_b.size else 0.0
+                model = byte_model(nnz, n, n, k)
+                rec = {"scale": scale, "n": n, "nnz": nnz, "semiring": semi.name, "k": k, "inputs": "quarter" if quarter else "random",
+                       "ms": {a: round(v, 4) for a, v in t.items()}, "speedup_vs_mxv": round(t["mxv"] / t["spmm"], 2),
+                       "byte_model": model, "gather_bytes": nnz * k * 4, "share_of_hbm_model": round(model / HBM_BPS / (t["spmm"] * 1e-3), 3),
+                       "kernels": kern, "checks": check}
+                if "csr-mxm" in t:
+                    rec["speedup_vs_csr_mxm"] = round(t["csr-mxm"] / t["spmm"], 2)
+                print(rec, flush=True)
+                out.append(rec)
+                del arms, X, cols, ws, C, Xc
+        del A
+
+
+def profile_split(scale):
+    from torch.profiler import ProfilerActivity, profile
+    n, indptr, indices, vals = graph(scale, False)
+    A = Matrix.from_csr(indptr, indices, vals, n, n, FP32)
+    X = Matrix.from_numpy(xblock(n, 32, False))
+    M = Matrix.from_numpy((np.arange(n * 32).reshape(n, 32) % 3 == 0).astype(np.float32))
+    C = Matrix.from_numpy(np.ones((n, 32), np.float32))
+    f = lambda: A.mxm(X, semiring=FP32.PLUS_TIMES, out=C, mask=M, accum=FP32.PLUS)
+    f(); gb.lib.B200_device_synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        f(); gb.lib.B200_device_synchronize()
+    groups = {"prep": ("seg_", "scan_", "cast_", "narrow_"), "conversion": ("dense_", "csr_scatter"),
+              "spmm": ("spmm_kernel", "spmm_combine"), "write-back": ("vec_finalize",)}
+    split = {g: 0.0 for g in groups}; other = 0.0
+    for ev in prof.key_averages():
+        us = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+        for g, keys in groups.items():
+            if any(k in ev.key for k in keys):
+                split[g] += us
+                break
+        else:
+            other += us
+    print({"profile": f"scale {scale} k=32 FP32 PLUS_TIMES, dense mask and PLUS accumulator", "device_us": {**{g: round(v, 1) for g, v in split.items()}, "other": round(other, 1)},
+           "kernels": last_kernel()})
+    print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=12))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--scale", type=int, default=22)
+    ap.add_argument("--scale-csr", type=int, default=20)
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--profile", action="store_true")
+    a = ap.parse_args()
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True).stdout.strip()
+    print({"card": card})
+    stream = lib_stream()
+    if a.profile:
+        profile_split(a.scale)
+        return
+    out = []
+    run_scale(stream, a.scale, False, a.reps, a.warmup, out)
+    if a.scale_csr:
+        run_scale(stream, a.scale_csr, True, a.reps, a.warmup, out)
+
+
+if __name__ == "__main__":
+    main()

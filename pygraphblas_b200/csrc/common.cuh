@@ -341,6 +341,12 @@ GrB_Info csr_to_dense(const Csr &c, size_t vsize, DevBuf<void> &val, DevBuf<uint
 // C<Mask> = accum(C, op(A) (+).(x) B) for a dense-form B, not transposed, and a builtin non-positional semiring (spmm.cu)
 GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
                   const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
+// the multiply with its operands swapped, mirror(y, x) = op(x, y), by opcode; -1 when the library has none (POW)
+int op_mirror(int op);
+// C<Mask> = accum(C, op(A) (+).(x) op(B)) for a dense-form A, a B without one, a multiply with a mirror and a k x m C of at most
+// 2^31-1 entries (spmm.cu)
+GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                       const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
 
 // ---------------------------------------------------------------- scalar carrier
 // A value of any builtin type held in 64 bits: BOOL/UINT* in .u, INT* in .i, FP* in .d

@@ -1127,6 +1127,8 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     G.last_kernel.clear();
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
     if (B->dn.valid && !f.tran1) return spmm_mxm(C, Mask, accum, semiring, A, B, f, burble);         // dense X: DESIGN.md section 3.6
+    if (A->dn.valid && !B->dn.valid && op_mirror(mul) >= 0 && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))
+        return spmm_left_mxm(C, Mask, accum, semiring, A, B, f, burble);                            // dense X on the left
     Csr T; bool masked = false;
     GB_TRY(mxm_product(Mask, f, xt, zt, add, mul, A, B, MxmPos(), T, &masked, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);

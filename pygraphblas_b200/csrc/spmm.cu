@@ -9,6 +9,9 @@
 // each segment's partial goes to scratch and a second kernel folds the partials of a row pairwise in a fixed tree over the
 // segment order (deterministic, no atomics).  The result is written back through the vector write-back over the flattened m*k positions, so C keeps the
 // dense form; only a CSR mask sends T through the CSR write-back.
+//
+// A dense X on the left, C = X (+).(x) op(B), runs as C' = op(B)' (+).(x)' X' on the same kernels (spmm_left_mxm), with the
+// multiply's operands swapped and dense_transpose_kernel turning X into X' and T' into T.
 #include "common.cuh"
 #include "spmv_common.cuh"
 
@@ -87,6 +90,52 @@ GrB_Info dense_to_csr(const void *val, const uint8_t *pres, int64_t nrows, int64
     GB_TRY(dev_build_rowptr32(t, err));
     CU_TRY(cudaGetLastError(), err);
     c = std::move(t);
+    return GrB_SUCCESS;
+}
+
+// out (cols x rows) = in (rows x cols)', both row-major, presence bytes carried along (ipres NULL: no presence is written).
+// A CTA of 32 x 8 threads moves one 32 x 32 tile at a time through shared memory (one column of padding), so both the loads
+// and the stores run along rows; the CTAs stride over the tiles, so any rows * cols < 2^31 fits a capped grid.
+template <typename V>
+__global__ void __launch_bounds__(256) dense_transpose_kernel(const V *in, const uint8_t *ipres, int64_t rows, int64_t cols,
+                                                              V *out, uint8_t *opres) {
+    __shared__ V tv[32][33];
+    __shared__ uint8_t tp[32][33];
+    const int64_t tcols = ceil_div(cols, 32), ntiles = ceil_div(rows, 32) * tcols;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int64_t r0 = t / tcols * 32, c0 = t % tcols * 32;
+        for (int y = ty; y < 32; y += 8) {
+            const int64_t r = r0 + y, c = c0 + tx;
+            if (r < rows && c < cols) {
+                tv[y][tx] = in[r * cols + c];
+                if (ipres) tp[y][tx] = ipres[r * cols + c];
+            }
+        }
+        __syncthreads();
+        for (int y = ty; y < 32; y += 8) {
+            const int64_t c = c0 + y, r = r0 + tx;     // out(c, r) = in(r, c)
+            if (c < cols && r < rows) {
+                out[c * rows + r] = tv[tx][y];
+                if (ipres) opres[c * rows + r] = tp[tx][y];
+            }
+        }
+        __syncthreads();
+    }
+}
+
+static GrB_Info dense_transpose(const void *val,const uint8_t *pres, int64_t rows, int64_t cols, size_t vsize, void *oval, uint8_t *opres,
+                         std::string *err) {
+    if (rows == 0 || cols == 0) return GrB_SUCCESS;
+    const int grid = grid_for(ceil_div(rows, 32) * ceil_div(cols, 32), 1);
+    switch (vsize) {
+        case 1: dense_transpose_kernel<uint8_t><<<grid, 256, 0, G.stream>>>((const uint8_t *)val, pres, rows, cols, (uint8_t *)oval, opres); break;
+        case 2: dense_transpose_kernel<uint16_t><<<grid, 256, 0, G.stream>>>((const uint16_t *)val, pres, rows, cols, (uint16_t *)oval, opres); break;
+        case 4: dense_transpose_kernel<uint32_t><<<grid, 256, 0, G.stream>>>((const uint32_t *)val, pres, rows, cols, (uint32_t *)oval, opres); break;
+        default: dense_transpose_kernel<uint64_t><<<grid, 256, 0, G.stream>>>((const uint64_t *)val, pres, rows, cols, (uint64_t *)oval, opres); break;
+    }
+    GB_LAUNCHED();
+    CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
 
@@ -343,5 +392,76 @@ GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     const double bytes = (double)a.nnz * (4 + tc_size(A->type->code)) + (double)(m + 1) * 4 +
                          (double)(n * k) * (tc_size(B->type->code) + (B->dn.pres ? 1 : 0)) + (double)(m * k) * (tc_size(zt) + 1);
     burble.note("spmm", bytes);
+    return spmm_writeback(C, Mask, accum, f, std::move(tval), std::move(tpres), zt, err);
+}
+
+int op_mirror(int op) {
+    switch (op) {
+        case OP_FIRST: return OP_SECOND;   case OP_SECOND: return OP_FIRST;
+        case OP_ANY: return OP_FIRST;      // the device's ANY returns y, op(B)'s value: FIRST of the swapped operands
+        case OP_MINUS: return OP_RMINUS;   case OP_RMINUS: return OP_MINUS;
+        case OP_DIV: return OP_RDIV;       case OP_RDIV: return OP_DIV;
+        case OP_ISGT: return OP_ISLT;      case OP_ISLT: return OP_ISGT;
+        case OP_ISGE: return OP_ISLE;      case OP_ISLE: return OP_ISGE;
+        case OP_GT: return OP_LT;          case OP_LT: return OP_GT;
+        case OP_GE: return OP_LE;          case OP_LE: return OP_GE;
+        case OP_TIMES: case OP_PLUS: case OP_PAIR: case OP_MIN: case OP_MAX: case OP_ISEQ: case OP_ISNE: case OP_EQ: case OP_NE:
+        case OP_LOR: case OP_LAND: case OP_LXOR: case OP_BOR: case OP_BAND: case OP_BXOR: case OP_BXNOR: return op;
+        default: return -1;                // POW, positional, user-defined
+    }
+}
+
+// C<Mask> = accum(C, X (+).(x) op(B)) for a dense-form X = op(A) (k x n), as C' = op(B)' (+).(x)' X' on the kernel above, where
+// (x)' is the multiply with its operands swapped.  op(B)' is B's cached transpose, or B's own CSR under INP1 = TRAN; X' (n x k) is
+// A's dense form itself under INP0 = TRAN (or when k = 1), else its dense transpose, built per call.  T' (m x k) is transposed into
+// T (k x m) in fresh buffers (C may alias A or B), unless m = 1, and T goes through the right route's write-back.
+GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                       const GrB_Matrix B, const DescFlags &f, GbBurble &burble) {
+    std::string *err = &C->err;
+    const GrB_BinaryOp mulop = s->mul, addop = s->add->op;
+    const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = op_mirror(mulop->opcode);
+    gb_kernel_used("spmm");
+    gb_kernel_used("spmm-left");
+    if (f.tran1) GB_TRY(matrix_ensure_device(B)); else GB_TRY(matrix_ensure_transpose(B));
+    const Csr &b = f.tran1 ? B->dev : B->devT;
+    if (!b.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
+    const int64_t m = b.nrows, n = b.ncols, k = (int64_t)(f.tran0 ? A->ncols : A->nrows);
+    // operands cast to the multiply's input types, as in the CSR path: op(B)' takes the swapped multiply's x, X its y
+    DevBuf<void> b_cast, x_cast;
+    const void *bval = b.val, *xval = A->dn.val;
+    const uint8_t *xpres = A->dn.pres;
+    if (mul_reads_x(mul) && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
+    if (mul_reads_y(mul) && A->type->code != xt) { GB_TRY(dev_cast_values(x_cast, xt, A->dn.val, A->type->code, n * k, err)); xval = x_cast; }
+    // X' (n x k): the row-major k x n form transposed, unless A already is n x k (INP0 = TRAN) or k = 1
+    const bool xtr = !f.tran0 && k > 1;
+    const size_t bx = mul_reads_y(mul) ? tc_size(xt) : tc_size(A->type->code);
+    DevBuf<void> xtval; DevBuf<uint8_t> xtpres;
+    if (xtr) {
+        GB_TRY(xtval.alloc((size_t)(n * k) * bx + 16, err));
+        if (xpres) GB_TRY(xtpres.alloc((size_t)(n * k), err));
+        GB_TRY(dense_transpose(xval, xpres, k, n, bx, xtval, xtpres, err));
+        x_cast.reset();
+        xval = xtval; xpres = xtpres;
+        gb_kernel_used("x-transpose");
+    }
+    // T' (m x k), then T (k x m); both in fresh buffers
+    DevBuf<void> tval; DevBuf<uint8_t> tpres;
+    GB_TRY(tval.alloc((size_t)(m * k) * tc_size(zt) + 16, err));
+    GB_TRY(tpres.alloc((size_t)(m * k), err));
+    if (m > 0 && k > 0) GB_TRY(spmm_product(b, bval, xval, xpres, k, xt, zt, add, mul, tval, tpres, err));
+    b_cast.reset(); x_cast.reset(); xtval.reset(); xtpres.reset();
+    if (m > 1) {
+        DevBuf<void> uval; DevBuf<uint8_t> upres;
+        GB_TRY(uval.alloc((size_t)(m * k) * tc_size(zt) + 16, err));
+        GB_TRY(upres.alloc((size_t)(m * k), err));
+        GB_TRY(dense_transpose(tval, tpres, m, k, tc_size(zt), uval, upres, err));
+        tval = std::move(uval); tpres = std::move(upres);
+        gb_kernel_used("t-transpose");
+    }
+    // algorithmic bytes: the right route's (op(B)', X once, T), plus the transposes (each reads and writes its array)
+    const double xb = (double)(n * k) * (tc_size(A->type->code) + (A->dn.pres ? 1 : 0)), tb = (double)(m * k) * (tc_size(zt) + 1);
+    const double bytes = (double)b.nnz * (4 + tc_size(B->type->code)) + (double)(m + 1) * 4 + xb + tb + (xtr ? 2 * xb : 0.0) +
+                         (m > 1 ? 2 * tb : 0.0);
+    burble.note("spmm-left", bytes);
     return spmm_writeback(C, Mask, accum, f, std::move(tval), std::move(tpres), zt, err);
 }

@@ -12,7 +12,12 @@ quarter-valued inputs, and within 1e-6 relative of an fp64 scipy reference on ra
 
 and the share of it is over the data sheet's 3.35 TB/s.  --profile prints one torch.profiler split of a call instead.
 
-    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile]"""
+--left measures the dense left operand, C = X (+).(x) A with X a k x n dense form, against (b) k back-to-back GrB_vxm calls,
+(c) the right route on X' stored n x k (A' (+).(x) X' with T0: the same kernel without the two transposes) and (d) the CSR
+GrB_mxm (at --scale-csr and k = 8, one repetition), plus a k = 32 SSSP sweep D <- min(D, D min.+ A) against 32 single-source
+GrB_vxm sweeps; --left --profile splits one call into x-transpose, kernel, combine, t-transpose and write-back.
+
+    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile] [--left]"""
 import argparse
 import os
 import subprocess
@@ -165,6 +170,163 @@ def profile_split(scale):
     print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=12))
 
 
+def stack_vectors(ws, k, m):
+    v, p = np.zeros((k, m), np.float32), np.zeros((k, m), np.uint8)
+    for r in range(k):
+        x, q = ws[r].to_numpy()
+        v[r], p[r] = np.where(q.astype(bool), x, 0), q
+    return v, p
+
+
+def run_scale_left(stream, scale, with_csr, reps, warmup, out):
+    """--left: C = X (+).(x) A with X a k x n dense form (the left route) against (b) k GrB_vxm calls, (c) the right route on X'
+    stored n x k (A' (+).(x) X' with T0: the same kernel without the two transposes) and (d) the CSR GrB_mxm at --scale-csr, k = 8."""
+    for quarter in (True, False):
+        n, indptr, indices, vals = graph(scale, quarter)
+        nnz = len(indices)
+        A = Matrix.from_csr(indptr, indices, vals, n, n, FP32)
+        S64t = sp.csr_matrix((vals.astype(np.float64), indices, indptr), shape=(n, n)).T.tocsr() if not quarter else None
+        for semi in (FP32.PLUS_TIMES, FP32.MAX_PLUS):
+            if not quarter and semi is not FP32.PLUS_TIMES:
+                continue
+            for k in KS:
+                xt = xblock(n, k, quarter)                     # n x k
+                x = np.ascontiguousarray(xt.T)                 # k x n: the rows are the vectors
+                X, Xt = Matrix.from_numpy(x), Matrix.from_numpy(xt)
+                rows = [Vector.from_numpy(x[r]) for r in range(k)]
+                ws = [Vector.sparse(FP32, n) for _ in range(k)]
+                C, R = Matrix.sparse(FP32, k, n), Matrix.sparse(FP32, n, k)
+                arms = {"left": lambda: X.mxm(A, semiring=semi, out=C),
+                        "vxm": lambda: [rows[r].vxm(A, semiring=semi, out=ws[r]) for r in range(k)],
+                        "right-on-Xt": lambda: A.mxm(Xt, semiring=semi, out=R, desc=gb.descriptor.T0)}
+                t = alternate(stream, arms, reps, warmup)
+                Xc = None
+                if with_csr and k == 8:
+                    Xc = Matrix.from_csr(np.arange(0, n * k + 1, n, dtype=np.int64), np.tile(np.arange(n, dtype=np.uint32), k), x.reshape(-1), k, n, FP32)
+                    Cc = Matrix.sparse(FP32, k, n)
+                    t.update(alternate(stream, {"csr-mxm": lambda: Xc.mxm(A, semiring=semi, out=Cc)}, 1, 0))
+                X.mxm(A, semiring=semi, out=C)
+                kern = last_kernel()
+                got, pres = C.to_numpy()
+                got = np.where(pres.astype(bool), got, np.float32(0))
+                vx, vp = stack_vectors(ws, k, n)
+                rv, rp = R.to_numpy()
+                rv, rp = np.where(rp.astype(bool), rv, np.float32(0)).T, rp.T
+                check = {"presence_equal_vxm": bool(np.array_equal(pres, vp)), "presence_equal_right": bool(np.array_equal(pres, rp))}
+                if quarter:
+                    check["bits_equal_vxm"] = bool(np.array_equal(got.view(np.uint32), vx.view(np.uint32)))
+                    check["bits_equal_right"] = bool(np.array_equal(got.view(np.uint32), rv.view(np.uint32)))
+                    if Xc is not None:
+                        cx, cp = Cc.to_numpy()
+                        check["bits_equal_csr_mxm"] = bool(np.array_equal(cp, pres) and np.array_equal(np.where(cp.astype(bool), cx, 0).view(np.uint32), got.view(np.uint32)))
+                else:
+                    want = (S64t @ xt.astype(np.float64)).T
+                    nz = pres.astype(bool)
+                    for name, g in (("left", got), ("vxm", vx), ("right", rv)):
+                        rel = np.abs(g[nz] - want[nz]) / np.maximum(np.abs(want[nz]), 1e-300)
+                        check[f"max_rel_err_fp64_{name}"] = float(rel.max()) if rel.size else 0.0
+                # the right route's bytes plus the two transposes (X' read and written, T' read and written)
+                model = byte_model(nnz, n, n, k) + 2 * n * k * 4 + 2 * n * k * 5
+                rec = {"mode": "left", "scale": scale, "n": n, "nnz": nnz, "semiring": semi.name, "k": k, "inputs": "quarter" if quarter else "random",
+                       "ms": {a: round(v, 4) for a, v in t.items()}, "left_vs_vxm": round(t["vxm"] / t["left"], 2),
+                       "left_over_right": round(t["left"] / t["right-on-Xt"], 3), "byte_model": model,
+                       "share_of_hbm_model": round(model / HBM_BPS / (t["left"] * 1e-3), 3), "kernels": kern, "checks": check}
+                print(rec, flush=True)
+                out.append(rec)
+                del arms, X, Xt, rows, ws, C, R, Xc
+        del A
+
+
+def sssp_left(stream, scale, reps, warmup, k=32):
+    """k-source SSSP sweeps D <- min(D, D min.+ A) on the left route against k single-source sweeps w <- min(w, w min.+ A) of
+    GrB_vxm, the same number of steps each (the steps the k-source sweep takes to converge)."""
+    n, indptr, indices = cached_graph(scale)
+    rng = np.random.default_rng(7)
+    w = rng.integers(1, 10, len(indices)).astype(np.float32)
+    A = Matrix.from_csr(indptr, indices, w, n, n, FP32)
+    src = rng.choice(n, k, replace=False)
+    d0, p0 = np.zeros((k, n), np.float32), np.zeros((k, n), np.uint8)
+    p0[np.arange(k), src] = 1
+    D = Matrix.from_numpy(d0, present=p0)
+    steps, prev = 0, D.to_numpy()
+    while True:
+        D.mxm(A, semiring=FP32.MIN_PLUS, accum=FP32.MIN, out=D)
+        steps += 1
+        cur = D.to_numpy()
+        if np.array_equal(cur[1], prev[1]) and np.array_equal(cur[0], prev[0]):
+            break
+        prev = cur
+    kern = last_kernel()
+    state = {}
+
+    def prep_left():
+        state["D"] = Matrix.from_numpy(d0, present=p0)
+
+    def left():
+        Dl = state["D"]
+        for _ in range(steps):
+            Dl.mxm(A, semiring=FP32.MIN_PLUS, accum=FP32.MIN, out=Dl)
+
+    def prep_vxm():
+        state["w"] = [Vector.from_numpy(d0[r], present=p0[r]) for r in range(k)]
+
+    def vxm():
+        for wr in state["w"]:
+            for _ in range(steps):
+                wr.vxm(A, semiring=FP32.MIN_PLUS, accum=FP32.MIN, out=wr)
+
+    # the arms alternated, each from fresh distances prepared outside the timed region
+    ts = {"left": [], "vxm": []}
+    for rep in range(warmup + reps):
+        for name, prep, f in (("left", prep_left, left), ("vxm", prep_vxm, vxm)):
+            prep()
+            gb.lib.B200_device_synchronize()
+            ms = time_once(stream, f)
+            if rep >= warmup:
+                ts[name].append(ms)
+    t = {a: float(np.median(v)) for a, v in ts.items()}
+    got, pres = state["D"].to_numpy()
+    vx, vp = stack_vectors(state["w"], k, n)
+    rec = {"mode": "left-sssp", "scale": scale, "k": k, "steps": steps, "ms": {a: round(v, 3) for a, v in t.items()},
+           "left_vs_vxm": round(t["vxm"] / t["left"], 2), "kernels": kern,
+           "checks": {"equal_vxm": bool(np.array_equal(pres, vp) and np.array_equal(np.where(pres.astype(bool), got, 0), vx)),
+                      "equal_converged": bool(np.array_equal(pres, cur[1]) and np.array_equal(got[pres == 1], cur[0][pres == 1]))}}
+    print(rec, flush=True)
+
+
+def profile_left(scale, k=32):
+    """torch.profiler split of one unmasked left-route call: the two dense transposes told apart by their start times."""
+    from torch.profiler import ProfilerActivity, profile
+    n, indptr, indices, vals = graph(scale, False)
+    A = Matrix.from_csr(indptr, indices, vals, n, n, FP32)
+    X = Matrix.from_numpy(np.ascontiguousarray(xblock(n, k, False).T))
+    C = Matrix.sparse(FP32, k, n)
+    f = lambda: X.mxm(A, semiring=FP32.PLUS_TIMES, out=C)
+    f(); gb.lib.B200_device_synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        f(); gb.lib.B200_device_synchronize()
+    groups = {"spmm kernel": ("spmm_kernel",), "combine": ("spmm_combine",), "prep": ("seg_", "scan_", "cast_", "narrow_"),
+              "write-back": ("vec_finalize",)}
+    split = {"x-transpose": 0.0, "t-transpose": 0.0, **{g: 0.0 for g in groups}}
+    other = 0.0
+    kernels = [e for e in prof.events() if getattr(e, "device_type", None) is not None and e.device_type.name == "CUDA"]
+    tr = sorted((e for e in kernels if "dense_transpose" in e.name), key=lambda e: e.time_range.start)
+    for i, e in enumerate(tr):
+        split["x-transpose" if i == 0 and len(tr) == 2 else "t-transpose"] += e.time_range.elapsed_us()
+    for e in kernels:
+        if "dense_transpose" in e.name:
+            continue
+        for g, keys in groups.items():
+            if any(s in e.name for s in keys):
+                split[g] += e.time_range.elapsed_us()
+                break
+        else:
+            other += e.time_range.elapsed_us()
+    print({"profile": f"left route, scale {scale} k={k} FP32 PLUS_TIMES, no mask", "device_us": {**{g: round(v, 1) for g, v in split.items()}, "other": round(other, 1)},
+           "kernels": last_kernel()})
+    print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=12))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=int, default=22)
@@ -172,13 +334,25 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--left", action="store_true", help="the dense left operand, X (+).(x) A (the batched vxm)")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     print({"card": card})
     stream = lib_stream()
     if a.profile:
-        profile_split(a.scale)
+        if a.left:
+            for k in (8, 32):
+                profile_left(a.scale, k)
+        else:
+            profile_split(a.scale)
+        return
+    if a.left:
+        out = []
+        run_scale_left(stream, a.scale, False, a.reps, a.warmup, out)
+        if a.scale_csr:
+            run_scale_left(stream, a.scale_csr, True, a.reps, a.warmup, out)
+        sssp_left(stream, a.scale, max(2, a.reps // 3), 1)
         return
     out = []
     run_scale(stream, a.scale, False, a.reps, a.warmup, out)

@@ -253,7 +253,7 @@ struct GbBurble {
 // stream, so a slot is never in use twice).  Large transient cudaMallocAsync / cudaFreeAsync pairs were measured to cost
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
 enum WsSlot : int { WS_WORDS = 0, WS_FOUND, WS_FLOPS, WS_TOTAL, WS_CS, WS_CM, WS_CL, WS_C1, WS_SROW, WS_SIDX, WS_SCNT, WS_MROW, WS_MIDX, WS_MCNT,
-                    WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_COUNT };
+                    WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW, WS_COUNT };
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh = nullptr);
 template <typename T> static inline GrB_Info ws_array(int slot, T **p, size_t count, std::string *err, bool *fresh = nullptr) {
     return ws_get(slot, (void **)p, count * sizeof(T) + 16, err, fresh);
@@ -347,6 +347,19 @@ int op_mirror(int op);
 // 2^31-1 entries (spmm.cu)
 GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
                        const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
+// values one lane folds in order before a dot product is split (bounds the FP32 rounding error of a sequential fold; the
+// partials are folded pairwise): entries of a row of op(A) in the SpMM kernel, positions k in the masked dense-dense kernel
+static constexpr int SPMM_SEG = 64;
+// out (cols x rows) = in (rows x cols)', both row-major, presence bytes carried along when pres is given (spmm.cu)
+GrB_Info dense_transpose(const void *val, const uint8_t *pres, int64_t rows, int64_t cols, size_t vsize, void *oval, uint8_t *opres,
+                         std::string *err);
+// (pattern of M, one found flag and one value of vsize bytes per entry of M) -> the CSR T of the found entries, rowptr32
+// included; T's dimensions are the caller's (spgemm.cu)
+GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err);
+// C<Mask> = accum(C, op(A) (+).(x) op(B)) for dense-form A and B, a builtin non-positional semiring and a CSR mask of fewer than
+// 2^32 entries, already on the device and not complemented: one dot product per entry of the mask (sddmm.cu)
+GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                   const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
 
 // ---------------------------------------------------------------- scalar carrier
 // A value of any builtin type held in 64 bits: BOOL/UINT* in .u, INT* in .i, FP* in .d

@@ -968,8 +968,15 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
             words = typed;
         }
     }
-    void *tval = words;
-    // compact (pattern of M, found) -> CSR
+    GB_TRY(masked_compact(M, found, words, zsz, T, err));
+    typed.reset();
+    trace.mark("compaction");
+    CU_TRY(cudaGetLastError(), err);
+    return GrB_SUCCESS;
+}
+
+GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
+    const int64_t nrows = M.nrows;
     GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
     CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
     if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, found, nrows, T.rowptr); GB_LAUNCHED(); }
@@ -977,16 +984,12 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
     int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
     T.nnz = nnz; G.last_nnz_out = (uint64_t)nnz;
     GB_TRY(T.col.alloc((size_t)nnz, err));
-    GB_TRY(T.val.alloc((size_t)nnz * zsz + 16, err));
+    GB_TRY(T.val.alloc((size_t)nnz * vsize + 16, err));
     if (nnz > 0) {
-        row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)zsz,
+        row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)vsize,
                                                                           nrows, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
     }
-    typed.reset();
-    GB_TRY(dev_build_rowptr32(T, err));
-    trace.mark("compaction");
-    CU_TRY(cudaGetLastError(), err);
-    return GrB_SUCCESS;
+    return dev_build_rowptr32(T, err);
 }
 
 // C<M> = accum(C, T) into a fresh CSR `out` of C's type (T has type ttc)
@@ -1126,6 +1129,10 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     GbBurble burble("GrB_mxm");
     G.last_kernel.clear();
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
+    if (A->dn.valid && B->dn.valid && Mask && !f.mask_comp && !Mask->dn.valid) {                   // two dense operands under a sparse mask
+        GB_TRY(matrix_ensure_device(Mask));
+        if (Mask->dev.rowptr32) return sddmm_mxm(C, Mask, accum, semiring, A, B, f, burble);
+    }
     if (B->dn.valid && !f.tran1) return spmm_mxm(C, Mask, accum, semiring, A, B, f, burble);         // dense X: DESIGN.md section 3.6
     if (A->dn.valid && !B->dn.valid && op_mirror(mul) >= 0 && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))
         return spmm_left_mxm(C, Mask, accum, semiring, A, B, f, burble);                            // dense X on the left

@@ -15,9 +15,6 @@
 #include "common.cuh"
 #include "spmv_common.cuh"
 
-static constexpr int SPMM_SEG = 64;       // entries of op(A) one group folds in order before a row is split (bounds the FP32
-                                          // rounding error of a sequential fold; the partials are folded pairwise)
-
 // ------------------------------------------------------------------ dense form <-> CSR
 __device__ __forceinline__ void copy_value(uint8_t *dst, int64_t d, const uint8_t *src, int64_t s, int vsize) {
     switch (vsize) {
@@ -124,7 +121,7 @@ __global__ void __launch_bounds__(256) dense_transpose_kernel(const V *in, const
     }
 }
 
-static GrB_Info dense_transpose(const void *val,const uint8_t *pres, int64_t rows, int64_t cols, size_t vsize, void *oval, uint8_t *opres,
+GrB_Info dense_transpose(const void *val,const uint8_t *pres, int64_t rows, int64_t cols, size_t vsize, void *oval, uint8_t *opres,
                          std::string *err) {
     if (rows == 0 || cols == 0) return GrB_SUCCESS;
     const int grid = grid_for(ceil_div(rows, 32) * ceil_div(cols, 32), 1);

@@ -88,7 +88,17 @@ class Matrix:
     @classmethod
     def from_numpy(cls, x, present=None, typ=None):
         """Dense import of a 2-D array straight into HBM (B200 extension `B200_Matrix_import_dense`).  `present`
-        (same shape, nonzero = present) marks the entries; None means every entry is present."""
+        (same shape, nonzero = present) marks the entries; None means every entry is present.
+
+        Two dense forms under a sparse mask multiply one dot product per entry of the mask, and a sparse matrix times a dense
+        form is the SpMM: the two halves of a GNN layer on a graph A (n x n) with features H (n x d), on the device throughout
+        (`mxm` sizes a missing `out` without looking at T1, so the scores get theirs passed):
+
+        >>> H = Matrix.from_numpy(h)                                         # doctest: +SKIP
+        >>> S = Matrix.sparse(FP32, n, n)                                    # doctest: +SKIP
+        >>> H.mxm(H, mask=A, desc=descriptor.ST1, out=S)    # S<A> = H H'    # doctest: +SKIP
+        >>> Z = S.mxm(H)                                    # Z = S H        # doctest: +SKIP
+        """
         x = np.asarray(x)
         if x.ndim != 2:
             raise ValueError("from_numpy expects a 2-D array")

@@ -17,7 +17,19 @@ and the share of it is over the data sheet's 3.35 TB/s.  --profile prints one to
 GrB_mxm (at --scale-csr and k = 8, one repetition), plus a k = 32 SSSP sweep D <- min(D, D min.+ A) against 32 single-source
 GrB_vxm sweeps; --left --profile splits one call into x-transpose, kernel, combine, t-transpose and write-back.
 
-    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile] [--left]"""
+--sddmm measures two dense-form operands under a sparse mask, C<M> = X (+).(x) Y' (DESIGN.md section 3.6): M = the R-MAT graph
+as a structural mask, X and Y random FP32 (and quarter-valued) n x d, desc = ST1, against (b) the same call without T1 on Y
+stored d x n (what y-transpose costs), (c) the CSR path on the same operands imported as CSR, at scale <= 14 and d = 8 only (above
+2^18 entries of Y that path forms m d n products and does not finish), and (d) torch on the same device, (X[rows] * Y[cols]).sum(1)
+in edge chunks (PLUS_TIMES only).  Checks: (a) = (b) bit for bit, (a) = (c) bit for bit on quarter values, (a) within 1e-6 relative
+of fp64 numpy on 10^6 sampled edges plus the edges of the 16 longest mask rows.  Its byte model is
+
+    nnz(M) 4 + (m + 1) 4 + m d b_X + n d b_Y + nnz(T) (4 + b_C) + (m + 1) 8   [+ 2 n d b_Y for y-transpose]
+
+which leaves out the gather, nnz(M) d b_Y (reported beside it); --sddmm --profile splits one call into row ids, kernel,
+transposes and write-back.
+
+    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile] [--left | --sddmm] [--ds 8,32,128]"""
 import argparse
 import os
 import subprocess
@@ -327,6 +339,127 @@ def profile_left(scale, k=32):
     print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=12))
 
 
+def sddmm_byte_model(nnz, m, n, d, b=4, y_transposed=False):
+    return nnz * 4 + (m + 1) * 4 + m * d * b + n * d * b + nnz * (4 + b) + (m + 1) * 8 + (2 * n * d * b if y_transposed else 0)
+
+
+def sddmm_values(C):
+    I, J, V = C.to_arrays()
+    return np.asarray(I), np.asarray(J), np.asarray(V)
+
+
+def edge_dots64(x, y, r, c, chunk=1 << 18):
+    """Per edge (r, c): the fp64 dot product of x[r] and y[c], and that of their absolute values (the error scale)."""
+    want, scale = np.empty(len(r)), np.empty(len(r))
+    for s0 in range(0, len(r), chunk):
+        a, b = x[r[s0:s0 + chunk]].astype(np.float64), y[c[s0:s0 + chunk]].astype(np.float64)
+        want[s0:s0 + chunk] = np.einsum("ij,ij->i", a, b)
+        scale[s0:s0 + chunk] = np.einsum("ij,ij->i", np.abs(a), np.abs(b))
+    return want, scale
+
+
+def run_scale_sddmm(stream, scale, with_csr, reps, warmup, ds, out):
+    n, indptr, indices = cached_graph(scale)
+    nnz = len(indices)
+    rows = np.repeat(np.arange(n, dtype=np.int64), np.diff(indptr))
+    M = Matrix.from_csr(indptr, indices, np.ones(nnz, np.bool_), n, n, gb.BOOL)
+    rows_t, cols_t = torch.from_numpy(rows).cuda(), torch.from_numpy(indices.astype(np.int64)).cuda()
+    rng = np.random.default_rng(11)
+    longest = np.argsort(np.diff(indptr))[-16:]
+    sample = np.unique(np.concatenate([rng.integers(0, nnz, 1 << 20)] + [np.arange(indptr[r], indptr[r + 1]) for r in longest]))
+    ST1, S = gb.descriptor.ST1, gb.descriptor.S
+    for quarter in (True, False):
+        for semi in (FP32.PLUS_TIMES, FP32.MAX_PLUS):
+            if not quarter and semi is not FP32.PLUS_TIMES:
+                continue
+            for d in ds:
+                x, y = xblock(n, d, quarter, seed=3), xblock(n, d, quarter, seed=5)
+                X, Y, Yt = Matrix.from_numpy(x), Matrix.from_numpy(y), Matrix.from_numpy(np.ascontiguousarray(y.T))
+                # every call writes a fresh, empty C, so the result is T itself; a C that holds entries (without GrB_REPLACE) adds the
+                # row-wise merge of T with C that every masked mxm shares ("merge-into-C", one arm, for scale)
+                res = {}
+                arms = {"sddmm": lambda: res.__setitem__("a", X.mxm(Y, semiring=semi, mask=M, desc=ST1, out=Matrix.sparse(FP32, n, n))),
+                        "y-given-d-x-n": lambda: res.__setitem__("b", X.mxm(Yt, semiring=semi, mask=M, desc=S, out=Matrix.sparse(FP32, n, n)))}
+                if d == 32 and semi is FP32.PLUS_TIMES:
+                    Cm = Matrix.sparse(FP32, n, n)
+                    arms["merge-into-C"] = lambda: X.mxm(Y, semiring=semi, mask=M, desc=ST1, out=Cm)
+                if semi is FP32.PLUS_TIMES:
+                    xd, yd = torch.from_numpy(x).cuda(), torch.from_numpy(y).cuda()
+                    td = torch.empty(nnz, dtype=torch.float32, device="cuda")
+                    chunk = max(1, (1 << 28) // d)               # 1 GiB of gathered FP32 values per operand and chunk
+
+                    def torch_arm():
+                        with torch.cuda.stream(stream):
+                            for s0 in range(0, nnz, chunk):
+                                td[s0:s0 + chunk] = (xd[rows_t[s0:s0 + chunk]] * yd[cols_t[s0:s0 + chunk]]).sum(1)
+                    arms["torch"] = torch_arm
+                t = alternate(stream, arms, reps, warmup)
+                arms["sddmm"]()
+                kern = last_kernel()
+                I, J, V = sddmm_values(res["a"])
+                I2, J2, V2 = sddmm_values(res["b"])
+                check = {"pattern_is_mask": bool(np.array_equal(I, rows) and np.array_equal(J, indices)),
+                         "bits_equal_y_given_d_x_n": bool(np.array_equal(I, I2) and np.array_equal(J, J2) and np.array_equal(V.view(np.uint32), V2.view(np.uint32)))}
+                if with_csr and d == 8:
+                    ptr = np.arange(0, n * d + 1, d, dtype=np.int64); ids = np.tile(np.arange(d, dtype=np.uint32), n)
+                    Xc, Yc = Matrix.from_csr(ptr, ids, x.reshape(-1), n, d, FP32), Matrix.from_csr(ptr, ids, y.reshape(-1), n, d, FP32)
+                    Cc = Matrix.sparse(FP32, n, n)
+                    t.update(alternate(stream, {"csr-mxm": lambda: Xc.mxm(Yc, semiring=semi, mask=M, desc=ST1, out=Cc)}, 3, 1))
+                    check["csr_kernels"] = last_kernel()
+                    Ic, Jc, Vc = sddmm_values(Cc)
+                    if quarter:
+                        check["bits_equal_csr_mxm"] = bool(np.array_equal(I, Ic) and np.array_equal(J, Jc) and np.array_equal(V.view(np.uint32), Vc.view(np.uint32)))
+                if semi is FP32.PLUS_TIMES:
+                    want, scale_ = edge_dots64(x, y, rows[sample], indices[sample])
+                    check["max_rel_err_fp64_sampled"] = float((np.abs(V[sample] - want) / np.maximum(scale_, 1e-300)).max())
+                    check["sampled_edges"] = int(len(sample))
+                    tv = td.cpu().numpy()
+                    check["max_rel_err_fp64_torch"] = float((np.abs(tv[sample] - want) / np.maximum(scale_, 1e-300)).max())
+                model, gather = sddmm_byte_model(nnz, n, n, d), nnz * d * 4
+                sec = t["sddmm"] * 1e-3
+                rec = {"mode": "sddmm", "scale": scale, "n": n, "nnz": nnz, "semiring": semi.name, "d": d, "inputs": "quarter" if quarter else "random",
+                       "ms": {a: round(v, 4) for a, v in t.items()}, "y_transpose_cost": round(t["y-given-d-x-n"] / t["sddmm"], 3),
+                       "byte_model": model, "gather_bytes": gather, "share_of_hbm_model": round(model / HBM_BPS / sec, 3),
+                       "share_of_hbm_with_gather": round((model + gather) / HBM_BPS / sec, 3), "kernels": kern, "checks": check}
+                if "torch" in t:
+                    rec["speedup_vs_torch"] = round(t["torch"] / t["sddmm"], 2)
+                print(rec, flush=True)
+                out.append(rec)
+                del arms, res, X, Y, Yt
+    del M
+
+
+def profile_sddmm(scale, d=32):
+    """torch.profiler split of one call with T1 and of one without (which builds y-transpose)."""
+    from torch.profiler import ProfilerActivity, profile
+    n, indptr, indices = cached_graph(scale)
+    M = Matrix.from_csr(indptr, indices, np.ones(len(indices), np.bool_), n, n, gb.BOOL)
+    x, y = xblock(n, d, False, seed=3), xblock(n, d, False, seed=5)
+    X, Y, Yt = Matrix.from_numpy(x), Matrix.from_numpy(y), Matrix.from_numpy(np.ascontiguousarray(y.T))
+    C = Matrix.sparse(FP32, n, n)
+    fresh = lambda: Matrix.sparse(FP32, n, n)
+    groups = {"row ids": ("sddmm_rowid",), "kernel": ("sddmm_kernel",), "transposes": ("dense_transpose",),
+              "compaction": ("row_found", "scan", "Scan"), "write-back": ("mat_finalize", "cast_", "rowptr32")}
+    for name, f in (("desc=ST1, empty C", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.ST1, out=fresh())),
+                    ("desc=S, Y given d x n, empty C", lambda: X.mxm(Yt, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.S, out=fresh())),
+                    ("desc=ST1, C holds the last result", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.ST1, out=C))):
+        f(); gb.lib.B200_device_synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            f(); gb.lib.B200_device_synchronize()
+        split = {g: 0.0 for g in groups}; other = 0.0
+        for ev in prof.key_averages():
+            us = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+            for g, keys in groups.items():
+                if any(k in ev.key for k in keys):
+                    split[g] += us
+                    break
+            else:
+                other += us
+        print({"profile": f"sddmm, scale {scale} d={d} FP32 PLUS_TIMES, structural mask, {name}",
+               "device_us": {**{g: round(v, 1) for g, v in split.items()}, "other (copies of M's pattern, memsets)": round(other, 1)}, "kernels": last_kernel()})
+        print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=8))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=int, default=22)
@@ -335,11 +468,22 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--left", action="store_true", help="the dense left operand, X (+).(x) A (the batched vxm)")
+    ap.add_argument("--sddmm", action="store_true", help="two dense operands under a sparse mask, C<M> = X (+).(x) Y'")
+    ap.add_argument("--ds", default="8,32,128", help="--sddmm: the inner dimensions d")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     print({"card": card})
     stream = lib_stream()
+    if a.sddmm:
+        if a.profile:
+            profile_sddmm(a.scale)
+            return
+        out, ds = [], tuple(int(v) for v in a.ds.split(","))
+        run_scale_sddmm(stream, a.scale, False, a.reps, a.warmup, ds, out)
+        if a.scale_csr:
+            run_scale_sddmm(stream, min(a.scale_csr, 14), True, a.reps, a.warmup, (8,), out)
+        return
     if a.profile:
         if a.left:
             for k in (8, 32):

@@ -110,7 +110,10 @@ extern "C" GrB_Info B200_Comm_free(B200_Comm *comm) {
         for (int p = 0; p < c->world; ++p) if (p != c->rank && c->peer[p]) cudaIpcCloseMemHandle(c->peer[p]);
         cudaFree(c->region);
     }
-    if (c->view) { c->view->dval = nullptr; c->view->dpres = nullptr; c->view->dev_valid = false; GrB_Vector_free(&c->view); }
+    if (c->view) {
+        if (c->view->borrowed) { c->view->dval = nullptr; c->view->dpres = nullptr; c->view->dev_valid = false; c->view->borrowed = false; }
+        GrB_Vector_free(&c->view);           // frees what the view owns
+    }
     c->magic = GB_FREED; delete c; *comm = nullptr;
     return GrB_SUCCESS;
 }
@@ -190,6 +193,8 @@ static inline int pgrid(size_t bytes) { return (int)std::max<size_t>(1, std::min
 
 static void comm_set_view(B200_Comm c, int which) {
     unsigned char *b = comm_buf(c, c->region, which);
+    vector_invalidate_device(c->view);       // buffers the view came to own (an import into it, a write with it as output) are freed
+    c->view->use_recorded = false;
     c->view->dval = b; c->view->dpres = b + c->val_bytes; c->view->dev_valid = true; c->view->dev_nvals = -1; c->view->borrowed = true;
     c->view->host_valid = false; c->view->hi.clear(); c->view->hx.clear(); c->view->pi.clear(); c->view->px.clear();
 }

@@ -433,6 +433,12 @@ static void vector_join_copies(GrB_Vector v) {
     if (v->h2d_pending) { cudaStreamWaitEvent(G.stream, v->ev_h2d, 0); v->h2d_pending = false; }
     if (v->d2h_pending) { cudaStreamWaitEvent(G.stream, v->ev_d2h, 0); v->d2h_pending = false; }
 }
+// an overlapped import still running on the import stream must land before the compute stream reads v
+static void vector_join_import(GrB_Vector v) {
+    if (v->h2d_pending) { cudaStreamWaitEvent(G.stream, v->ev_h2d, 0); v->h2d_pending = false; }
+}
+// ev_use marks the end of the last kernels that touch v.  Every call that enqueues work reading or writing v's buffers goes
+// through vector_ensure_device or vector_adopt_device, which drop the mark; mxv / vxm set it again once their kernels are enqueued.
 void vector_mark_used(GrB_Vector v) {
     if (v && v->ev_use) { cudaEventRecord(v->ev_use, G.stream); v->use_recorded = true; }
 }
@@ -461,6 +467,7 @@ bool matrix_known_empty(const GrB_Matrix A) {
 }
 void vector_adopt_device(GrB_Vector v, void *vals, uint8_t *pres) {
     vector_invalidate_device(v);
+    v->use_recorded = false;       // the new buffers are filled (and their pool blocks were last used) by work enqueued since
     v->dval = vals; v->dpres = pres; v->dev_valid = true; v->dev_nvals = pres ? -1 : (int64_t)v->n;
     v->hi.clear(); v->hx.clear(); v->pi.clear(); v->px.clear(); v->host_valid = false;
 }
@@ -593,6 +600,7 @@ GrB_Info matrix_ensure_transpose(GrB_Matrix A) {
 GrB_Info vector_ensure_host(GrB_Vector v) {
     if (v->host_valid) return vector_flush_pending(v);
     if (!v->dev_valid) { v->host_valid = true; return GrB_SUCCESS; }
+    vector_join_import(v);
     const size_t sz = v->type->size, n = (size_t)v->n;
     std::vector<uint8_t> vals(n * sz), pres;
     CU_TRY(cudaMemcpyAsync(vals.data(), v->dval, n * sz, cudaMemcpyDeviceToHost, G.stream), &v->err);
@@ -615,7 +623,8 @@ __global__ void vec_scatter_kernel(const uint64_t *idx, const uint8_t *x, uint8_
 GrB_Info vector_ensure_device(GrB_Vector v) {
     if (!G.have_device) return gb_fail(GrB_PANIC, &v->err, "no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
     if (v->host_valid) GB_TRY(vector_flush_pending(v));
-    if (v->h2d_pending) { cudaStreamWaitEvent(G.stream, v->ev_h2d, 0); v->h2d_pending = false; }     // an overlapped import is in flight
+    vector_join_import(v);
+    v->use_recorded = false;       // the caller enqueues work on v after the last recorded use
     if (v->dev_valid) return GrB_SUCCESS;
     if (v->n > DEV_DIM_MAX) return gb_fail(GrB_INVALID_VALUE, &v->err, "vector size %llu exceeds the 2^31-1 limit of the HBM layout", (unsigned long long)v->n);
     const size_t sz = v->type->size, n = (size_t)v->n, k = v->hi.size();
@@ -891,6 +900,7 @@ extern "C" GrB_Info GrB_Vector_dup(GrB_Vector *w, const GrB_Vector u) {
     GB_LOCK; GB_CHECK_INIT;
     if (!w) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_Vector_dup: NULL handle");
     GB_VECTOR_OK(u, "GrB_Vector_dup");
+    if (!u->host_valid) GB_TRY(vector_ensure_device(u));      // the copies below read u on the compute stream
     GB_Vector_opaque *o = new GB_Vector_opaque();
     o->magic = GB_MAGIC; o->type = u->type; o->n = u->n;
     if (u->host_valid) {
@@ -902,9 +912,11 @@ extern "C" GrB_Info GrB_Vector_dup(GrB_Vector *w, const GrB_Vector u) {
         DevBuf<void> dval; DevBuf<uint8_t> dpres;
         GrB_Info r = dval.alloc(n * sz + 16, &u->err);
         if (r == GrB_SUCCESS && u->dpres) r = dpres.alloc(n, &u->err);
+        if (r == GrB_SUCCESS && cudaMemcpyAsync(dval, u->dval, n * sz, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+            r = gb_fail(GrB_PANIC, &u->err, "GrB_Vector_dup: copy of the values failed");
+        if (r == GrB_SUCCESS && u->dpres && cudaMemcpyAsync(dpres, u->dpres, n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+            r = gb_fail(GrB_PANIC, &u->err, "GrB_Vector_dup: copy of the presence failed");
         if (r != GrB_SUCCESS) { delete o; return r; }
-        cudaMemcpyAsync(dval, u->dval, n * sz, cudaMemcpyDeviceToDevice, G.stream);
-        if (u->dpres) cudaMemcpyAsync(dpres, u->dpres, n, cudaMemcpyDeviceToDevice, G.stream);
         o->dval = dval.release(); o->dpres = dpres.release(); o->dev_valid = true; o->dev_nvals = u->dev_nvals;
     }
     *w = o; return GrB_SUCCESS;
@@ -925,7 +937,7 @@ extern "C" GrB_Info GrB_Vector_nvals(GrB_Index *n, const GrB_Vector v) {
     if (v->host_valid) { GB_TRY(vector_flush_pending(v)); *n = v->hi.size(); return GrB_SUCCESS; }
     if (v->dev_nvals < 0) {
         if (!v->dpres) v->dev_nvals = (int64_t)v->n;
-        else GB_TRY(dev_count_present(v->dpres, (int64_t)v->n, &v->dev_nvals, &v->err));
+        else { vector_join_import(v); GB_TRY(dev_count_present(v->dpres, (int64_t)v->n, &v->dev_nvals, &v->err)); }
     }
     *n = (GrB_Index)v->dev_nvals; return GrB_SUCCESS;
 }
@@ -1194,17 +1206,18 @@ extern "C" GrB_Info B200_Vector_set_dense(GrB_Vector v, const void *x, const uin
     if (v->n > DEV_DIM_MAX) return gb_fail(GrB_INVALID_VALUE, &v->err, "vector size exceeds 2^31-1");
     const size_t sz = v->type->size, n = (size_t)v->n;
     if (where == 2) GB_TRY(vector_async_setup(v));
-    const bool fresh = !v->dev_valid || !v->dval || (present && !v->dpres) || (!present && v->dpres);
-    if (!v->dev_valid || !v->dval) { vector_invalidate_device(v); GB_TRY(dmalloc(&v->dval, n * sz + 16, &v->err)); }
+    // a borrowed view (B200_Comm_result) gets buffers of its own: the communicator's region is neither written nor freed here
+    const bool fresh = v->borrowed || !v->dev_valid || !v->dval || (present && !v->dpres) || (!present && v->dpres);
+    if (v->borrowed || !v->dev_valid || !v->dval) { vector_invalidate_device(v); GB_TRY(dmalloc(&v->dval, n * sz + 16, &v->err)); }
     if (present && !v->dpres) GB_TRY(dmalloc((void **)&v->dpres, n + 16, &v->err));
     if (!present && v->dpres) { vector_join_copies(v); dfree(v->dpres); v->dpres = nullptr; }
     if (where == 2) {
         // pinned host memory, copied on the import stream so that it overlaps kernels already enqueued on the compute stream.
-        // The copy may start once the last kernels that READ this vector are done (their event, recorded by the call that
-        // used it) -- or, when the buffers are new or the use was not recorded, once everything enqueued so far is done.
+        // The copy may start once the last kernels that touch this vector are done (their event, recorded by the mxv / vxm that
+        // read it last and dropped by any later read or write) -- or, when the buffers are new or no use is recorded, once
+        // everything enqueued so far is done.
         if (v->use_recorded && !fresh) cudaStreamWaitEvent(G.h2d, v->ev_use, 0);
         else { cudaEventRecord(v->ev_use, G.stream); cudaStreamWaitEvent(G.h2d, v->ev_use, 0); }
-        v->use_recorded = false;
         if (v->d2h_pending) cudaStreamWaitEvent(G.h2d, v->ev_d2h, 0);
         CU_TRY(cudaMemcpyAsync(v->dval, x, n * sz, cudaMemcpyHostToDevice, G.h2d), &v->err);
         if (present) CU_TRY(cudaMemcpyAsync(v->dpres, present, n, cudaMemcpyHostToDevice, G.h2d), &v->err);
@@ -1215,6 +1228,7 @@ extern "C" GrB_Info B200_Vector_set_dense(GrB_Vector v, const void *x, const uin
         GB_TRY(copy_in(v->dval, x, n * sz, where, &v->err));
         if (present) GB_TRY(copy_in(v->dpres, present, n, where, &v->err));
     }
+    v->use_recorded = false;       // this call wrote v: an earlier use no longer orders the next import
     v->dev_valid = true; v->dev_nvals = present ? -1 : (int64_t)n;
     v->hi.clear(); v->hx.clear(); v->pi.clear(); v->px.clear(); v->host_valid = false;
     return GrB_SUCCESS;

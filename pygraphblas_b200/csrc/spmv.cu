@@ -478,6 +478,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
 
     if (in_place) {                    // T was formed in w's own buffers: only the bookkeeping changes
         w->dev_nvals = -1; w->host_valid = false; w->hi.clear(); w->hx.clear(); w->pi.clear(); w->px.clear();
+        w->use_recorded = false;       // the kernels above write w: an import into w waits for them
         CU_TRY(cudaGetLastError(), err);
         return GrB_SUCCESS;
     }

@@ -235,14 +235,15 @@ uint64_t B200_kernel_launches(void);
 void B200_debug_fail_alloc(int64_t k);
 int64_t B200_debug_live_allocs(void);
 /* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("tile (specialised, 8 items)",
- * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-L",
+ * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "spa-split", "masked-warp", "stream-L",
  * "dot", ...); recorded whether the burble is on or not, valid until the next such call.  Host-decided variants follow
  * their entry as "key=value" tokens: "filter=exact" or "filter=bloom" after each "stream-S" / "stream-M" / "stream-L"
  * (the mask-row membership filter is an exact bitmap or a one-hash Bloom filter), and "mxv=in-place" after an mxv / vxm
  * entry when the product was formed straight in w's buffers */
 const char *B200_debug_last_kernel(void);
 /* per-matrix SpGEMM/SpMV work figures of the most recent GrB_mxm (flops = number of
- * multiplies, nnz_out = nvals of the semiring product before accum/mask) */
+ * multiplies, nnz_out = nvals of the product T as the kernels formed it, before the accumulator and the write-back:
+ * unmasked calls report the whole product, masked ones (complemented or not) only the entries the mask lets through) */
 GrB_Info B200_last_mxm_stats(uint64_t *flops, uint64_t *nnz_out);
 /* ------------------------------------------------------------------ multi-GPU exchange (csrc/dist.cu)
  * One process per GPU; A is 1-D row-block partitioned (SURVEY.md section 8e).  The library moves the output

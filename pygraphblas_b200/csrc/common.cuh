@@ -253,7 +253,8 @@ struct GbBurble {
 // stream, so a slot is never in use twice).  Large transient cudaMallocAsync / cudaFreeAsync pairs were measured to cost
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
 enum WsSlot : int { WS_WORDS = 0, WS_FOUND, WS_FLOPS, WS_TOTAL, WS_CS, WS_CM, WS_CL, WS_C1, WS_SROW, WS_SIDX, WS_SCNT, WS_MROW, WS_MIDX, WS_MCNT,
-                    WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW, WS_COUNT };
+                    WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW,
+                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_COUNT };
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh = nullptr);
 template <typename T> static inline GrB_Info ws_array(int slot, T **p, size_t count, std::string *err, bool *fresh = nullptr) {
     return ws_get(slot, (void **)p, count * sizeof(T) + 16, err, fresh);
@@ -356,6 +357,9 @@ GrB_Info dense_transpose(const void *val, const uint8_t *pres, int64_t rows, int
 // (pattern of M, one found flag and one value of vsize bytes per entry of M) -> the CSR T of the found entries, rowptr32
 // included; T's dimensions are the caller's (spgemm.cu)
 GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err);
+// the entries of a valued mask M (type mtc) that are true, x != 0 as in mask_value_true (NaN true, +-0 false), as a CSR pattern with
+// 32-bit row pointers: the columns a complemented mask blocks (select_kernel with SEL_NONZERO, matrix_ops.cu)
+GrB_Info mask_true_pattern(const Csr &M, int mtc, Csr &out, std::string *err);
 // C<Mask> = accum(C, op(A) (+).(x) op(B)) for dense-form A and B, a builtin non-positional semiring and a CSR mask of fewer than
 // 2^32 entries, already on the device and not complemented: one dot product per entry of the mask (sddmm.cu)
 GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,

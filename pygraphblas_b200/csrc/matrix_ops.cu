@@ -84,8 +84,10 @@ __global__ void __launch_bounds__(256) select_kernel(const SelectArgs a) {
             if (FILL && keep) {
                 const int64_t o = out + __popc(m & ((1u << lane) - 1u));
                 a.o_col[o] = c;
-                const uint8_t *src = (const uint8_t *)a.val + (size_t)e * vs; uint8_t *dst = (uint8_t *)a.o_val + (size_t)o * vs;
-                for (int q = 0; q < vs; ++q) dst[q] = src[q];
+                if (a.o_val) {                          // no value array: the pattern only (mask_true_pattern)
+                    const uint8_t *src = (const uint8_t *)a.val + (size_t)e * vs; uint8_t *dst = (uint8_t *)a.o_val + (size_t)o * vs;
+                    for (int q = 0; q < vs; ++q) dst[q] = src[q];
+                }
             }
             out += __popc(m);
         }
@@ -134,6 +136,21 @@ extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const
     if (T.nnz > 0) { select_kernel<true><<<grid_for(T.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
+}
+GrB_Info mask_true_pattern(const Csr &M, int mtc, Csr &out, std::string *err) {
+    SelectArgs a{};
+    a.code = SEL_NONZERO; a.rowptr = M.rowptr; a.col = M.col; a.val = M.val; a.tc = mtc; a.nrows = M.nrows;
+    out = Csr(); out.nrows = M.nrows; out.ncols = M.ncols;
+    GB_TRY(out.rowptr.alloc((size_t)M.nrows + 1, err));
+    CU_TRY(cudaMemsetAsync(out.rowptr, 0, ((size_t)M.nrows + 1) * 8, G.stream), err);
+    a.o_ptr = out.rowptr;
+    if (M.nnz > 0) { select_kernel<false><<<grid_for(M.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    GB_TRY(dev_exclusive_scan(out.rowptr, M.nrows + 1, err));
+    GB_TRY(read_i64(out.rowptr + M.nrows, &out.nnz, err));
+    GB_TRY(out.col.alloc((size_t)out.nnz, err));
+    a.o_col = out.col; a.o_val = nullptr;       // the filter reads the pattern only
+    if (out.nnz > 0) { select_kernel<true><<<grid_for(M.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+    return dev_build_rowptr32(out, err);
 }
 __global__ void vec_select_kernel(const SelectArgs a, const uint8_t *upres, uint8_t *tpres) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.nrows; i += (int64_t)gridDim.x * blockDim.x) {

@@ -8,7 +8,8 @@
 //               columns in a shared-memory hash table (atomicCAS probing) and form their
 //               values by expand-sort-compress in shared memory; rows beyond the shared-memory
 //               budget use a dense accumulator in HBM owned by a persistent CTA.  Rows come out
-//               sorted (in-smem bitonic sort / ordered bitmap sweep).
+//               sorted (in-smem bitonic sort / ordered bitmap sweep).  A complemented mask runs the same pipeline
+//               with the mask's blocking entries filtered inside each kernel (COMP instantiations).
 //   masked      C<M> = A*B with a non-complemented mask: the mask row M(i,:) is loaded into
 //               the table first, products are accumulated only where they hit it, so both
 //               the work kept and the output are bounded by nnz(M) (triangle counting,
@@ -168,9 +169,23 @@ template <bool WARP> __device__ void bitonic_sort_u64(unsigned long long *a, int
     }
 }
 
+// ------------------------------------------------------------------ complemented mask: the columns that block a position
+// COMP instantiations of the unmasked kernels compute T = (A (+).(x) B)<!M'> where M' (m_ptr / m_col, sorted rows) holds the
+// mask entries that block: a column j of row i survives when it is not in M'(i, [ms, me)).  A binary search of the mask row
+// keeps the test at log2(ncols) loads however long the row is (the path counts of betweenness centrality are full rows).
+__device__ __forceinline__ bool mask_blocks(const uint32_t *m_col, uint32_t ms, uint32_t me, uint32_t j) {
+    uint32_t lo = ms, hi = me;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(m_col + mid) < j) lo = mid + 1; else hi = mid;
+    }
+    return lo < me && __ldg(m_col + lo) == j;
+}
+
 // ------------------------------------------------------------------ unmasked, symbolic pass: shared-memory hash
-// One row per group (a warp, or the whole CTA): count its distinct columns.
-template <bool WARP>
+// One row per group (a warp, or the whole CTA): count its distinct columns (COMP: those not blocked by M', tested once per
+// distinct column, when it first enters the table).
+template <bool WARP, bool COMP = false>
 __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
     extern __shared__ unsigned char smem_raw[];
     const int gsize = WARP ? 32 : blockDim.x;
@@ -190,6 +205,8 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
     if (active) {
         const int64_t row = p.rows[idx];
         const uint32_t as = p.a_ptr[row], ae = p.a_ptr[row + 1];
+        uint32_t ms = 0, me = 0;
+        if (COMP) { ms = p.m_ptr[row]; me = p.m_ptr[row + 1]; }
         if (WARP) {       // lane per A entry, each lane walks its B row
             for (uint32_t pa = as + tid; pa < ae; pa += 32) {
                 const uint32_t k = p.a_col[pa];
@@ -198,7 +215,7 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
                     uint32_t s = hash_col(j, hshift);
                     while (true) {
                         const uint32_t seen = atomicCAS(&keys[s], EMPTY_KEY, j);
-                        if (seen == EMPTY_KEY) { ++mine; break; }
+                        if (seen == EMPTY_KEY) { if (!COMP || !mask_blocks(p.m_col, ms, me, j)) ++mine; break; }
                         if (seen == j) break;
                         s = (s + 1) & tmask;
                     }
@@ -213,7 +230,7 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
                     uint32_t s = hash_col(j, hshift);
                     while (true) {
                         const uint32_t seen = atomicCAS(&keys[s], EMPTY_KEY, j);
-                        if (seen == EMPTY_KEY) { ++mine; break; }
+                        if (seen == EMPTY_KEY) { if (!COMP || !mask_blocks(p.m_col, ms, me, j)) ++mine; break; }
                         if (seen == j) break;
                         s = (s + 1) & tmask;
                     }
@@ -255,12 +272,13 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int *s_warp, int *tot
 // power of two of the row's own product count, and equal columns are COMPRESSED by folding their values in position order.  No
 // atomics and no table to clear; a floating-point PLUS monoid gives the same bit pattern on every run.  One warp per row of the
 // small bin (<= 128 products), one CTA per row of the medium bin (<= 2048).  The row's output count comes from the symbolic
-// pass (c_ptr).
+// pass (c_ptr).  COMP: a column blocked by M' is dropped at the compress step, one test per distinct column, and output positions
+// are ranks among the survivors (the symbolic pass counted the same survivors).
 static constexpr int ESC_SMALL = 128, ESC_MEDIUM = 2048;
 static constexpr size_t ESC_SMEM_SMALL = (size_t)8 * ESC_SMALL * 16;                       // 8 warps x (keys 8 B + value words 8 B)
 static constexpr size_t ESC_SMEM_MEDIUM = (size_t)ESC_MEDIUM * 16 + 3 * 256 * 4 + 256 * 8;   // + offsets, starts, lengths, A values of a chunk
 
-template <typename XT, typename ZT, int ADD, int MUL, bool WARP>
+template <typename XT, typename ZT, int ADD, int MUL, bool WARP, bool COMP = false>
 __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
     typedef typename SlotWord<ZT>::W W;
     constexpr int CAP = WARP ? ESC_SMALL : ESC_MEDIUM;
@@ -356,7 +374,8 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
         const bool valid = i < F;
         const unsigned long long e = valid ? keys[i] : 0ull;
         const uint32_t col = (uint32_t)(e >> 32);
-        const bool head = valid && (i == 0 || (uint32_t)(keys[i - 1] >> 32) != col);
+        bool head = valid && (i == 0 || (uint32_t)(keys[i - 1] >> 32) != col);
+        if (COMP && head) head = !mask_blocks(p.m_col, p.m_ptr[row], p.m_ptr[row + 1], col);
         int rank = 0, total = 0;
         if constexpr (WARP) {
             const unsigned m = __ballot_sync(0xffffffffu, head);
@@ -377,7 +396,9 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
     }
 }
 
-template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC>
+// COMP: each CTA owns a second bitmap, the slice gridDim.x slices further on in spa_bits.  M'(row,:) is set into it when the
+// row starts and a product tests it before its atomics, so a blocked column costs no atomic; the sweep clears it.
+template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC, bool COMP = false>
 __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
     typedef typename SlotWord<ZT>::W W;
     __shared__ int s_warp[33];
@@ -385,6 +406,7 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
     const int add = ADD >= 0 ? ADD : p.add_op;
     const int mul = MUL >= 0 ? MUL : p.mul_op;
     uint32_t *bits = p.spa_bits + (size_t)blockIdx.x * p.spa_words;
+    uint32_t *mbits = COMP ? p.spa_bits + (size_t)(gridDim.x + blockIdx.x) * p.spa_words : nullptr;
     W *spa = NUMERIC ? static_cast<W *>(p.spa_val) + (size_t)blockIdx.x * p.ncols : nullptr;
     const W ident = pack_slot<ZT>(accum_init<ZT>(add));
     const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
@@ -397,6 +419,13 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
         if (idx >= p.nbin) break;
         const int64_t row = p.rows[idx];
         const uint32_t as = p.a_ptr[row], ae = p.a_ptr[row + 1];
+        if (COMP) {
+            for (uint32_t q = p.m_ptr[row] + threadIdx.x; q < p.m_ptr[row + 1]; q += blockDim.x) {
+                const uint32_t j = __ldg(p.m_col + q);
+                atomicOr(&mbits[j >> 5], 1u << (j & 31));
+            }
+            __syncthreads();
+        }
         for (uint32_t pa = as + warp; pa < ae; pa += nwarps) {
             const uint32_t k = p.a_col[pa];
             XT av = (XT)1;
@@ -404,6 +433,7 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
             for (uint32_t pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
                 const uint32_t j = __ldg(p.b_col + pb);
                 const uint32_t bit = 1u << (j & 31);
+                if (COMP && (mbits[j >> 5] & bit)) continue;
                 if (!(bits[j >> 5] & bit)) atomicOr(&bits[j >> 5], bit);
                 if (NUMERIC) {
                     const XT bv = p.need_b ? gload<XT>(bval + pb) : (XT)1;
@@ -417,6 +447,7 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
         const int64_t w0 = (int64_t)threadIdx.x * per, w1 = min(w0 + per, p.spa_words);
         int cnt = 0;
         for (int64_t w = w0; w < w1; ++w) cnt += __popc(bits[w]);
+        if (COMP) for (int64_t w = w0; w < w1; ++w) if (mbits[w]) mbits[w] = 0;
         int total = 0;
         int off = block_exclusive_scan(cnt, s_warp, &total);
         if (NUMERIC) {
@@ -440,6 +471,140 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
             if (threadIdx.x == 0) p.c_cnt[row] = total;
         }
         __syncthreads();
+    }
+}
+
+// ------------------------------------------------------------------ complemented mask: split dense accumulators (spa-split)
+// Rows with more than SPLIT_FLOPS products are spread over the whole GPU instead of owning one CTA of spa_kernel.  They are
+// processed in groups; each row of a group (its slot) owns a dense accumulator, a presence bitmap and a bitmap of M'(row,:) in
+// HBM.  A(row,:) is cut into chunks of about CHUNK_FLOPS products (equal runs of A entries) that persistent CTAs take from a
+// queue.  The sweeps split each row into ranges of SPLIT_RANGE_WORDS bitmap words, one CTA per (range, slot).
+struct SplitArgs {
+    const uint32_t *a_col; const void *a_val; const uint32_t *b_ptr, *b_col; const void *b_val;
+    const uint32_t *m_ptr, *m_col;
+    const int32_t *rows;                 // the rows of the group, by slot
+    const uint32_t *chunks;              // per chunk: slot, first A entry, end A entry
+    int64_t nchunks; unsigned int *queue;
+    uint32_t *pres, *mbit; void *acc;    // per slot: words bitmap words, ncols accumulator words
+    int64_t words, ncols, nrange;
+    int add_op, mul_op, need_a, need_b;
+    int64_t *c_cnt; const int64_t *c_ptr; uint32_t *c_col; void *c_val;
+    int64_t *range_cnt;                  // numeric: per (slot, range) count, then its exclusive scan
+};
+static constexpr int64_t SPLIT_RANGE_WORDS = 2048;
+
+// M'(row,:) into the mask bitmap of every slot (blockIdx.y = slot)
+__global__ void split_mask_kernel(const SplitArgs s) {
+    const int64_t row = s.rows[blockIdx.y];
+    uint32_t *mb = s.mbit + (size_t)blockIdx.y * s.words;
+    for (uint32_t q = s.m_ptr[row] + blockIdx.x * blockDim.x + threadIdx.x; q < s.m_ptr[row + 1]; q += gridDim.x * blockDim.x) {
+        const uint32_t j = __ldg(s.m_col + q);
+        atomicOr(&mb[j >> 5], 1u << (j & 31));
+    }
+}
+
+template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC>
+__global__ void __launch_bounds__(512) split_chunk_kernel(const SplitArgs s) {
+    typedef typename SlotWord<ZT>::W W;
+    __shared__ unsigned int s_next;
+    const int add = ADD >= 0 ? ADD : s.add_op;
+    const int mul = MUL >= 0 ? MUL : s.mul_op;
+    const XT *aval = static_cast<const XT *>(s.a_val), *bval = static_cast<const XT *>(s.b_val);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    while (true) {
+        if (threadIdx.x == 0) s_next = atomicAdd(s.queue, 1u);
+        __syncthreads();
+        const unsigned int idx = s_next;
+        __syncthreads();
+        if (idx >= s.nchunks) break;
+        const uint32_t slot = s.chunks[3 * (size_t)idx], pa0 = s.chunks[3 * (size_t)idx + 1], pa1 = s.chunks[3 * (size_t)idx + 2];
+        uint32_t *bits = s.pres + (size_t)slot * s.words;
+        const uint32_t *mb = s.mbit + (size_t)slot * s.words;
+        W *acc = NUMERIC ? static_cast<W *>(s.acc) + (size_t)slot * s.ncols : nullptr;
+        for (uint32_t pa = pa0 + warp; pa < pa1; pa += nwarps) {
+            const uint32_t k = s.a_col[pa];
+            XT av = (XT)1;
+            if (NUMERIC && s.need_a) av = gload<XT>(aval + pa);
+            for (uint32_t pb = s.b_ptr[k] + lane; pb < s.b_ptr[k + 1]; pb += 32) {
+                const uint32_t j = __ldg(s.b_col + pb);
+                const uint32_t bit = 1u << (j & 31);
+                if (mb[j >> 5] & bit) continue;
+                if (!(bits[j >> 5] & bit)) atomicOr(&bits[j >> 5], bit);
+                if (NUMERIC) {
+                    const XT bv = s.need_b ? gload<XT>(bval + pb) : (XT)1;
+                    atomic_combine<ZT>(&acc[j], MulApply<XT, ZT>::f(mul, av, bv), add);
+                }
+            }
+        }
+    }
+}
+
+// popcount of one (range, slot): symbolic (CLEAR) adds it to c_cnt[row] and clears both bitmaps of the range; numeric stores it
+template <bool CLEAR>
+__global__ void __launch_bounds__(256) split_count_kernel(const SplitArgs s) {
+    __shared__ int s_warp[33];
+    const int64_t slot = blockIdx.y, r = blockIdx.x;
+    const int64_t w0 = r * SPLIT_RANGE_WORDS, w1 = min(w0 + SPLIT_RANGE_WORDS, s.words);
+    uint32_t *bits = s.pres + (size_t)slot * s.words, *mb = s.mbit + (size_t)slot * s.words;
+    int cnt = 0;
+    for (int64_t w = w0 + threadIdx.x; w < w1; w += blockDim.x) {
+        const uint32_t m = bits[w];
+        cnt += __popc(m);
+        if (CLEAR) { if (m) bits[w] = 0; if (mb[w]) mb[w] = 0; }
+    }
+    int total = 0;
+    block_exclusive_scan(cnt, s_warp, &total);
+    if (threadIdx.x == 0) {
+        if (CLEAR) { if (total) atomicAdd(reinterpret_cast<unsigned long long *>(&s.c_cnt[s.rows[slot]]), (unsigned long long)total); }
+        else s.range_cnt[slot * s.nrange + r] = total;
+    }
+}
+
+// ordered sweep of one (range, slot): the entries go out sorted at c_ptr[row] + (their range's offset within the row), the
+// accumulator words are reset to ident and both bitmaps cleared
+template <typename ZT>
+__global__ void __launch_bounds__(256) split_fill_kernel(const SplitArgs s, typename SlotWord<ZT>::W ident) {
+    typedef typename SlotWord<ZT>::W W;
+    __shared__ int s_warp[33];
+    const int64_t slot = blockIdx.y, r = blockIdx.x;
+    const int64_t w0r = r * SPLIT_RANGE_WORDS, w1r = min(w0r + SPLIT_RANGE_WORDS, s.words);
+    uint32_t *bits = s.pres + (size_t)slot * s.words, *mb = s.mbit + (size_t)slot * s.words;
+    W *acc = static_cast<W *>(s.acc) + (size_t)slot * s.ncols;
+    const int64_t per = ceil_div(w1r - w0r, (int64_t)blockDim.x);
+    const int64_t w0 = w0r + (int64_t)threadIdx.x * per, w1 = min(w0 + per, w1r);
+    int cnt = 0;
+    for (int64_t w = w0; w < w1; ++w) cnt += __popc(bits[w]);
+    int total = 0;
+    int off = block_exclusive_scan(cnt, s_warp, &total);
+    const int64_t row = s.rows[slot];
+    const int64_t base = s.c_ptr[row] + s.range_cnt[slot * s.nrange + r] - s.range_cnt[slot * s.nrange];
+    ZT *cval = static_cast<ZT *>(s.c_val);
+    for (int64_t w = w0; w < w1; ++w) {
+        if (mb[w]) mb[w] = 0;
+        uint32_t m = bits[w];
+        if (!m) continue;
+        bits[w] = 0;
+        while (m) {
+            const int b = __ffs(m) - 1; m &= m - 1;
+            const uint32_t j = (uint32_t)(w * 32 + b);
+            s.c_col[base + off] = j;
+            cval[base + off] = unpack_slot<ZT>(acc[j]);
+            acc[j] = ident;
+            ++off;
+        }
+    }
+}
+
+// the rows of the dense-accumulator bin with more than split_flops products leave it: (row, flops, A range) into the split list
+__global__ void split_pick_kernel(const int32_t *rows, int64_t n, const int64_t *flops, int64_t split_flops, const uint32_t *a_ptr,
+                                  int32_t *keep, int64_t *split, unsigned int *counters) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t row = rows[r];
+        const int64_t f = flops[row];
+        if (f > split_flops) {
+            const unsigned int q = atomicAdd(&counters[1], 1u);
+            split[4 * (size_t)q] = row; split[4 * (size_t)q + 1] = f; split[4 * (size_t)q + 2] = a_ptr[row]; split[4 * (size_t)q + 3] = a_ptr[row + 1];
+        } else keep[atomicAdd(&counters[0], 1u)] = row;
     }
 }
 
@@ -717,6 +882,10 @@ static GrB_Info read_counts(const unsigned int *d, unsigned int *h, int n, std::
 static constexpr int SMALL_TABLE = 256, SMALL_FLOPS = 128;      // warp per row
 static constexpr int MEDIUM_TABLE = 4096, MEDIUM_FLOPS = 2048;  // CTA per row
 static constexpr int MIDSMALL_TABLE = 1024;                       // masked: CTA per chunk, mask rows up to 512 entries
+static constexpr int64_t CHUNK_FLOPS = 32768;     // flop budget of one CTA-level work unit
+// complemented mask: rows with more products go to spa-split (DESIGN.md section 3.2); the HBM buffers of one group of split rows
+static constexpr int64_t SPLIT_FLOPS = (int64_t)1 << 18;
+static constexpr int64_t SPLIT_BUDGET = (int64_t)1 << 28;
 
 // dispatch helpers: KERNEL is a macro taking (XT, ZT, ADD, MUL)
 #define GB_FOR_SEMIRING(xt, zt, add, mul, KERNEL, err)                                                        \
@@ -757,9 +926,108 @@ static size_t masked_smem(int table, int groups, size_t wsize) {
     return (size_t)groups * ((per + 15) & ~(size_t)15);
 }
 
-// T = A (+).(x) B, unmasked.  A and B values already of the multiply's operand type.
+// The split rows of a complemented product: slots in row order, groups of `group` rows, the chunk list of each group
+struct SplitPlan {
+    int64_t nsplit = 0, nkeep = 0, group = 0, ncols = 0, words = 0, nrange = 0;
+    DevBuf<int32_t> keep;                        // the rows that stay in spa_kernel
+    std::vector<int64_t> chunk_off;              // per group: its first chunk; one more entry at the end
+    int32_t *rows = nullptr; uint32_t *chunks = nullptr;
+    void *acc = nullptr; uint32_t *pres = nullptr, *mbit = nullptr; int64_t *range_cnt = nullptr;
+    DevBuf<unsigned int> queue;
+};
+
+static GrB_Info split_prepare(const RowBins &bins, const int64_t *flops, const Csr &A, int64_t ncols, size_t wsize, SplitPlan &sp,
+                              std::string *err) {
+    const unsigned int n3 = bins.count[3];
+    DevBuf<unsigned int> cnt; DevBuf<int64_t> picked;
+    GB_TRY(cnt.alloc(2, err));
+    CU_TRY(cudaMemsetAsync(cnt, 0, 8, G.stream), err);
+    GB_TRY(sp.keep.alloc(n3, err)); GB_TRY(picked.alloc((size_t)4 * n3, err));
+    split_pick_kernel<<<grid_for(n3), 256, 0, G.stream>>>(bins.rows + bins.offset[3], n3, flops, SPLIT_FLOPS, A.rowptr32, sp.keep, picked, cnt);
+    GB_LAUNCHED();
+    unsigned int h[2];
+    GB_TRY(read_counts(cnt, h, 2, err));
+    sp.nkeep = h[0]; sp.nsplit = h[1];
+    if (!sp.nsplit) { sp.keep.reset(); return GrB_SUCCESS; }
+    std::vector<int64_t> hs((size_t)4 * sp.nsplit);
+    CU_TRY(cudaMemcpyAsync(hs.data(), picked, hs.size() * 8, cudaMemcpyDeviceToHost, G.stream), err);
+    CU_TRY(cudaStreamSynchronize(G.stream), err);
+    std::vector<int64_t> ord((size_t)sp.nsplit);
+    for (int64_t q = 0; q < sp.nsplit; ++q) ord[q] = q;
+    std::sort(ord.begin(), ord.end(), [&](int64_t x, int64_t y) { return hs[4 * x] < hs[4 * y]; });
+    sp.ncols = ncols; sp.words = ceil_div(ncols, 32); sp.nrange = ceil_div(sp.words, SPLIT_RANGE_WORDS);
+    const int64_t per_row = ncols * (int64_t)wsize + 2 * sp.words * 4;
+    sp.group = std::max<int64_t>(1, std::min<int64_t>(sp.nsplit, SPLIT_BUDGET / per_row));
+    std::vector<int32_t> rows;
+    std::vector<uint32_t> chunks;
+    sp.chunk_off.assign(1, 0);
+    for (int64_t q = 0; q < sp.nsplit; ++q) {
+        const int64_t *e = &hs[4 * ord[q]];
+        rows.push_back((int32_t)e[0]);
+        const int64_t as = e[2], len = e[3] - e[2];
+        const int64_t n = std::max<int64_t>(1, std::min<int64_t>(len, ceil_div(e[1], CHUNK_FLOPS)));
+        for (int64_t c = 0; c < n; ++c) {
+            chunks.push_back((uint32_t)(q % sp.group));
+            chunks.push_back((uint32_t)(as + len * c / n)); chunks.push_back((uint32_t)(as + len * (c + 1) / n));
+        }
+        if ((q + 1) % sp.group == 0 || q + 1 == sp.nsplit) sp.chunk_off.push_back((int64_t)chunks.size() / 3);
+    }
+    GB_TRY(ws_array(WS_SPLIT_ROWS, &sp.rows, rows.size(), err));
+    GB_TRY(ws_array(WS_SPLIT_CHUNKS, &sp.chunks, chunks.size(), err));
+    GB_TRY(ws_array(WS_SPLIT_RANGES, &sp.range_cnt, (size_t)(sp.group * sp.nrange + 1), err));
+    void *buf = nullptr;
+    GB_TRY(ws_get(WS_SPLIT_BUF, &buf, (size_t)(sp.group * per_row) + 16, err));
+    sp.acc = buf;
+    sp.pres = reinterpret_cast<uint32_t *>(static_cast<char *>(buf) + (size_t)sp.group * ncols * wsize);
+    sp.mbit = sp.pres + (size_t)sp.group * sp.words;
+    CU_TRY(cudaMemsetAsync(sp.pres, 0, (size_t)sp.group * sp.words * 8, G.stream), err);       // both bitmaps
+    GB_TRY(sp.queue.alloc(1, err));
+    CU_TRY(cudaMemcpyAsync(sp.rows, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, G.stream), err);
+    CU_TRY(cudaMemcpyAsync(sp.chunks, chunks.data(), chunks.size() * 4, cudaMemcpyHostToDevice, G.stream), err);
+    CU_TRY(cudaStreamSynchronize(G.stream), err);      // the host vectors are the sources of the copies
+    return GrB_SUCCESS;
+}
+
+// the launches of group g: its mask bitmaps, then the chunk kernel on a fresh queue; returns the group's argument block
+static SplitArgs split_group(const SplitPlan &sp, const SplitArgs &base, int64_t g, int64_t *ng, std::string *err) {
+    SplitArgs s = base;
+    s.rows = sp.rows + g * sp.group;
+    *ng = std::min(sp.group, sp.nsplit - g * sp.group);
+    s.chunks = sp.chunks + 3 * sp.chunk_off[g];
+    s.nchunks = sp.chunk_off[g + 1] - sp.chunk_off[g];
+    split_mask_kernel<<<dim3((unsigned)std::min<int64_t>(ceil_div(sp.ncols, 256), 128), (unsigned)*ng), 256, 0, G.stream>>>(s);
+    GB_LAUNCHED();
+    cudaMemsetAsync(s.queue, 0, 4, G.stream);          // errors surface at the caller's cudaGetLastError
+    return s;
+}
+static int split_ctas(int64_t nchunks) { return (int)std::max<int64_t>(1, std::min<int64_t>(nchunks, (int64_t)G.num_sms * 2)); }
+
+template <typename XT, typename ZT, int ADD, int MUL>
+static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgs &base, std::string *err) {
+    typedef typename SlotWord<ZT>::W W;
+    const int add = ADD >= 0 ? ADD : base.add_op;
+    fill_words_kernel<W><<<grid_for(sp.group * sp.ncols), 256, 0, G.stream>>>(static_cast<W *>(sp.acc), pack_slot<ZT>(accum_init<ZT>(add)),
+                                                                                 sp.group * sp.ncols);
+    GB_LAUNCHED();
+    for (int64_t g = 0; g + 1 < (int64_t)sp.chunk_off.size(); ++g) {
+        int64_t ng = 0;
+        const SplitArgs s = split_group(sp, base, g, &ng, err);
+        split_chunk_kernel<XT, ZT, ADD, MUL, true><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
+        split_count_kernel<false><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
+        CU_TRY(cudaMemsetAsync(sp.range_cnt + ng * sp.nrange, 0, 8, G.stream), err);
+        GB_TRY(dev_exclusive_scan(sp.range_cnt, ng * sp.nrange + 1, err));
+        split_fill_kernel<ZT><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s, pack_slot<ZT>(accum_init<ZT>(add)));
+        G.launches += 4;
+    }
+    CU_TRY(cudaGetLastError(), err);
+    return GrB_SUCCESS;
+}
+
+// T = A (+).(x) B, unmasked.  A and B values already of the multiply's operand type.  With Mb (the entries of a complemented
+// mask that block, see mask_true_pattern) holding entries, T = (A (+).(x) B)<!Mb>: the same bins, chosen by the unfiltered
+// product counts, run their COMP instantiations, which never form a blocked entry.
 static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt,
-                                int add, int mul, bool need_a, bool need_b, Csr &T, std::string *err) {
+                                int add, int mul, bool need_a, bool need_b, const Csr *Mb, Csr &T, std::string *err) {
     const int64_t nrows = A.nrows, ncols = B.ncols;
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
     GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
@@ -772,35 +1040,57 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
     int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
     G.last_flops = (uint64_t)total_flops;
+    const bool comp = Mb && Mb->nnz > 0;
+    const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
+    // the dense-accumulator bin: with a complemented mask its rows above SPLIT_FLOPS go to spa-split
+    SplitPlan sp;
+    if (comp && bins.count[3]) GB_TRY(split_prepare(bins, flops, A, ncols, wsize, sp, err));
+    const int32_t *spa_rows = sp.nsplit ? sp.keep.get() : bins.rows + bins.offset[3];
+    const int64_t spa_n = sp.nsplit ? sp.nkeep : (int64_t)bins.count[3];
     flops.reset(); total.reset();
 
     GemmArgs g{};
     g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
     g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
     g.c_cnt = T.rowptr;
-    const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
-    const int spa_ctas = std::max(1, std::min<int>((int)bins.count[3], G.num_sms * 2));
+    if (comp) { g.m_ptr = Mb->rowptr32; g.m_col = Mb->col; }
+    SplitArgs sa{};
+    sa.a_col = A.col; sa.a_val = aval; sa.b_ptr = B.rowptr32; sa.b_col = B.col; sa.b_val = bval; sa.m_ptr = g.m_ptr; sa.m_col = g.m_col;
+    sa.queue = sp.queue; sa.pres = sp.pres; sa.mbit = sp.mbit; sa.acc = sp.acc; sa.words = sp.words; sa.ncols = ncols; sa.nrange = sp.nrange;
+    sa.add_op = add; sa.mul_op = mul; sa.need_a = need_a; sa.need_b = need_b; sa.c_cnt = T.rowptr; sa.range_cnt = sp.range_cnt;
+    const int spa_ctas = std::max(1, std::min<int>((int)spa_n, G.num_sms * 2));
     DevBuf<unsigned int> queue; DevBuf<uint32_t> spa_bits;
-    if (bins.count[3]) {
+    if (spa_n) {
         g.spa_words = ceil_div(ncols, 32);
-        GB_TRY(spa_bits.alloc((size_t)spa_ctas * g.spa_words, err));
+        const size_t words = (size_t)spa_ctas * g.spa_words * (comp ? 2 : 1);     // comp: + the mask bitmaps
+        GB_TRY(spa_bits.alloc(words, err));
         g.spa_bits = spa_bits;
-        CU_TRY(cudaMemsetAsync(g.spa_bits, 0, (size_t)spa_ctas * g.spa_words * 4, G.stream), err);
+        CU_TRY(cudaMemsetAsync(g.spa_bits, 0, words * 4, G.stream), err);
         GB_TRY(queue.alloc(2, err));
         CU_TRY(cudaMemsetAsync(queue, 0, 8, G.stream), err);
     }
     // ---- symbolic
     if (bins.count[1]) {
         g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1]; g.table = SMALL_TABLE;
-        hash_symbolic_kernel<true><<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g); GB_LAUNCHED();
+        (comp ? hash_symbolic_kernel<true, true> : hash_symbolic_kernel<true>)<<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g);
+        GB_LAUNCHED();
     }
     if (bins.count[2]) {
         g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
-        hash_symbolic_kernel<false><<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g); GB_LAUNCHED();
+        (comp ? hash_symbolic_kernel<false, true> : hash_symbolic_kernel<false>)<<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g);
+        GB_LAUNCHED();
     }
-    if (bins.count[3]) {
-        g.rows = bins.rows + bins.offset[3]; g.nbin = bins.count[3]; g.queue = queue;
-        spa_kernel<bool, bool, -1, -1, false><<<spa_ctas, 512, 0, G.stream>>>(g); GB_LAUNCHED();
+    if (spa_n) {
+        g.rows = spa_rows; g.nbin = spa_n; g.queue = queue;
+        (comp ? spa_kernel<bool, bool, -1, -1, false, true> : spa_kernel<bool, bool, -1, -1, false>)<<<spa_ctas, 512, 0, G.stream>>>(g);
+        GB_LAUNCHED();
+    }
+    for (int64_t k = 0; k + 1 < (int64_t)sp.chunk_off.size(); ++k) {
+        int64_t ng = 0;
+        const SplitArgs s = split_group(sp, sa, k, &ng, err);
+        split_chunk_kernel<bool, bool, -1, -1, false><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
+        split_count_kernel<true><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
+        G.launches += 2;
     }
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
@@ -811,23 +1101,30 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
     // ---- numeric (shared-memory bins: expand-sort-compress)
     if (bins.count[1]) {
         g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1];
-#define K_ESC_SMALL(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, true><<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
+#define K_ESC_SMALL(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, true, true> : esc_numeric_kernel<XT, ZT, A_, M_, true>) \
+            <<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); GB_LAUNCHED(); gb_kernel_used("esc-small");
     }
     if (bins.count[2]) {
         g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2];
-#define K_ESC_MEDIUM(XT, ZT, A_, M_) esc_numeric_kernel<XT, ZT, A_, M_, false><<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
+#define K_ESC_MEDIUM(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, false, true> : esc_numeric_kernel<XT, ZT, A_, M_, false>) \
+            <<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); GB_LAUNCHED(); gb_kernel_used("esc-medium");
     }
-    if (bins.count[3]) {
-        g.rows = bins.rows + bins.offset[3]; g.nbin = bins.count[3]; g.queue = queue + 1;
+    if (spa_n) {
+        g.rows = spa_rows; g.nbin = spa_n; g.queue = queue + 1;
         DevBuf<void> spa_val;
         GB_TRY(spa_val.alloc((size_t)spa_ctas * ncols * wsize + 16, err));
         g.spa_val = spa_val;
 #define K_SPA(XT, ZT, A_, M_) do { \
         fill_accum_init<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
-        spa_kernel<XT, ZT, A_, M_, true><<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
+        (comp ? spa_kernel<XT, ZT, A_, M_, true, true> : spa_kernel<XT, ZT, A_, M_, true>)<<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2; gb_kernel_used("spa");
+    }
+    if (sp.nsplit) {
+        sa.c_ptr = T.rowptr; sa.c_col = T.col; sa.c_val = T.val;
+#define K_SPLIT(XT, ZT, A_, M_) GB_TRY((split_numeric<XT, ZT, A_, M_>(sp, sa, err)))
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_SPLIT, err); gb_kernel_used("spa-split");
     }
     spa_bits.reset(); queue.reset(); bins.rows.reset();
     GB_TRY(dev_build_rowptr32(T, err));
@@ -837,8 +1134,7 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
 
 // T<M> = A (+).(x) B restricted to a non-complemented mask M (pattern of T is a subset of M's).
 // dot == true computes A (+).(x) B' by row intersections instead (B given un-transposed).
-static constexpr int64_t CHUNK_FLOPS = 32768;     // flop budget of one CTA-level work unit
-static constexpr int WARP_FLOPS = 2048;           // rows at most this heavy (and with short mask rows) run warp-per-row
+static constexpr int WARP_FLOPS = 2048;          // rows at most this heavy (and with short mask rows) run warp-per-row
 
 // B200GRB_SPGEMM_TRACE=1: device time of the phases of one masked call (events on the compute stream), printed to stderr
 struct PhaseTrace {
@@ -1063,13 +1359,13 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
 // index, side 2 = each entry of op(B) its row index; through ids (hypersparse operands) when given, plus off, of type tc
 struct MxmPos { int side = 0; int tc = 0; int64_t off = 0; const uint64_t *ids = nullptr; };
 
-// T = op(A) (+).(x) op(B), masked by Mask when it is not complemented (*masked tells the write-back)
+// T = op(A) (+).(x) op(B) under Mask (*masked tells the write-back): a mask that is not complemented selects the masked
+// methods; a complemented one runs the unmasked bins with the filter of the entries that block (DESIGN.md section 3.2)
 static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, int zt, int add, int mul, const GrB_Matrix A, const GrB_Matrix B,
                             const MxmPos &pos, Csr &T, bool *masked, std::string *err) {
     const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
-    // masked methods apply to non-complemented masks
     const bool use_mask = Mask && !f.mask_comp;
-    *masked = use_mask;
+    *masked = Mask != nullptr;
     if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
     GB_TRY(matrix_ensure_device(B));
     // C<M> = A*B': small problems intersect rows of A and B directly (no transpose); large ones
@@ -1098,7 +1394,13 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
 
     GrB_Info r;
     if (use_mask) r = spgemm_masked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, Mask->dev, Mask->type->code, f.mask_struct, dot, T, err);
-    else r = spgemm_unmasked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, T, err);
+    else {
+        Csr mtrue;                              // a valued complemented mask: its true entries
+        const Csr *mb = nullptr;
+        if (Mask && f.mask_struct) mb = &Mask->dev;
+        else if (Mask) { GB_TRY(mask_true_pattern(Mask->dev, Mask->type->code, mtrue, err)); mb = &mtrue; }
+        r = spgemm_unmasked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, T, err);
+    }
     a_cast.reset(); b_cast.reset();
     return r;
 }

@@ -27,6 +27,7 @@
 struct B200_Comm_opaque {
     int magic; int rank, world;
     uint64_t n;                 // length of the replicated vectors
+    GrB_Type type;              // type of the replicated vectors: every slice and partial must have it
     size_t esize;               // bytes per value (<= 8)
     size_t val_bytes, pres_bytes, buf_bytes, region_bytes;
     unsigned char *region = nullptr;                 // this rank's exchange region
@@ -56,7 +57,7 @@ extern "C" GrB_Info B200_Comm_create(B200_Comm *comm, int rank, int world, GrB_I
     if (n == 0 || n >= ((uint64_t)1 << 31)) return gb_fail(GrB_INVALID_VALUE, nullptr, "B200_Comm_create: vector length must be in [1, 2^31)");
     if (!G.have_device) return gb_fail(GrB_PANIC, nullptr, "B200_Comm_create: no CUDA device: the exchange runs only over GPU peer memory (no CPU fallback)");
     B200_Comm c = new B200_Comm_opaque();
-    c->magic = GB_MAGIC; c->rank = rank; c->world = world; c->n = n; c->esize = type->size;
+    c->magic = GB_MAGIC; c->rank = rank; c->world = world; c->n = n; c->type = type; c->esize = type->size;
     c->val_bytes = (((size_t)n * c->esize) + 255) & ~(size_t)255;
     c->pres_bytes = ((size_t)n + 255) & ~(size_t)255;
     c->buf_bytes = c->val_bytes + c->pres_bytes;
@@ -151,6 +152,29 @@ __global__ void __launch_bounds__(512) comm_push_kernel(const uint4 *vsrc, size_
     if (threadIdx.x == 0) __threadfence_system();      // cumulative over the CTA's stores (ordered before it by the barrier)
 }
 
+// the bytes after the last whole 16-byte word of each array: thread t < vtail copies value byte vsrc[t] to dst[peer] + voff + t,
+// the next ptail threads presence bytes likewise.  A separate launch, only for slices that end inside a word, so that the word
+// loop above stays as it was and nothing outside the slice is read or written.
+__global__ void comm_push_tail_kernel(const unsigned char *vsrc, int vtail, size_t voff, const unsigned char *psrc, int ptail, size_t poff,
+                                      PeerPtrs dst, int world) {
+    const int t = threadIdx.x;
+    if (t < vtail + ptail) {
+        const bool isv = t < vtail;
+        const unsigned char x = isv ? vsrc[t] : psrc[t - vtail];
+        const size_t o = isv ? voff + t : poff + (t - vtail);
+        for (int p = 0; p < world; ++p) dst.p[p][o] = x;
+    }
+    __threadfence_system();
+}
+
+// the device-wide nanosecond clock: unlike clock64 it neither depends on the SM clock nor differs between the SMs a preempted
+// warp may resume on
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
 // one warp: lane p raises this rank's flag (slot, value `step`) in rank p's region, then waits until rank p's flag here shows `step`
 __global__ void comm_signal_wait_kernel(PeerPtrs regions, size_t flag_off, const unsigned long long *my_flags, int world, int rank, int flag_slot,
                                         unsigned long long step) {
@@ -160,10 +184,10 @@ __global__ void comm_signal_wait_kernel(PeerPtrs regions, size_t flag_off, const
         asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(f), "l"(step) : "memory");
         const unsigned long long *g = my_flags + flag_slot * MAX_WORLD + threadIdx.x;
         unsigned long long v;
-        const long long t0 = clock64();
+        const unsigned long long t0 = globaltimer_ns();
         do {
             asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(g) : "memory");
-            if (v < step && clock64() - t0 > 40000000000ll) asm volatile("trap;");       // ~20 s: a peer died -- fail loudly instead of hanging the GPU
+            if (v < step && globaltimer_ns() - t0 > 20000000000ull) asm volatile("trap;");   // 20 s: a peer died -- fail loudly instead of hanging the GPU
         } while (v < step);
     }
     __syncwarp();
@@ -181,7 +205,7 @@ __global__ void __launch_bounds__(256) comm_fold_kernel(PeerPtrs part, int world
             const uint8_t pr = reinterpret_cast<const volatile uint8_t *>(part.p[p] + val_bytes)[i];
             if (pr) {
                 const T v = reinterpret_cast<const T *>(part.p[p])[i];
-                acc = has ? op_apply<T>(op, acc, v) : v; has = true;
+                acc = has ? MulApply<T, T>::f(op, acc, v) : v; has = true;      // the rule of every typed fold: OP_EQ is LXNOR
             }
         }
         oval[k] = acc; opres[k] = has;
@@ -205,15 +229,22 @@ static void comm_signal_wait(B200_Comm c, int slot, unsigned long long step) {
     comm_signal_wait_kernel<<<1, 32, 0, G.stream>>>(regions, 3 * c->buf_bytes, comm_flags(c, c->region), c->world, c->rank, slot, step); GB_LAUNCHED();
 }
 
-// push (vals, pres) of `len` positions starting at row0 into buffer `which` of every rank, raise flag slot 0, wait for everybody
+// push (vals, pres) of `len` positions starting at row0 into buffer `which` of every rank, raise flag slot 0, wait for everybody.
+// Exactly [row0, row0 + len) is written: positions no rank's slice covers keep whatever the buffer held (unspecified; zero in a
+// communicator's first two collectives).
 static GrB_Info comm_push_and_wait(B200_Comm c, const void *vals, const uint8_t *pres, uint64_t row0, uint64_t len, int which) {
-    // slices start at multiples of 16 positions (the partition guarantees it) so that both arrays move as 16-byte words
+    // non-empty slices start at multiples of 16 positions (the partition guarantees it) so that both arrays move as 16-byte words
     PeerPtrs dst{};
     for (int p = 0; p < c->world; ++p) dst.p[p] = comm_buf(c, c->peer[p], which);
-    const size_t vbytes = ((size_t)len * c->esize + 15) & ~(size_t)15, pbytes = ((size_t)len + 15) & ~(size_t)15;
+    const size_t vall = (size_t)len * c->esize, vbytes = vall & ~(size_t)15, pbytes = (size_t)len & ~(size_t)15;
+    const size_t voff = (size_t)row0 * c->esize, poff = c->val_bytes + (size_t)row0;
     const unsigned long long step = c->step + 1;
-    if (len) { comm_push_kernel<<<pgrid(vbytes + pbytes), 512, 0, G.stream>>>((const uint4 *)vals, vbytes, (size_t)row0 * c->esize, (const uint4 *)pres, pbytes,
-                                                                              c->val_bytes + (size_t)row0, dst, c->world); GB_LAUNCHED(); }
+    if (vbytes + pbytes) { comm_push_kernel<<<pgrid(vbytes + pbytes), 512, 0, G.stream>>>((const uint4 *)vals, vbytes, voff, (const uint4 *)pres, pbytes, poff,
+                                                                                        dst, c->world); GB_LAUNCHED(); }
+    if (vall > vbytes || len > pbytes) {
+        comm_push_tail_kernel<<<1, 32, 0, G.stream>>>((const unsigned char *)vals + vbytes, (int)(vall - vbytes), voff + vbytes, pres + pbytes, (int)(len - pbytes),
+                                                      poff + pbytes, dst, c->world); GB_LAUNCHED();
+    }
     comm_signal_wait(c, 0, step);
     CU_TRY(cudaGetLastError(), &c->err);
     c->step = step;
@@ -225,7 +256,7 @@ static GrB_Info comm_check(B200_Comm c, const GrB_Vector v, const char *fn) {
     if (!comm_ok(c) || !v) return gb_fail(GrB_NULL_POINTER, nullptr, "%s: invalid argument", fn);
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid vector", fn);
     if (!c->connected) return gb_fail(GrB_INVALID_VALUE, &c->err, "%s: B200_Comm_connect has not been called", fn);
-    if (v->type->size != c->esize) return gb_fail(GrB_DOMAIN_MISMATCH, &c->err, "%s: the vector's type does not match the communicator's", fn);
+    if (v->type->code != c->type->code) return gb_fail(GrB_DOMAIN_MISMATCH, &c->err, "%s: the vector's type does not match the communicator's", fn);
     return GrB_SUCCESS;
 }
 
@@ -237,7 +268,8 @@ __global__ void fill_bytes_kernel(uint8_t *p, int64_t n, uint8_t v) {
 extern "C" GrB_Info B200_Comm_allgather(B200_Comm c, const GrB_Vector slice, GrB_Index row0) {
     GB_LOCK; GB_CHECK_INIT;
     GB_TRY(comm_check(c, slice, "B200_Comm_allgather"));
-    if (row0 + slice->n > c->n || (row0 & 15)) return gb_fail(GrB_INVALID_VALUE, &c->err, "B200_Comm_allgather: slice [%llu, +%llu) must lie inside the vector and start at a multiple of 16",
+    // an empty slice writes nothing and is valid at any row0 <= n (equal_row_blocks starts empty trailing blocks at n)
+    if (row0 + slice->n > c->n || (slice->n && (row0 & 15))) return gb_fail(GrB_INVALID_VALUE, &c->err, "B200_Comm_allgather: slice [%llu, +%llu) must lie inside the vector and, unless empty, start at a multiple of 16",
                                                             (unsigned long long)row0, (unsigned long long)slice->n);
     GbBurble burble("B200_Comm_allgather");
     GB_TRY(vector_ensure_device(slice));

@@ -355,7 +355,7 @@ static constexpr int SPMM_SEG = 64;
 GrB_Info dense_transpose(const void *val, const uint8_t *pres, int64_t rows, int64_t cols, size_t vsize, void *oval, uint8_t *opres,
                          std::string *err);
 // (pattern of M, one found flag and one value of vsize bytes per entry of M) -> the CSR T of the found entries, rowptr32
-// included; T's dimensions are the caller's (spgemm.cu)
+// included, of M's dimensions (spgemm.cu)
 GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err);
 // the entries of a valued mask M (type mtc) that are true, x != 0 as in mask_value_true (NaN true, +-0 false), as a CSR pattern with
 // 32-bit row pointers: the columns a complemented mask blocks (select_kernel with SEL_NONZERO, matrix_ops.cu)
@@ -810,3 +810,30 @@ static inline int grid_for(int64_t n, int threads = 256, int per_sm = 16) {
 }
 // one 8-byte count from the device (synchronises the compute stream)
 GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err);
+
+// ---------------------------------------------------------------- CSR results
+// op(A): the CSR of A, or of its cached transpose when tran
+static inline GrB_Info source_csr(GrB_Matrix A, bool tran, Csr **out) {
+    if (tran) { GB_TRY(matrix_ensure_transpose(A)); *out = &A->devT; }
+    else { GB_TRY(matrix_ensure_device(A)); *out = &A->dev; }
+    return GrB_SUCCESS;
+}
+// T = a fresh nrows x ncols CSR formed row by row.  count(rowptr) enqueues the work that leaves all nrows + 1 slots defined:
+// the entry count of row r in slot r, 0 in slot nrows.  The slots are scanned into row offsets, T.nnz is read back, and T gets
+// col and, when vsize > 0, val (vsize bytes per entry, plus the 16-byte tail of every value array).  fill(T) writes them and
+// runs only when T has entries.  Both return GrB_Info.  rowptr32 is built last.
+template <typename Count, typename Fill>
+static GrB_Info csr_from_row_counts(int64_t nrows, int64_t ncols, size_t vsize, Csr &T, std::string *err, Count &&count, Fill &&fill) {
+    T = Csr(); T.nrows = nrows; T.ncols = ncols;
+    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
+    GB_TRY(count(T.rowptr.get()));
+    GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
+    GB_TRY(read_i64(T.rowptr + nrows, &T.nnz, err));
+    GB_TRY(T.col.alloc((size_t)T.nnz, err));
+    if (vsize) GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
+    if (T.nnz > 0) GB_TRY(fill(T));
+    return dev_build_rowptr32(T, err);
+}
+// T = src's pattern in fresh arrays, with a value array of vsize bytes per entry holding src's values when with_values
+// (device_ops.cu).  rowptr32 is left to the caller, to be built once the values are in place.
+GrB_Info csr_copy(const Csr &src, size_t vsize, bool with_values, Csr &T, std::string *err);

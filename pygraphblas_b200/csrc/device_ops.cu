@@ -165,6 +165,19 @@ GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int fro
     return GrB_SUCCESS;
 }
 
+GrB_Info csr_copy(const Csr &src, size_t vsize, bool with_values, Csr &T, std::string *err) {
+    T = Csr(); T.nrows = src.nrows; T.ncols = src.ncols; T.nnz = src.nnz;
+    GB_TRY(T.rowptr.alloc((size_t)src.nrows + 1, err));
+    GB_TRY(T.col.alloc((size_t)src.nnz, err));
+    GB_TRY(T.val.alloc((size_t)src.nnz * vsize + 16, err));
+    CU_TRY(cudaMemcpyAsync(T.rowptr, src.rowptr, ((size_t)src.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
+    if (src.nnz) {
+        CU_TRY(cudaMemcpyAsync(T.col, src.col, (size_t)src.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
+        if (with_values) CU_TRY(cudaMemcpyAsync(T.val, src.val, (size_t)src.nnz * vsize, cudaMemcpyDeviceToDevice, G.stream), err);
+    }
+    return GrB_SUCCESS;
+}
+
 GrB_Info read_i64(const int64_t *d, int64_t *h, std::string *err) {
     CU_TRY(cudaMemcpyAsync(h, d, 8, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);

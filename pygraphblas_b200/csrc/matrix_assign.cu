@@ -92,17 +92,9 @@ __global__ void fill_entries_kernel(const int64_t *rowptr, int64_t nrows, const 
     }
 }
 static GrB_Info region_filled(const Region &R, int64_t nrows, int64_t ncols, int tc, Sc x, Csr &T, std::string *err) {
-    T = Csr(); T.nrows = nrows; T.ncols = ncols;
-    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
-    fill_count_kernel<<<grid_for(nrows + 1), 256, 0, G.stream>>>(R.rowflag, nrows, R.nj_distinct, T.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
-    T.nnz = R.ni_distinct * R.nj_distinct;
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(tc) + 16, err));
-    if (T.nnz > 0) { fill_entries_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(T.rowptr, nrows, R.jsorted, T.col, T.val, tc, x); GB_LAUNCHED(); }
-    GB_TRY(dev_build_rowptr32(T, err));
-    CU_TRY(cudaGetLastError(), err);
-    return GrB_SUCCESS;
+    return csr_from_row_counts(nrows, ncols, tc_size(tc), T, err,
+        [&](int64_t *rowptr) { fill_count_kernel<<<grid_for(nrows + 1), 256, 0, G.stream>>>(R.rowflag, nrows, R.nj_distinct, rowptr); GB_LAUNCHED(); return GrB_SUCCESS; },
+        [&](Csr &t) { fill_entries_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(t.rowptr, nrows, R.jsorted, t.col, t.val, tc, x); GB_LAUNCHED(); return GrB_SUCCESS; });
 }
 
 // ------------------------------------------------------------------ C minus the region (entries of C outside I x J)
@@ -129,20 +121,16 @@ __global__ void outside_fill_kernel(const int64_t *ptr, const uint32_t *col, con
     }
 }
 static GrB_Info csr_outside_region(const Csr &c, size_t vsize, const Region &R, Csr &out, std::string *err) {
-    out = Csr(); out.nrows = c.nrows; out.ncols = c.ncols;
-    GB_TRY(out.rowptr.alloc((size_t)c.nrows + 1, err));
-    outside_count_kernel<<<grid_for(c.nrows + 1), 256, 0, G.stream>>>(c.rowptr, c.col, c.nrows, R.rowflag, R.colflag, out.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(out.rowptr, c.nrows + 1, err));
-    GB_TRY(read_i64(out.rowptr + c.nrows, &out.nnz, err));
-    GB_TRY(out.col.alloc((size_t)out.nnz, err));
-    GB_TRY(out.val.alloc((size_t)out.nnz * vsize + 16, err));
-    if (out.nnz > 0) {
-        outside_fill_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr, c.col, (const uint8_t *)c.val, (int)vsize, c.nrows, R.rowflag, R.colflag,
-                                                                  out.rowptr, out.col, (uint8_t *)out.val); GB_LAUNCHED();
-    }
-    GB_TRY(dev_build_rowptr32(out, err));
-    CU_TRY(cudaGetLastError(), err);
-    return GrB_SUCCESS;
+    return csr_from_row_counts(c.nrows, c.ncols, vsize, out, err,
+        [&](int64_t *rowptr) {
+            outside_count_kernel<<<grid_for(c.nrows + 1), 256, 0, G.stream>>>(c.rowptr, c.col, c.nrows, R.rowflag, R.colflag, rowptr); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            outside_fill_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr, c.col, (const uint8_t *)c.val, (int)vsize, c.nrows, R.rowflag, R.colflag,
+                                                                      t.rowptr, t.col, (uint8_t *)t.val); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        });
 }
 
 // ------------------------------------------------------------------ GrB_assign write-back:  C<Mask>(region) = accum(C(region), T)
@@ -160,11 +148,16 @@ static GrB_Info assign_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_
     if (Mask) GB_TRY(GrB_Matrix_dup(&Zm, C));
     GrB_Info r = GrB_SUCCESS;
     if (!accum && !t_covers_region && !whole) {
-        // entries of C inside the region that T lacks are deleted: drop the region from C first
+        // entries of C inside the region that T lacks are deleted: drop the region from C first, into a scratch matrix
+        // when Z would go straight into C, so that a failure later in the call leaves C as it was
         r = matrix_ensure_device(Zm);
         if (r == GrB_SUCCESS && Zm->dev.nnz > 0) {
             Csr keep;
             r = csr_outside_region(Zm->dev, Zm->type->size, R, keep, err);
+            if (r == GrB_SUCCESS && Zm == C) {
+                r = GrB_Matrix_new(&Zm, C->type, C->nrows, C->ncols);      // NULL when it fails
+                C->devT = Csr();        // a cache the result drops anyway: only C's CSR is held beside Z
+            }
             if (r == GrB_SUCCESS) matrix_adopt_device(Zm, std::move(keep));
         }
     }
@@ -172,14 +165,15 @@ static GrB_Info assign_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_
         if (!accum && whole) r = matrix_writeback(Zm, nullptr, nullptr, plain, std::move(T), ttc, false, err);        // Z = T
         else r = matrix_writeback(Zm, nullptr, merge, plain, std::move(T), ttc, false, err);                          // Z = C (+) T
     }
-    if (!Mask || r != GrB_SUCCESS) { if (Zm != C) GrB_Matrix_free(&Zm); return r; }
-    // C<Mask> = Z  (mask and GrB_REPLACE span all of C)
-    r = matrix_ensure_device(Zm);
-    if (r == GrB_SUCCESS) {
-        Csr z = std::move(Zm->dev); Zm->host_valid = true;      // steal Z's CSR (values already of C's type)
-        r = matrix_writeback(C, Mask, nullptr, f, std::move(z), ctc, false, err);
+    if (r == GrB_SUCCESS && Zm != C) {
+        r = matrix_ensure_device(Zm);
+        if (r == GrB_SUCCESS) {
+            Csr z = std::move(Zm->dev); Zm->host_valid = true;      // steal Z's CSR (values already of C's type)
+            if (Mask) r = matrix_writeback(C, Mask, nullptr, f, std::move(z), ctc, false, err);    // C<Mask> = Z (mask and GrB_REPLACE span all of C)
+            else matrix_adopt_device(C, std::move(z));
+        }
     }
-    GrB_Matrix_free(&Zm);
+    if (Zm != C) GrB_Matrix_free(&Zm);
     return r;
 }
 
@@ -285,8 +279,8 @@ extern "C" GrB_Info GrB_Matrix_extract(GrB_Matrix C, const GrB_Matrix Mask, cons
                        (unsigned long long)C->ncols, (unsigned long long)tn, (unsigned long long)tm);
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
     GbBurble burble(fn);
-    if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
-    const Csr &a = f.tran0 ? A->devT : A->dev;
+    Csr *pa; GB_TRY(source_csr(A, f.tran0, &pa));
+    const Csr &a = *pa;
     const size_t vsize = A->type->size;
     DevBuf<uint32_t> d_rows, d_jsv, d_jsq;
     bool need_sort = false;
@@ -299,19 +293,18 @@ extern "C" GrB_Info GrB_Matrix_extract(GrB_Matrix C, const GrB_Matrix Mask, cons
         for (size_t q = 0; q < ord.size(); ++q) { jsv[q] = (uint32_t)Jv[ord[q]]; if (ord[q] != q) need_sort = true; }
         GB_TRY(upload(jsv, d_jsv, err)); GB_TRY(upload(ord, d_jsq, err));
     }
-    Csr T; T.nrows = (int64_t)tn; T.ncols = (int64_t)tm;
-    GB_TRY(T.rowptr.alloc((size_t)tn + 1, err));
-    extract_count_kernel<<<grid_for((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), T.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)tn + 1, err));
-    GB_TRY(read_i64(T.rowptr + tn, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
-    if (T.nnz > 0) {
-        extract_fill_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jsv, d_jsq,
-                                                                    (int64_t)Jv.size(), T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
-        if (need_sort) { rows_insertion_sort_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(T.rowptr, (int64_t)tn, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
-    }
-    GB_TRY(dev_build_rowptr32(T, err));
+    Csr T;
+    GB_TRY(csr_from_row_counts((int64_t)tn, (int64_t)tm, vsize, T, err,
+        [&](int64_t *rowptr) {
+            extract_count_kernel<<<grid_for((int64_t)tn + 1), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, d_jsv, (int64_t)Jv.size(), rowptr); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            extract_fill_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(d_rows, (int64_t)tn, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jsv, d_jsq,
+                                                                        (int64_t)Jv.size(), t.rowptr, t.col, (uint8_t *)t.val); GB_LAUNCHED();
+            if (need_sort) { rows_insertion_sort_kernel<<<grid_for((int64_t)tn), 256, 0, G.stream>>>(t.rowptr, (int64_t)tn, t.col, (uint8_t *)t.val, (int)vsize); GB_LAUNCHED(); }
+            return GrB_SUCCESS;
+        }));
     d_rows.reset(); d_jsv.reset(); d_jsq.reset();
     burble.note("row gather + column map", (double)T.nnz * (4 + vsize) * 2);
     return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
@@ -346,15 +339,17 @@ extern "C" GrB_Info GxB_Matrix_diag(GrB_Matrix C, const GrB_Vector v, int64_t k,
     if (dim >= ((uint64_t)1 << 31)) return gb_fail(GrB_INVALID_VALUE, err, "%s: dimensions beyond 2^31 are not supported in HBM", fn);
     GB_TRY(vector_ensure_device(v));
     const size_t vsize = v->type->size;
-    Csr T; T.nrows = T.ncols = (int64_t)dim;
-    GB_TRY(T.rowptr.alloc((size_t)dim + 1, err));
-    diag_build_kernel<<<grid_for((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, T.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, (int64_t)dim + 1, err));
-    GB_TRY(read_i64(T.rowptr + dim, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
-    if (T.nnz > 0) { diag_fill_kernel<<<grid_for((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
-    GB_TRY(dev_build_rowptr32(T, err));
+    Csr T;
+    GB_TRY(csr_from_row_counts((int64_t)dim, (int64_t)dim, vsize, T, err,
+        [&](int64_t *rowptr) {
+            diag_build_kernel<<<grid_for((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, rowptr); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            diag_fill_kernel<<<grid_for((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, t.rowptr, t.col,
+                                                                           (uint8_t *)t.val); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        }));
     DescFlags plain{};
     return matrix_writeback(C, nullptr, nullptr, plain, std::move(T), v->type->code, false, err);
 }
@@ -436,22 +431,18 @@ extern "C" GrB_Info GrB_Matrix_kronecker_BinaryOp(GrB_Matrix C, const GrB_Matrix
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn);
     if (am * bm >= ((uint64_t)1 << 31) || an * bn >= ((uint64_t)1 << 31)) return gb_fail(GrB_INVALID_VALUE, err, "%s: result dimensions beyond 2^31 are not supported in HBM", fn);
     GbBurble burble(fn);
-    if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
-    if (f.tran1) GB_TRY(matrix_ensure_transpose(B)); else GB_TRY(matrix_ensure_device(B));
-    const Csr &a = f.tran0 ? A->devT : A->dev; const Csr &b = f.tran1 ? B->devT : B->dev;
+    Csr *a, *b; GB_TRY(source_csr(A, f.tran0, &a)); GB_TRY(source_csr(B, f.tran1, &b));
     const int ztc = op->ztype->code;
-    Csr T; T.nrows = (int64_t)(am * bm); T.ncols = (int64_t)(an * bn);
-    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    kron_count_kernel<<<grid_for(T.nrows + 1), 256, 0, G.stream>>>(a.rowptr, b.rowptr, (int64_t)am, (int64_t)bm, T.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
-    GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(ztc) + 16, err));
-    if (T.nnz > 0) {
-        kron_fill_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(a.rowptr, a.col, a.val, A->type->code, b.rowptr, b.col, b.val, B->type->code, (int64_t)am, (int64_t)bm,
-                                                              (int64_t)bn, op->opcode, op->xtype->code, op->ytype->code, ztc, T.rowptr, T.col, T.val); GB_LAUNCHED();
-    }
-    GB_TRY(dev_build_rowptr32(T, err));
+    const int64_t tn = (int64_t)(am * bm);
+    Csr T;
+    GB_TRY(csr_from_row_counts(tn, (int64_t)(an * bn), tc_size(ztc), T, err,
+        [&](int64_t *rowptr) { kron_count_kernel<<<grid_for(tn + 1), 256, 0, G.stream>>>(a->rowptr, b->rowptr, (int64_t)am, (int64_t)bm, rowptr); GB_LAUNCHED(); return GrB_SUCCESS; },
+        [&](Csr &t) {
+            kron_fill_kernel<<<grid_for(tn), 256, 0, G.stream>>>(a->rowptr, a->col, a->val, A->type->code, b->rowptr, b->col, b->val, B->type->code, (int64_t)am,
+                                                               (int64_t)bm, (int64_t)bn, op->opcode, op->xtype->code, op->ytype->code, ztc, t.rowptr, t.col, t.val);
+            GB_LAUNCHED();
+            return GrB_SUCCESS;
+        }));
     burble.note("row-pair expansion", (double)T.nnz * (4 + tc_size(ztc)));
     return matrix_writeback(C, Mask, accum, f, std::move(T), ztc, false, err);
 }
@@ -653,8 +644,8 @@ extern "C" GrB_Info GrB_Matrix_assign(GrB_Matrix C, const GrB_Matrix Mask, const
     if (an != tn || am != tm) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: A is %llux%llu, the index lists select %llux%llu", fn,
                                              (unsigned long long)an, (unsigned long long)am, (unsigned long long)tn, (unsigned long long)tm);
     GbBurble burble(fn);
-    GB_TRY(f.tran0 ? matrix_ensure_transpose(A) : matrix_ensure_device(A));
-    const Csr &a = f.tran0 ? A->devT : A->dev;
+    Csr *pa; GB_TRY(source_csr(A, f.tran0, &pa));
+    const Csr &a = *pa;
     const size_t vsize = A->type->size;
     DevBuf<int32_t> d_rowsrc; DevBuf<uint32_t> d_jmap; bool need_sort = false, j_repeats = false;
     if (!R.all_rows) {
@@ -674,18 +665,19 @@ extern "C" GrB_Info GrB_Matrix_assign(GrB_Matrix C, const GrB_Matrix Mask, const
         for (size_t q = 0; q < jmap.size(); ++q) if (jmap[q] != JDROP) { if (!first && jmap[q] <= prev) need_sort = true; prev = jmap[q]; first = false; }
         GB_TRY(upload(jmap, d_jmap, err));
     }
-    Csr T; T.nrows = (int64_t)C->nrows; T.ncols = (int64_t)C->ncols;
-    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    massign_count_kernel<<<grid_for(T.nrows + 1), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, j_repeats ? d_jmap.get() : nullptr, T.rowptr); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
-    GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
-    if (T.nnz > 0) {
-        massign_fill_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(d_rowsrc, T.nrows, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jmap, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
-        if (need_sort) { rows_insertion_sort_kernel<<<grid_for(T.nrows), 256, 0, G.stream>>>(T.rowptr, T.nrows, T.col, (uint8_t *)T.val, (int)vsize); GB_LAUNCHED(); }
-    }
-    GB_TRY(dev_build_rowptr32(T, err));
+    const int64_t tr = (int64_t)C->nrows;
+    Csr T;
+    GB_TRY(csr_from_row_counts(tr, (int64_t)C->ncols, vsize, T, err,
+        [&](int64_t *rowptr) {
+            massign_count_kernel<<<grid_for(tr + 1), 256, 0, G.stream>>>(d_rowsrc, tr, a.rowptr, a.col, j_repeats ? d_jmap.get() : nullptr, rowptr); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            massign_fill_kernel<<<grid_for(tr), 256, 0, G.stream>>>(d_rowsrc, tr, a.rowptr, a.col, (const uint8_t *)a.val, (int)vsize, d_jmap, t.rowptr, t.col,
+                                                                   (uint8_t *)t.val); GB_LAUNCHED();
+            if (need_sort) { rows_insertion_sort_kernel<<<grid_for(tr), 256, 0, G.stream>>>(t.rowptr, tr, t.col, (uint8_t *)t.val, (int)vsize); GB_LAUNCHED(); }
+            return GrB_SUCCESS;
+        }));
     d_rowsrc.reset(); d_jmap.reset();
     return assign_writeback(C, Mask, accum, f, R, std::move(T), A->type->code, /*t_covers_region=*/false, err);
 }

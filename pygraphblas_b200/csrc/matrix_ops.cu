@@ -24,22 +24,6 @@
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "%s: invalid vector handle", fn); } while (0)
 #define GB_NEED_DEVICE(errp, fn) do { if (!G.have_device) return gb_fail(GrB_PANIC, errp, "%s: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)", fn); } while (0)
 
-// op(A): the CSR of A or of its cached transpose
-static GrB_Info source_csr(GrB_Matrix A, bool tran, const Csr **out) {
-    if (tran) { GB_TRY(matrix_ensure_transpose(A)); *out = &A->devT; }
-    else { GB_TRY(matrix_ensure_device(A)); *out = &A->dev; }
-    return GrB_SUCCESS;
-}
-static GrB_Info new_pattern_like(const Csr &src, size_t vsize, Csr &T, std::string *err) {
-    T = Csr(); T.nrows = src.nrows; T.ncols = src.ncols; T.nnz = src.nnz;
-    GB_TRY(T.rowptr.alloc((size_t)src.nrows + 1, err));
-    GB_TRY(T.col.alloc((size_t)src.nnz, err));
-    GB_TRY(T.val.alloc((size_t)src.nnz * vsize + 16, err));
-    CU_TRY(cudaMemcpyAsync(T.rowptr, src.rowptr, ((size_t)src.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
-    if (src.nnz) CU_TRY(cudaMemcpyAsync(T.col, src.col, (size_t)src.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-    return GrB_SUCCESS;
-}
-
 // ------------------------------------------------------------------ select
 struct SelectArgs {
     const int64_t *rowptr; const uint32_t *col; const void *val; int tc; int64_t nrows;
@@ -106,6 +90,23 @@ static GrB_Info select_args(const GxB_SelectOp op, const GxB_Scalar thunk, int t
     }
     return GrB_SUCCESS;
 }
+// T = the entries of src that a (code, k, thunk, tc set) keeps, with their values when vsize > 0, only their pattern when 0
+static GrB_Info select_csr(const Csr &src, SelectArgs a, size_t vsize, Csr &T, std::string *err) {
+    a.rowptr = src.rowptr; a.col = src.col; a.val = src.val; a.nrows = src.nrows;
+    const int grid = grid_for(src.nrows * 32);
+    return csr_from_row_counts(src.nrows, src.ncols, vsize, T, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)src.nrows + 1) * 8, G.stream), err);
+            a.o_ptr = rowptr;       // without entries there is nothing to count: the memset has zeroed every slot
+            if (src.nnz > 0) { select_kernel<false><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            a.o_col = t.col; a.o_val = vsize ? t.val.get() : nullptr;
+            select_kernel<true><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        });
+}
 extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GxB_SelectOp op, const GrB_Matrix A,
                                       const GxB_Scalar thunk, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
@@ -121,36 +122,15 @@ extern "C" GrB_Info GxB_Matrix_select(GrB_Matrix C, const GrB_Matrix Mask, const
     SelectArgs a{};
     GB_TRY(select_args(op, thunk, A->type->code, a, fn));
     GB_NEED_DEVICE(err, fn);
-    const Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
-    a.rowptr = src->rowptr; a.col = src->col; a.val = src->val; a.tc = A->type->code; a.nrows = src->nrows;
-    Csr T; T.nrows = src->nrows; T.ncols = src->ncols;
-    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
-    a.o_ptr = T.rowptr;
-    select_kernel<false><<<grid_for(T.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
-    GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * A->type->size + 16, err));
-    a.o_col = T.col; a.o_val = T.val;
-    if (T.nnz > 0) { select_kernel<true><<<grid_for(T.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    GB_TRY(dev_build_rowptr32(T, err));
+    Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
+    a.tc = A->type->code;
+    Csr T; GB_TRY(select_csr(*src, a, A->type->size, T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }
 GrB_Info mask_true_pattern(const Csr &M, int mtc, Csr &out, std::string *err) {
     SelectArgs a{};
-    a.code = SEL_NONZERO; a.rowptr = M.rowptr; a.col = M.col; a.val = M.val; a.tc = mtc; a.nrows = M.nrows;
-    out = Csr(); out.nrows = M.nrows; out.ncols = M.ncols;
-    GB_TRY(out.rowptr.alloc((size_t)M.nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(out.rowptr, 0, ((size_t)M.nrows + 1) * 8, G.stream), err);
-    a.o_ptr = out.rowptr;
-    if (M.nnz > 0) { select_kernel<false><<<grid_for(M.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    GB_TRY(dev_exclusive_scan(out.rowptr, M.nrows + 1, err));
-    GB_TRY(read_i64(out.rowptr + M.nrows, &out.nnz, err));
-    GB_TRY(out.col.alloc((size_t)out.nnz, err));
-    a.o_col = out.col; a.o_val = nullptr;       // the filter reads the pattern only
-    if (out.nnz > 0) { select_kernel<true><<<grid_for(M.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    return dev_build_rowptr32(out, err);
+    a.code = SEL_NONZERO; a.tc = mtc;
+    return select_csr(M, a, 0, out, err);       // the filter reads the pattern only
 }
 __global__ void vec_select_kernel(const SelectArgs a, const uint8_t *upres, uint8_t *tpres) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.nrows; i += (int64_t)gridDim.x * blockDim.x) {
@@ -203,8 +183,8 @@ static GrB_Info mat_apply(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     const uint64_t an = f.tran0 ? A->ncols : A->nrows, am = f.tran0 ? A->nrows : A->ncols;
     if (C->nrows != an || C->ncols != am || (Mask && (Mask->nrows != an || Mask->ncols != am))) return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: dimensions do not match", fn);
     GB_NEED_DEVICE(err, fn);
-    const Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
-    Csr T; GB_TRY(new_pattern_like(*src, (size_t)tc_size(ztc), T, err));
+    Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
+    Csr T; GB_TRY(csr_copy(*src, (size_t)tc_size(ztc), false, T, err));
     ApplyArgs a{};
     a.nnz = src->nnz; a.aval = src->val; a.atc = A->type->code; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar; a.tval = T.val;
     if (mode == AP_UNARY ? uop_is_positional(opcode) : op_is_positional(opcode)) {
@@ -299,7 +279,7 @@ static GrB_Info mat_reduce_vector(GrB_Vector w, const GrB_Vector mask, const GrB
     const uint64_t rows = f.tran0 ? A->ncols : A->nrows;
     if (w->n != rows || (mask && mask->n != rows)) return gb_fail(GrB_DIMENSION_MISMATCH, &w->err, "%s: dimensions do not match", fn);
     GB_NEED_DEVICE(&w->err, fn);
-    const Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
+    Csr *src; GB_TRY(source_csr(A, f.tran0, &src));
     RowReduceArgs a{};
     a.rowptr = src->rowptr; a.val = src->val; a.atc = A->type->code; a.nrows = src->nrows; a.op = op->opcode; a.mtc = op->ztype->code;
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
@@ -369,23 +349,24 @@ static GrB_Info mat_ewise(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
     if (an != bn || am != bm || C->nrows != an || C->ncols != am || (Mask && (Mask->nrows != an || Mask->ncols != am)))
         return gb_fail(GrB_DIMENSION_MISMATCH, err, "%s: dimensions do not match", fn);
     GB_NEED_DEVICE(err, fn);
-    const Csr *sa, *sb; GB_TRY(source_csr(A, f.tran0, &sa)); GB_TRY(source_csr(B, f.tran1, &sb));
+    Csr *sa, *sb; GB_TRY(source_csr(A, f.tran0, &sa)); GB_TRY(source_csr(B, f.tran1, &sb));
     MergeArgs a{};
     a.a_ptr = sa->rowptr; a.a_col = sa->col; a.a_val = sa->val; a.atc = A->type->code;
     a.b_ptr = sb->rowptr; a.b_col = sb->col; a.b_val = sb->val; a.btc = B->type->code;
     a.nrows = sa->nrows; a.mult = mult; a.op = op->opcode; a.xtc = op->xtype->code; a.ztc = op->ztype->code;
-    Csr T; T.nrows = sa->nrows; T.ncols = sa->ncols;
-    GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
-    a.o_ptr = T.rowptr;
-    merge_rows_kernel<false><<<grid_for(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(T.rowptr, T.nrows + 1, err));
-    GB_TRY(read_i64(T.rowptr + T.nrows, &T.nnz, err));
-    GB_TRY(T.col.alloc((size_t)T.nnz, err));
-    GB_TRY(T.val.alloc((size_t)T.nnz * tc_size(a.ztc) + 16, err));
-    a.o_col = T.col; a.o_val = T.val;
-    if (T.nnz > 0) { merge_rows_kernel<true><<<grid_for(T.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    GB_TRY(dev_build_rowptr32(T, err));
+    Csr T;
+    GB_TRY(csr_from_row_counts(sa->nrows, sa->ncols, tc_size(a.ztc), T, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)a.nrows + 1) * 8, G.stream), err);
+            a.o_ptr = rowptr;
+            merge_rows_kernel<false><<<grid_for(a.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            a.o_col = t.col; a.o_val = t.val;
+            merge_rows_kernel<true><<<grid_for(a.nrows), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        }));
     return matrix_writeback(C, Mask, accum, f, std::move(T), a.ztc, false, err);
 }
 #define GB_MAT_EWISE(NAME, KIND, OPEXPR, MULT) \

@@ -185,15 +185,10 @@ GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
     const bool full = !X.pres && !Y.pres;
     // with nothing absent and a structural mask, T has exactly M's pattern: the kernel writes T's values in place
     const bool pattern_mask = full && f.mask_struct && d > 0;
-    Csr T; T.nrows = m; T.ncols = n;
+    Csr T;
     void *tval = nullptr; uint8_t *found = nullptr;
     if (pattern_mask) {
-        GB_TRY(T.rowptr.alloc((size_t)m + 1, err));
-        GB_TRY(T.col.alloc((size_t)M.nnz, err));
-        GB_TRY(T.val.alloc((size_t)M.nnz * zsz + 16, err));
-        CU_TRY(cudaMemcpyAsync(T.rowptr, M.rowptr, ((size_t)m + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
-        if (M.nnz > 0) CU_TRY(cudaMemcpyAsync(T.col, M.col, (size_t)M.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-        T.nnz = M.nnz;
+        GB_TRY(csr_copy(M, zsz, false, T, err));
         tval = T.val;
     } else {
         GB_TRY(ws_get(WS_WORDS, &tval, (size_t)M.nnz * zsz + 16, err));

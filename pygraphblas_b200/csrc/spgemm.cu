@@ -1029,106 +1029,110 @@ static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgs &base, std::s
 static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt,
                                 int add, int mul, bool need_a, bool need_b, const Csr *Mb, Csr &T, std::string *err) {
     const int64_t nrows = A.nrows, ncols = B.ncols;
-    T = Csr(); T.nrows = nrows; T.ncols = ncols;
-    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-    DevBuf<int64_t> flops; DevBuf<unsigned long long> total;
-    GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
-    CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
-    flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
-    RowBins bins;
-    GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
-    int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
-    G.last_flops = (uint64_t)total_flops;
     const bool comp = Mb && Mb->nnz > 0;
     const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
-    // the dense-accumulator bin: with a complemented mask its rows above SPLIT_FLOPS go to spa-split
+    RowBins bins;
     SplitPlan sp;
-    if (comp && bins.count[3]) GB_TRY(split_prepare(bins, flops, A, ncols, wsize, sp, err));
-    const int32_t *spa_rows = sp.nsplit ? sp.keep.get() : bins.rows + bins.offset[3];
-    const int64_t spa_n = sp.nsplit ? sp.nkeep : (int64_t)bins.count[3];
-    flops.reset(); total.reset();
-
     GemmArgs g{};
-    g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
-    g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
-    g.c_cnt = T.rowptr;
-    if (comp) { g.m_ptr = Mb->rowptr32; g.m_col = Mb->col; }
     SplitArgs sa{};
-    sa.a_col = A.col; sa.a_val = aval; sa.b_ptr = B.rowptr32; sa.b_col = B.col; sa.b_val = bval; sa.m_ptr = g.m_ptr; sa.m_col = g.m_col;
-    sa.queue = sp.queue; sa.pres = sp.pres; sa.mbit = sp.mbit; sa.acc = sp.acc; sa.words = sp.words; sa.ncols = ncols; sa.nrange = sp.nrange;
-    sa.add_op = add; sa.mul_op = mul; sa.need_a = need_a; sa.need_b = need_b; sa.c_cnt = T.rowptr; sa.range_cnt = sp.range_cnt;
-    const int spa_ctas = std::max(1, std::min<int>((int)spa_n, G.num_sms * 2));
+    const int32_t *spa_rows = nullptr;
+    int64_t spa_n = 0;
+    int spa_ctas = 1;
     DevBuf<unsigned int> queue; DevBuf<uint32_t> spa_bits;
-    if (spa_n) {
-        g.spa_words = ceil_div(ncols, 32);
-        const size_t words = (size_t)spa_ctas * g.spa_words * (comp ? 2 : 1);     // comp: + the mask bitmaps
-        GB_TRY(spa_bits.alloc(words, err));
-        g.spa_bits = spa_bits;
-        CU_TRY(cudaMemsetAsync(g.spa_bits, 0, words * 4, G.stream), err);
-        GB_TRY(queue.alloc(2, err));
-        CU_TRY(cudaMemsetAsync(queue, 0, 8, G.stream), err);
-    }
-    // ---- symbolic
-    if (bins.count[1]) {
-        g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1]; g.table = SMALL_TABLE;
-        (comp ? hash_symbolic_kernel<true, true> : hash_symbolic_kernel<true>)<<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g);
-        GB_LAUNCHED();
-    }
-    if (bins.count[2]) {
-        g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
-        (comp ? hash_symbolic_kernel<false, true> : hash_symbolic_kernel<false>)<<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g);
-        GB_LAUNCHED();
-    }
-    if (spa_n) {
-        g.rows = spa_rows; g.nbin = spa_n; g.queue = queue;
-        (comp ? spa_kernel<bool, bool, -1, -1, false, true> : spa_kernel<bool, bool, -1, -1, false>)<<<spa_ctas, 512, 0, G.stream>>>(g);
-        GB_LAUNCHED();
-    }
-    for (int64_t k = 0; k + 1 < (int64_t)sp.chunk_off.size(); ++k) {
-        int64_t ng = 0;
-        const SplitArgs s = split_group(sp, sa, k, &ng, err);
-        split_chunk_kernel<bool, bool, -1, -1, false><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
-        split_count_kernel<true><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
-        G.launches += 2;
-    }
-    GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
-    int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
-    T.nnz = nnz; G.last_nnz_out = (uint64_t)nnz;
-    GB_TRY(T.col.alloc((size_t)nnz, err));
-    GB_TRY(T.val.alloc((size_t)nnz * tc_size(zt) + 16, err));
-    g.c_ptr = T.rowptr; g.c_col = T.col; g.c_val = T.val;
+    // ---- symbolic: the bins count the entries of their rows
+    auto symbolic = [&](int64_t *cnt) {
+        CU_TRY(cudaMemsetAsync(cnt, 0, ((size_t)nrows + 1) * 8, G.stream), err);
+        DevBuf<int64_t> flops; DevBuf<unsigned long long> total;
+        GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
+        CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
+        flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
+        GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
+        int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
+        G.last_flops = (uint64_t)total_flops;
+        // the dense-accumulator bin: with a complemented mask its rows above SPLIT_FLOPS go to spa-split
+        if (comp && bins.count[3]) GB_TRY(split_prepare(bins, flops, A, ncols, wsize, sp, err));
+        spa_rows = sp.nsplit ? sp.keep.get() : bins.rows + bins.offset[3];
+        spa_n = sp.nsplit ? sp.nkeep : (int64_t)bins.count[3];
+        flops.reset(); total.reset();
+
+        g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
+        g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
+        g.c_cnt = cnt;
+        if (comp) { g.m_ptr = Mb->rowptr32; g.m_col = Mb->col; }
+        sa.a_col = A.col; sa.a_val = aval; sa.b_ptr = B.rowptr32; sa.b_col = B.col; sa.b_val = bval; sa.m_ptr = g.m_ptr; sa.m_col = g.m_col;
+        sa.queue = sp.queue; sa.pres = sp.pres; sa.mbit = sp.mbit; sa.acc = sp.acc; sa.words = sp.words; sa.ncols = ncols; sa.nrange = sp.nrange;
+        sa.add_op = add; sa.mul_op = mul; sa.need_a = need_a; sa.need_b = need_b; sa.c_cnt = cnt; sa.range_cnt = sp.range_cnt;
+        spa_ctas = std::max(1, std::min<int>((int)spa_n, G.num_sms * 2));
+        if (spa_n) {
+            g.spa_words = ceil_div(ncols, 32);
+            const size_t words = (size_t)spa_ctas * g.spa_words * (comp ? 2 : 1);     // comp: + the mask bitmaps
+            GB_TRY(spa_bits.alloc(words, err));
+            g.spa_bits = spa_bits;
+            CU_TRY(cudaMemsetAsync(g.spa_bits, 0, words * 4, G.stream), err);
+            GB_TRY(queue.alloc(2, err));
+            CU_TRY(cudaMemsetAsync(queue, 0, 8, G.stream), err);
+        }
+        // the bins are reported here: a complemented mask may block every product, and then the numeric pass does not run
+        if (bins.count[1]) {
+            g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1]; g.table = SMALL_TABLE;
+            (comp ? hash_symbolic_kernel<true, true> : hash_symbolic_kernel<true>)<<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g);
+            GB_LAUNCHED(); gb_kernel_used("esc-small");
+        }
+        if (bins.count[2]) {
+            g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
+            (comp ? hash_symbolic_kernel<false, true> : hash_symbolic_kernel<false>)<<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g);
+            GB_LAUNCHED(); gb_kernel_used("esc-medium");
+        }
+        if (spa_n) {
+            g.rows = spa_rows; g.nbin = spa_n; g.queue = queue;
+            (comp ? spa_kernel<bool, bool, -1, -1, false, true> : spa_kernel<bool, bool, -1, -1, false>)<<<spa_ctas, 512, 0, G.stream>>>(g);
+            GB_LAUNCHED(); gb_kernel_used("spa");
+        }
+        for (int64_t k = 0; k + 1 < (int64_t)sp.chunk_off.size(); ++k) {
+            int64_t ng = 0;
+            const SplitArgs s = split_group(sp, sa, k, &ng, err);
+            split_chunk_kernel<bool, bool, -1, -1, false><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
+            split_count_kernel<true><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
+            G.launches += 2;
+        }
+        if (sp.nsplit) gb_kernel_used("spa-split");
+        return GrB_SUCCESS;
+    };
     // ---- numeric (shared-memory bins: expand-sort-compress)
-    if (bins.count[1]) {
-        g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1];
+    auto numeric = [&](Csr &t) {
+        g.c_ptr = t.rowptr; g.c_col = t.col; g.c_val = t.val;
+        if (bins.count[1]) {
+            g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1];
 #define K_ESC_SMALL(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, true, true> : esc_numeric_kernel<XT, ZT, A_, M_, true>) \
-            <<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); GB_LAUNCHED(); gb_kernel_used("esc-small");
-    }
-    if (bins.count[2]) {
-        g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2];
+                <<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); GB_LAUNCHED();
+        }
+        if (bins.count[2]) {
+            g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2];
 #define K_ESC_MEDIUM(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, false, true> : esc_numeric_kernel<XT, ZT, A_, M_, false>) \
-            <<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); GB_LAUNCHED(); gb_kernel_used("esc-medium");
-    }
-    if (spa_n) {
-        g.rows = spa_rows; g.nbin = spa_n; g.queue = queue + 1;
-        DevBuf<void> spa_val;
-        GB_TRY(spa_val.alloc((size_t)spa_ctas * ncols * wsize + 16, err));
-        g.spa_val = spa_val;
+                <<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); GB_LAUNCHED();
+        }
+        if (spa_n) {
+            g.rows = spa_rows; g.nbin = spa_n; g.queue = queue + 1;
+            DevBuf<void> spa_val;
+            GB_TRY(spa_val.alloc((size_t)spa_ctas * ncols * wsize + 16, err));
+            g.spa_val = spa_val;
 #define K_SPA(XT, ZT, A_, M_) do { \
-        fill_accum_init<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
-        (comp ? spa_kernel<XT, ZT, A_, M_, true, true> : spa_kernel<XT, ZT, A_, M_, true>)<<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2; gb_kernel_used("spa");
-    }
-    if (sp.nsplit) {
-        sa.c_ptr = T.rowptr; sa.c_col = T.col; sa.c_val = T.val;
+            fill_accum_init<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
+            (comp ? spa_kernel<XT, ZT, A_, M_, true, true> : spa_kernel<XT, ZT, A_, M_, true>)<<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2;
+        }
+        if (sp.nsplit) {
+            sa.c_ptr = t.rowptr; sa.c_col = t.col; sa.c_val = t.val;
 #define K_SPLIT(XT, ZT, A_, M_) GB_TRY((split_numeric<XT, ZT, A_, M_>(sp, sa, err)))
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_SPLIT, err); gb_kernel_used("spa-split");
-    }
-    spa_bits.reset(); queue.reset(); bins.rows.reset();
-    GB_TRY(dev_build_rowptr32(T, err));
-    CU_TRY(cudaGetLastError(), err);
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_SPLIT, err);
+        }
+        spa_bits.reset(); queue.reset(); bins.rows.reset();
+        return GrB_SUCCESS;
+    };
+    GB_TRY(csr_from_row_counts(nrows, ncols, tc_size(zt), T, err, symbolic, numeric));
+    G.last_nnz_out = (uint64_t)T.nnz;
     return GrB_SUCCESS;
 }
 
@@ -1273,19 +1277,19 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
 
 GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
     const int64_t nrows = M.nrows;
-    GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-    if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, found, nrows, T.rowptr); GB_LAUNCHED(); }
-    GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
-    int64_t nnz = 0; GB_TRY(read_i64(T.rowptr + nrows, &nnz, err));
-    T.nnz = nnz; G.last_nnz_out = (uint64_t)nnz;
-    GB_TRY(T.col.alloc((size_t)nnz, err));
-    GB_TRY(T.val.alloc((size_t)nnz * vsize + 16, err));
-    if (nnz > 0) {
-        row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)vsize,
-                                                                          nrows, T.rowptr, T.col, (uint8_t *)T.val); GB_LAUNCHED();
-    }
-    return dev_build_rowptr32(T, err);
+    GB_TRY(csr_from_row_counts(nrows, M.ncols, vsize, T, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
+            if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, found, nrows, rowptr); GB_LAUNCHED(); }
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)vsize,
+                                                                              nrows, t.rowptr, t.col, (uint8_t *)t.val); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        }));
+    G.last_nnz_out = (uint64_t)T.nnz;
+    return GrB_SUCCESS;
 }
 
 // C<M> = accum(C, T) into a fresh CSR `out` of C's type (T has type ttc)
@@ -1301,21 +1305,18 @@ static GrB_Info matrix_finalize(const Csr *C, int ctc, const Csr &T, int ttc, co
     a.mask_comp = f.mask_comp; a.mask_struct = f.mask_struct; a.replace = f.replace;
     a.accum_op = accum ? accum->opcode : -1;
     a.accum_tc = accum ? accum->xtype->code : 0; a.accum_ztc = accum ? accum->ztype->code : 0;
-    out = Csr(); out.nrows = T.nrows; out.ncols = T.ncols;
-    GB_TRY(out.rowptr.alloc((size_t)nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(out.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-    a.o_cnt = out.rowptr;
-    mat_finalize_kernel<false><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED();
-    GB_TRY(dev_exclusive_scan(out.rowptr, nrows + 1, err));
-    int64_t nnz = 0; GB_TRY(read_i64(out.rowptr + nrows, &nnz, err));
-    out.nnz = nnz;
-    GB_TRY(out.col.alloc((size_t)nnz, err));
-    GB_TRY(out.val.alloc((size_t)nnz * tc_size(ctc) + 16, err));
-    a.o_ptr = out.rowptr; a.o_col = out.col; a.o_val = out.val;
-    if (nnz > 0) { mat_finalize_kernel<true><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    GB_TRY(dev_build_rowptr32(out, err));
-    CU_TRY(cudaGetLastError(), err);
-    return GrB_SUCCESS;
+    return csr_from_row_counts(nrows, T.ncols, tc_size(ctc), out, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
+            a.o_cnt = rowptr;
+            mat_finalize_kernel<false><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            a.o_ptr = t.rowptr; a.o_col = t.col; a.o_val = t.val;
+            mat_finalize_kernel<true><<<grid_for(nrows, 128), 128, 0, G.stream>>>(a); GB_LAUNCHED();
+            return GrB_SUCCESS;
+        });
 }
 
 // write T (type ttc) back into C under mask / accum / replace; consumes T
@@ -1366,14 +1367,14 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
     const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
     const bool use_mask = Mask && !f.mask_comp;
     *masked = Mask != nullptr;
-    if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
+    Csr *pa; GB_TRY(source_csr(A, f.tran0, &pa));
     GB_TRY(matrix_ensure_device(B));
     // C<M> = A*B': small problems intersect rows of A and B directly (no transpose); large ones
     // go through the cached transpose and the load-balanced masked hash kernels
     const bool dot = use_mask && f.tran1 && B->dev.nnz < ((int64_t)1 << 18);
     if (f.tran1 && !dot) GB_TRY(matrix_ensure_transpose(B));
     if (Mask) GB_TRY(matrix_ensure_device(Mask));
-    const Csr &a = f.tran0 ? A->devT : A->dev;
+    const Csr &a = *pa;
     const Csr &b = (f.tran1 && !dot) ? B->devT : B->dev;
     if (!a.rowptr32 || !b.rowptr32 || (Mask && !Mask->dev.rowptr32))
         return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
@@ -1470,10 +1471,6 @@ GrB_Info positional_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp 
     // ---- count form: product = i (FIRSTI) or j (SECONDJ), + off
     const bool idem = add == OP_MIN || add == OP_MAX || add == OP_ANY;       // the count is not needed, only the pattern
     GB_TRY(mxm_product(Mask, f, TC_INT64, TC_INT64, idem ? OP_ANY : OP_PLUS, OP_PAIR, A, B, MxmPos(), T, &masked, err));
-    if (!T.rowptr && T.nnz == 0) {      // an empty product may come without arrays
-        GB_TRY(T.rowptr.alloc((size_t)T.nrows + 1, err));
-        CU_TRY(cudaMemsetAsync(T.rowptr, 0, ((size_t)T.nrows + 1) * 8, G.stream), err);
-    }
     DevBuf<void> v;
     GB_TRY(v.alloc((size_t)T.nnz * tc_size(zt) + 16, err));
     GB_TRY(pos_csr_values(v, zt, (const int64_t *)T.val.get(), add, T, /*by_col=*/p.second, p.second ? ids_n : ids_m, p.off, err));
@@ -1496,19 +1493,8 @@ extern "C" GrB_Info GrB_transpose(GrB_Matrix C, const GrB_Matrix Mask, const GrB
     if (C->nrows != tn || C->ncols != tm || (Mask && (Mask->nrows != tn || Mask->ncols != tm)))
         return gb_fail(GrB_DIMENSION_MISMATCH, err, "GrB_transpose: dimensions do not match");
     if (!G.have_device) return gb_fail(GrB_PANIC, err, "GrB_transpose: no CUDA device: libb200grb computes only on the GPU (no CPU fallback)");
-    if (f.tran0) GB_TRY(matrix_ensure_device(A)); else GB_TRY(matrix_ensure_transpose(A));
-    const Csr &src = f.tran0 ? A->dev : A->devT;
-    // T = copy of src (C may alias A)
-    Csr T; T.nrows = src.nrows; T.ncols = src.ncols; T.nnz = src.nnz;
-    const size_t sz = A->type->size;
-    GB_TRY(T.rowptr.alloc((size_t)src.nrows + 1, err));
-    GB_TRY(T.col.alloc((size_t)src.nnz, err));
-    GB_TRY(T.val.alloc((size_t)src.nnz * sz + 16, err));
-    CU_TRY(cudaMemcpyAsync(T.rowptr, src.rowptr, ((size_t)src.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
-    if (src.nnz) {
-        CU_TRY(cudaMemcpyAsync(T.col, src.col, (size_t)src.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-        CU_TRY(cudaMemcpyAsync(T.val, src.val, (size_t)src.nnz * sz, cudaMemcpyDeviceToDevice, G.stream), err);
-    }
+    Csr *src; GB_TRY(source_csr(A, !f.tran0, &src));
+    Csr T; GB_TRY(csr_copy(*src, A->type->size, true, T, err));      // a copy: C may alias A
     GB_TRY(dev_build_rowptr32(T, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), A->type->code, false, err);
 }

@@ -70,23 +70,20 @@ __global__ void csr_scatter_dense_kernel(const int64_t *rowptr, const uint32_t *
 }
 
 GrB_Info dense_to_csr(const void *val, const uint8_t *pres, int64_t nrows, int64_t ncols, size_t vsize, Csr &c, std::string *err) {
-    Csr t; t.nrows = nrows; t.ncols = ncols;
-    GB_TRY(t.rowptr.alloc((size_t)nrows + 1, err));
-    CU_TRY(cudaMemsetAsync(t.rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-    if (nrows > 0) { dense_row_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(pres, nrows, ncols, t.rowptr); GB_LAUNCHED(); }
-    GB_TRY(dev_exclusive_scan(t.rowptr, nrows + 1, err));
-    int64_t nnz = 0; GB_TRY(read_i64(t.rowptr + nrows, &nnz, err));
-    t.nnz = nnz;
-    GB_TRY(t.col.alloc((size_t)nnz, err));
-    GB_TRY(t.val.alloc((size_t)nnz * vsize + 16, err));
-    if (nnz > 0) {
-        dense_compact_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>((const uint8_t *)val, pres, nrows, ncols, (int)vsize, t.rowptr,
-                                                                         t.col, (uint8_t *)t.val.get());
-        GB_LAUNCHED();
-    }
-    GB_TRY(dev_build_rowptr32(t, err));
-    CU_TRY(cudaGetLastError(), err);
-    c = std::move(t);
+    Csr r;
+    GB_TRY(csr_from_row_counts(nrows, ncols, vsize, r, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
+            if (nrows > 0) { dense_row_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(pres, nrows, ncols, rowptr); GB_LAUNCHED(); }
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            dense_compact_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>((const uint8_t *)val, pres, nrows, ncols, (int)vsize, t.rowptr,
+                                                                             t.col, (uint8_t *)t.val.get());
+            GB_LAUNCHED();
+            return GrB_SUCCESS;
+        }));
+    c = std::move(r);
     return GrB_SUCCESS;
 }
 
@@ -370,8 +367,8 @@ GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     const GrB_BinaryOp mulop = s->mul, addop = s->add->op;
     const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
     gb_kernel_used("spmm");
-    if (f.tran0) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
-    const Csr &a = f.tran0 ? A->devT : A->dev;
+    Csr *pa; GB_TRY(source_csr(A, f.tran0, &pa));
+    const Csr &a = *pa;
     if (!a.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
     const int64_t m = a.nrows, n = a.ncols, k = (int64_t)B->ncols;
     // operands cast to the multiply's input types, as in the CSR path

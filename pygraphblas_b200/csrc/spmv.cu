@@ -321,8 +321,8 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         return vector_write(w, nullptr, accum, f, nullptr, nullptr, zt, false, nullptr);
 
     // ---- operands in HBM
-    if (use_transpose) GB_TRY(matrix_ensure_transpose(A)); else GB_TRY(matrix_ensure_device(A));
-    Csr &c = use_transpose ? A->devT : A->dev;
+    Csr *pc; GB_TRY(source_csr(A, use_transpose, &pc));
+    Csr &c = *pc;
     GB_TRY(vector_ensure_device(u));
     if (mask) GB_TRY(vector_ensure_device(mask));
     const bool need_final = mask != nullptr || accum != nullptr;

@@ -252,3 +252,89 @@ def test_matrix_ops():
     _sweep(lambda: (_mat_lists(S, INT64),), extract, _same_csr(sp.csr_matrix(S[Il][:, Jl])))
     _sweep(lambda: (_mat_lists(S, INT64),), assign, _same_csr(sp.csr_matrix(D)))
     _sweep(lambda: (_mat_lists(S, INT64), _mat(B, INT64)), kron, _same_csr(sp.kron(S, B).tocsr()))
+
+    # GxB_Matrix_diag: v's present entries on diagonal k = 2 of a fresh matrix
+    vn = 150
+    vp = rng.random(vn) < 0.6
+    vv = rng.integers(1, 9, vn).astype(np.int64)
+
+    def diag(v):
+        C = Matrix.sparse(INT64, vn + 2, vn + 2)
+        gb.base._check(lib.GxB_Matrix_diag(C._matrix[0], v._vector[0], 2, ffi.NULL))
+        return C
+    Dg = np.zeros((vn + 2, vn + 2), np.int64); Dg[np.flatnonzero(vp), np.flatnonzero(vp) + 2] = vv[vp]
+    _sweep(lambda: (Vector.from_lists(np.flatnonzero(vp), vv[vp], vn, INT64),), diag, _same_csr(sp.csr_matrix(Dg)))
+
+    # GrB_Matrix_assign with a matrix: J repeats 9 (its later position wins) and, once that one is dropped, is not ascending
+    Jm = [9, 0, 9, 5]
+    Jr = ffi.new("GrB_Index[]", Jm)
+    Am = _rand_csr(rng, 4, 4, 0.6, np.int64)
+    Da = S.toarray(); Da[np.ix_(Il, sorted(set(Jm)))] = 0
+    for q in (1, 2, 3):
+        Da[Il, Jm[q]] = Am.toarray()[:, q]
+
+    def massign(C, A):
+        gb.base._check(lib.GrB_Matrix_assign(C._matrix[0], ffi.NULL, ffi.NULL, A._matrix[0], I, 4, Jr, 4, ffi.NULL))
+        return C
+    _sweep(lambda: (_mat_lists(S, INT64), _mat(Am, INT64)), massign, _same_csr(sp.csr_matrix(Da)))
+
+    # eWiseAdd / eWiseMult / apply (all values are positive: the union sums and the products have S's and S2's patterns)
+    S2 = _rand_csr(rng, 300, 200, 0.05, np.int64)
+    mk2 = lambda: (_mat_lists(S, INT64), _mat(S2, INT64))
+    _sweep(mk2, lambda A, B2: A.eadd(B2, INT64.PLUS), _same_csr(sp.csr_matrix(S + S2)))
+    _sweep(mk2, lambda A, B2: A.emult(B2, INT64.TIMES), _same_csr(sp.csr_matrix(S.multiply(S2))))
+    _sweep(lambda: (_mat_lists(S, INT64),), lambda A: A.apply(INT64.AINV), _same_csr(sp.csr_matrix(-S)))
+
+    # GrB_Row_assign: row 3 takes u at J; the rest of the row stays, the entries of C outside the row are kept around it
+    def row_assign(C, u):
+        gb.base._check(lib.GrB_Row_assign(C._matrix[0], ffi.NULL, ffi.NULL, u._vector[0], 3, J, 3, ffi.NULL))
+        return C
+    Dr = S.toarray(); Dr[3, Jl] = [21, 0, 23]
+    _sweep(lambda: (_mat_lists(S, INT64), Vector.from_lists([0, 2], [21, 23], 3, INT64)), row_assign, _same_csr(sp.csr_matrix(Dr)))
+
+    # select into a non-empty C under a valued mask with an accumulator (MAX: a repeated call leaves C as it is)
+    Cs = _rand_csr(rng, 300, 200, 0.05, np.int64)
+    Ms = _rand_csr(rng, 300, 200, 0.3, np.int64)
+    mval = rng.random(Ms.nnz) < 0.7
+    Md = np.zeros(Ms.shape, bool); Md[tuple(Ms.nonzero())] = mval
+    Ts = S.multiply(S > 4).toarray()
+    Dsel = np.where(Md, np.maximum(Cs.toarray(), Ts), Cs.toarray())
+
+    def select_accum(A, C, M):
+        return A.select(">", 4, out=C, mask=M, accum=INT64.MAX)
+    _sweep(lambda: (_mat_lists(S, INT64), _mat(Cs, INT64), Matrix.from_csr(Ms.indptr, Ms.indices, mval, *Ms.shape, BOOL)),
+           select_accum, _same_csr(sp.csr_matrix(Dsel)))
+
+
+@pytest.mark.parametrize("kind", ["row", "matrix"])
+def test_failed_assign_leaves_c(kind):
+    """GrB_Row_assign / GrB_Matrix_assign without a mask or an accumulator delete C's entries inside the region before the
+    write-back: a failure at any later allocation returns GrB_OUT_OF_MEMORY with C as it was."""
+    rng = np.random.default_rng(8)
+    S = _rand_csr(rng, 300, 200, 0.05, np.int64)
+    I = ffi.new("GrB_Index[]", [3, 1, 7, 100]); J = ffi.new("GrB_Index[]", [9, 0, 9, 5]); Jr = ffi.new("GrB_Index[]", [5, 0, 9])
+    Am = _mat(_rand_csr(rng, 4, 4, 0.6, np.int64), INT64)
+    u = Vector.from_lists([0, 2], [21, 23], 3, INT64)
+
+    def call(C):
+        if kind == "row":
+            return lib.GrB_Row_assign(C._matrix[0], ffi.NULL, ffi.NULL, u._vector[0], 3, Jr, 3, ffi.NULL)
+        return lib.GrB_Matrix_assign(C._matrix[0], ffi.NULL, ffi.NULL, Am._matrix[0], I, 4, J, 4, ffi.NULL)
+
+    before = _snap(_mat_lists(S, INT64))
+    failed = 0
+    for k in range(1, 400):
+        C = _mat_lists(S, INT64)
+        lib.B200_debug_fail_alloc(k)
+        try:
+            info = call(C)
+        finally:
+            lib.B200_debug_fail_alloc(0)
+        if info == lib.GrB_SUCCESS:
+            break
+        assert info == lib.GrB_OUT_OF_MEMORY, info
+        assert _same(_snap(C), before), f"C changed by the call that failed at allocation {k}"
+        failed += 1
+    else:
+        pytest.fail("the call never got through")
+    assert failed > 2 and not _same(_snap(C), before)

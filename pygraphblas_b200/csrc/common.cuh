@@ -109,6 +109,7 @@ struct RunPlan {
     DevBuf<uint32_t> nzrow;          // [nnzrows] ids of the non-empty rows, ascending
     DevBuf<uint8_t> pres_tmpl;       // [nrows] 1 where the row is non-empty
     int64_t nruns = 0, nnzrows = 0;
+    bool wide = false;               // built from the 64-bit row offsets (the wide route)
     // per-call scratch of the run kernels, kept with the plan (no allocation on the call path)
     DevBuf<void> ws_head, ws_tail;   // [nruns] x 8 bytes: partials of the rows a run starts / ends inside
     DevBuf<uint8_t> ws_head_has, ws_tail_has;
@@ -202,10 +203,14 @@ struct GBGlobal {
     int burble = 0;
     cudaEvent_t burble_e0 = nullptr, burble_e1 = nullptr;
     std::string last_kernel;      // kernel paths of the last GrB_mxv / GrB_vxm / GrB_mxm, separated by ';' (B200_debug_last_kernel)
+    int64_t debug_wide = 0;       // B200_debug_wide: > 0 puts every mxv / vxm / transpose on the wide route, transposes in chunks of this many entries
     std::recursive_mutex mu;
 };
 extern GBGlobal G;
 static inline void gb_kernel_used(const char *k) { if (!G.last_kernel.empty()) G.last_kernel += ';'; G.last_kernel += k; }
+// the wide route of mxv / vxm (DESIGN.md section 3.1): 64-bit entry offsets, for a CSR without rowptr32 (nnz >= 2^32), and for
+// every CSR while B200_debug_wide is on
+static inline bool csr_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide > 0; }
 extern thread_local std::string tl_error;
 
 GrB_Info gb_fail(GrB_Info code, std::string *where, const char *fmt, ...);

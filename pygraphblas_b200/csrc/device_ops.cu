@@ -122,32 +122,95 @@ __global__ void permute_kernel(const uint32_t *perm, const uint32_t *rowid, cons
     }
 }
 
+// ---- chunks of a transpose cut into pieces (matrices with more than TRANSPOSE_CHUNK entries)
+// row ids of the entries [k0, k0 + len), one warp per row: rows outside the window write nothing
+__global__ void expand_rows_window_kernel(const int64_t *rowptr, int64_t nrows, int64_t k0, int64_t len, uint32_t *rowid) {
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = warp; r < nrows; r += nwarps) {
+        const int64_t rs = max(rowptr[r], k0), re = min(rowptr[r + 1], k0 + len);
+        for (int64_t k = rs + lane; k < re; k += 32) rowid[k - k0] = (uint32_t)r;
+    }
+}
+// keys: the chunk's column ids sorted.  At the first sorted position k of column c in the chunk: off[c] = cursor[c] - k, so that
+// the chunk's entries of column c go to off[c] + k, behind those of the earlier chunks
+__global__ void chunk_offsets_kernel(const uint32_t *keys, int64_t len, const int64_t *cursor, int64_t *off) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < len; k += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t c = keys[k];
+        if (k == 0 || keys[k - 1] != c) off[c] = cursor[c] - k;
+    }
+}
+// the permute kernel of a chunk: entry k of the sorted chunk goes to off[c] + k of T; the last one of each column moves its cursor
+__global__ void chunk_scatter_kernel(const uint32_t *keys, const uint32_t *perm, const uint32_t *rowid, const uint8_t *val, int vsize,
+                                     int64_t k0, int64_t len, const int64_t *off, int64_t *cursor, uint32_t *tcol, uint8_t *tval) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < len; k += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t c = keys[k], p = perm[k];
+        const int64_t d = off[c] + k, s = k0 + p;
+        tcol[d] = rowid[p];
+        switch (vsize) {
+            case 1: tval[d] = val[s]; break;
+            case 2: ((uint16_t *)tval)[d] = ((const uint16_t *)val)[s]; break;
+            case 4: ((uint32_t *)tval)[d] = ((const uint32_t *)val)[s]; break;
+            default: ((uint64_t *)tval)[d] = ((const uint64_t *)val)[s]; break;
+        }
+        if (k == len - 1 || keys[k + 1] != c) cursor[c] = d + 1;
+    }
+}
+
 // T = A' as CSR.  A stable LSD radix sort of the entries by column keeps, inside
 // every column, the row-major order of A, i.e. ascending row ids: T's rows come out sorted.
 // (cub::DeviceRadixSort is used here only: this is a cached set-up step, not the hot path.)
+// A matrix of more than TRANSPOSE_CHUNK entries (B200_debug_wide: its chunk) is walked in order in chunks of that many: each chunk
+// is sorted stably by column and scattered behind the entries its columns already hold in T (per-column cursors, started at the
+// column offsets of T), so every column of T still receives its rows in ascending order -- the same arrays as one sort.
+// Peak scratch: 16 bytes per chunk entry (row ids, two permutations, sorted keys) + the sort's own (about 8 bytes per chunk entry)
+// + 16 bytes per column of A when chunked: about 3.2 GB at TRANSPOSE_CHUNK = 2^27.  A single chunk runs the unchunked launches.
+static constexpr int64_t TRANSPOSE_CHUNK = (int64_t)1 << 27;
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err) {
-    if (a.nnz >= ((int64_t)1 << 32)) return gb_fail(GrB_INVALID_VALUE, err, "transpose: nnz >= 2^32 not supported");
+    const int64_t chunk = G.debug_wide > 0 ? std::min(G.debug_wide, (int64_t)1 << 31) : TRANSPOSE_CHUNK;     // 32-bit permutations
+    const bool chunked = a.nnz > chunk;
     t = Csr(); t.nrows = a.ncols; t.ncols = a.nrows; t.nnz = a.nnz;
     GB_TRY(t.rowptr.alloc((size_t)t.nrows + 1, err));
     GB_TRY(t.col.alloc((size_t)t.nnz, err));
     GB_TRY(t.val.alloc((size_t)t.nnz * vsize + 16, err));
     CU_TRY(cudaMemsetAsync(t.rowptr, 0, ((size_t)t.nrows + 1) * 8, G.stream), err);
     if (a.nnz > 0) {
+        const int64_t cap = std::min(a.nnz, chunk);
         DevBuf<uint32_t> rowid, perm_in, perm_out, keys_out;
-        GB_TRY(rowid.alloc((size_t)a.nnz, err)); GB_TRY(perm_in.alloc((size_t)a.nnz, err));
-        GB_TRY(perm_out.alloc((size_t)a.nnz, err)); GB_TRY(keys_out.alloc((size_t)a.nnz, err));
-        expand_rows_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a.rowptr, a.nrows, rowid); GB_LAUNCHED();
-        count_cols_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a.col, a.nnz, t.rowptr); GB_LAUNCHED();
-        iota_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(perm_in, a.nnz); GB_LAUNCHED();
+        GB_TRY(rowid.alloc((size_t)cap, err)); GB_TRY(perm_in.alloc((size_t)cap, err));
+        GB_TRY(perm_out.alloc((size_t)cap, err)); GB_TRY(keys_out.alloc((size_t)cap, err));
+        DevBuf<int64_t> cursor, off;           // chunked: next free slot of every column of T, and the chunk's offset per column
         int end_bit = 1; while (end_bit < 32 && ((int64_t)1 << end_bit) < a.ncols) ++end_bit;
-        size_t tmp_bytes = 0;
-        CU_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, a.col.get(), keys_out.get(), perm_in.get(), perm_out.get(), (int64_t)a.nnz, 0, end_bit, G.stream), err);
-        DevBuf<void> tmp; GB_TRY(tmp.alloc(tmp_bytes, err));
-        CU_TRY(cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, a.col.get(), keys_out.get(), perm_in.get(), perm_out.get(), (int64_t)a.nnz, 0, end_bit, G.stream), err);
-        G.launches += 8;
-        permute_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(perm_out, rowid, (const uint8_t *)a.val, (int)vsize, a.nnz, t.col, (uint8_t *)t.val); GB_LAUNCHED();
+        DevBuf<void> tmp; size_t tmp_bytes = 0;
+        for (int64_t k0 = 0; k0 < a.nnz; k0 += chunk) {
+            const int64_t len = std::min(chunk, a.nnz - k0);
+            if (!chunked) { expand_rows_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a.rowptr, a.nrows, rowid); GB_LAUNCHED(); }
+            else { expand_rows_window_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a.rowptr, a.nrows, k0, len, rowid); GB_LAUNCHED(); }
+            if (k0 == 0) {
+                count_cols_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(a.col, a.nnz, t.rowptr); GB_LAUNCHED();
+                if (chunked) {
+                    GB_TRY(dev_exclusive_scan(t.rowptr, t.nrows + 1, err));
+                    GB_TRY(cursor.alloc((size_t)t.nrows + 1, err)); GB_TRY(off.alloc((size_t)t.nrows + 1, err));
+                    CU_TRY(cudaMemcpyAsync(cursor, t.rowptr, ((size_t)t.nrows + 1) * 8, cudaMemcpyDeviceToDevice, G.stream), err);
+                }
+            }
+            iota_kernel<<<grid_for(len), 256, 0, G.stream>>>(perm_in, len); GB_LAUNCHED();
+            if (!tmp) {
+                CU_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, a.col.get(), keys_out.get(), perm_in.get(), perm_out.get(), len, 0, end_bit, G.stream), err);
+                GB_TRY(tmp.alloc(tmp_bytes, err));
+            }
+            CU_TRY(cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, a.col.get() + k0, keys_out.get(), perm_in.get(), perm_out.get(), len, 0, end_bit, G.stream), err);
+            G.launches += 8;
+            if (!chunked) { permute_kernel<<<grid_for(a.nnz), 256, 0, G.stream>>>(perm_out, rowid, (const uint8_t *)a.val, (int)vsize, a.nnz, t.col, (uint8_t *)t.val); GB_LAUNCHED(); }
+            else {
+                chunk_offsets_kernel<<<grid_for(len), 256, 0, G.stream>>>(keys_out, len, cursor, off); GB_LAUNCHED();
+                chunk_scatter_kernel<<<grid_for(len), 256, 0, G.stream>>>(keys_out, perm_out, rowid, (const uint8_t *)a.val, (int)vsize, k0, len, off, cursor,
+                                                                        t.col, (uint8_t *)t.val); GB_LAUNCHED();
+            }
+        }
     }
-    GB_TRY(dev_exclusive_scan(t.rowptr, t.nrows + 1, err));
+    if (!chunked) GB_TRY(dev_exclusive_scan(t.rowptr, t.nrows + 1, err));
     GB_TRY(dev_build_rowptr32(t, err));
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;

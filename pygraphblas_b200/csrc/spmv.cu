@@ -342,7 +342,9 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const Tunables &tn = tunables();
     std::string hot_note;                    // the burble line names the cluster; it is printed when `burble` is destroyed
     GbBurble burble(fn);
-    GB_TRY(spmv_plan(c, err));
+    // wide route (csr_wide: nnz >= 2^32, or B200_debug_wide): 64-bit row offsets in the plan, pull and push kernels, no tile kernel
+    const bool wide = csr_wide(c);
+    if (!wide) GB_TRY(spmv_plan(c, err));
 
     DevBuf<void> a_cast, u_cast;
     const void *aval = c.val, *uval = u->dval;
@@ -381,14 +383,17 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         if (uval == u->dval && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
         // few frontier edges: push along the rows of the other orientation (already in HBM) instead of pulling every row
         const Csr &o = use_transpose ? A->dev : A->devT;
-        if (sparse_u && o.valid && o.rowptr32 && o.nnz == c.nnz && A->type->code == xt && !tn.no_push) {
-            PushArgs ps{};
-            ps.rowptr = o.rowptr32; ps.col = o.col; ps.aval = o.val; ps.nin = o.nrows; ps.uval = uval; ps.upres = u->dpres;
-            ps.mval = mask->dval; ps.mpres = mask->dpres; ps.mtc = mask->type->code; ps.mask_comp = f.mask_comp; ps.mask_struct = f.mask_struct;
-            ps.tval = tval; ps.tpres = tpres; ps.nout = n; ps.add_op = add; ps.mul_op = kmul; ps.flip = kflip;
-            GB_TRY(spmv_masked_push_try(xt, zt, ps, c.nnz, &pushed, err));
+        if (sparse_u && o.valid && (wide || o.rowptr32) && o.nnz == c.nnz && A->type->code == xt && !tn.no_push) {
+            auto push = [&](auto &ps, const auto *rowptr) {
+                ps.rowptr = rowptr; ps.col = o.col; ps.aval = o.val; ps.nin = o.nrows; ps.uval = uval; ps.upres = u->dpres;
+                ps.mval = mask->dval; ps.mpres = mask->dpres; ps.mtc = mask->type->code; ps.mask_comp = f.mask_comp; ps.mask_struct = f.mask_struct;
+                ps.tval = tval; ps.tpres = tpres; ps.nout = n; ps.add_op = add; ps.mul_op = kmul; ps.flip = kflip;
+                return spmv_masked_push_try(xt, zt, ps, c.nnz, &pushed, err);
+            };
+            PushArgs ps{}; PushArgsWide psw{};
+            GB_TRY(wide ? push(psw, o.rowptr.get()) : push(ps, o.rowptr32.get()));
         }
-        PullArgs pa{};
+        PullArgs pa{}; PullArgsWide paw{};
         pa.rowptr = c.rowptr32; pa.col = c.col; pa.aval = aval; pa.nrows = c.nrows; pa.uval = uval; pa.upres = u->dpres;
         pa.mval = mask->dval; pa.mpres = mask->dpres; pa.mtc = mask->type->code; pa.mask_comp = f.mask_comp; pa.mask_struct = f.mask_struct;
         pa.tval = tval; pa.tpres = tpres; pa.add_op = add; pa.mul_op = kmul; pa.flip = kflip;
@@ -399,12 +404,19 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         GB_TRY(long_count.alloc(4, err));
         pa.long_rows = long_rows; pa.long_count = long_count;
         CU_TRY(cudaMemsetAsync(pa.long_count, 0, sizeof(int), G.stream), err);
-        if (!pushed) GB_TRY(spmv_masked_pull_dispatch(xt, zt, pa, err));
+        if (!pushed && wide) {
+            paw.rowptr = c.rowptr; paw.col = pa.col; paw.aval = pa.aval; paw.nrows = pa.nrows; paw.uval = pa.uval; paw.upres = pa.upres;
+            paw.mval = pa.mval; paw.mpres = pa.mpres; paw.mtc = pa.mtc; paw.mask_comp = pa.mask_comp; paw.mask_struct = pa.mask_struct;
+            paw.tval = pa.tval; paw.tpres = pa.tpres; paw.add_op = pa.add_op; paw.mul_op = pa.mul_op; paw.flip = pa.flip;
+            paw.has_long = pa.has_long; paw.long_cap = pa.long_cap; paw.long_rows = pa.long_rows; paw.long_count = pa.long_count;
+            GB_TRY(spmv_masked_pull_dispatch(xt, zt, paw, err));
+        } else if (!pushed) GB_TRY(spmv_masked_pull_dispatch(xt, zt, pa, err));
     }
     // dense u + specialised semiring: warp-independent run kernel on the cached run plan
     const bool run_ok = !use_pull && (fast_sr || xt == zt || zt == TC_BOOL);     // specialised or run-time operators; dense or sparse u
     bool use_run = run_ok && c.nnz >= 4096;
     if (tn.spmv_run >= 0) use_run = run_ok && c.nnz > 0 && tn.spmv_run != 0;
+    if (wide) use_run = run_ok && c.nnz > 0;          // the wide route has no tile kernel: B200GRB_SPMV_RUN does not apply
     const char *kernel_name = "pull";
     int hot_cluster = 0, hot_ctas = 0; uint32_t hot_t0 = 0, hot_t1 = 0, hot_henc = 0;      // cluster size, grid and tiers of the hot-table launch
     if (use_pull) {
@@ -465,6 +477,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         GB_TRY(spmv_dispatch(xt, zt, add, kmul, sparse_u, a, err));
     }
     gb_kernel_used(kernel_name);
+    if (wide) gb_kernel_used("offsets=64");
     if (in_place) gb_kernel_used("mxv=in-place");
     if (hot_cluster > 0) {
         gb_kernel_used(("hot-cluster=" + std::to_string(hot_cluster)).c_str());
@@ -472,7 +485,8 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         gb_kernel_used(("hot-tiers=" + std::to_string(hot_t0) + "," + std::to_string(hot_t1) + "," + std::to_string(hot_henc)).c_str());
         if (burble.on) { hot_note = std::string(kernel_name) + " cluster " + std::to_string(hot_cluster) + ", T0 " + std::to_string(hot_t0); kernel_name = hot_note.c_str(); }
     }
-    if (burble.on) burble.note(kernel_name,(double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * 4 + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
+    if (burble.on && wide) { hot_note = std::string(kernel_name) + ", 64-bit offsets"; kernel_name = hot_note.c_str(); }
+    if (burble.on) burble.note(kernel_name,(double)c.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)(c.nrows + 1) * (wide ? 8 : 4) + (double)c.ncols * (need_u ? tc_size(xt) : 0) + (double)n * (zsz + 1));
     a_cast.reset(); u_cast.reset();
     vector_mark_used(u); if (mask) vector_mark_used(mask);          // an overlapped import into u may start as soon as these kernels are done
 

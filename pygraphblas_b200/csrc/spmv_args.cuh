@@ -39,8 +39,9 @@ struct Hot2Args {
 // saturates -- the BFS step `A.mxv(q, mask=visited, desc=RC, semiring=LOR_LAND)` of
 // reference: tests/test_descriptor.py:13-30 touches only the unvisited rows and, for each, only the
 // entries up to the first frontier hit.  Output: T restricted to the rows the mask lets through.
-struct PullArgs {
-    const uint32_t *rowptr; const uint32_t *col; const void *aval; int64_t nrows;
+// OT: the type of the row offsets (uint32_t: rowptr32; int64_t: rowptr, the wide route of matrices with >= 2^32 entries).
+template <typename OT> struct PullArgsT {
+    const OT *rowptr; const uint32_t *col; const void *aval; int64_t nrows;
     const void *uval; const uint8_t *upres;
     const void *mval; const uint8_t *mpres; int mtc; int mask_comp, mask_struct;
     void *tval; uint8_t *tpres;
@@ -48,6 +49,8 @@ struct PullArgs {
     int has_long; int64_t long_cap;
     uint32_t *long_rows; int *long_count;                      // work list of the rows left to the CTA-per-row kernel
 };
+using PullArgs = PullArgsT<uint32_t>;
+using PullArgsWide = PullArgsT<int64_t>;
 constexpr uint32_t PULL_LONG = 4096;          // rows longer than this go to the CTA-per-row kernel
 
 // ------------------------------------------------------------------ masked push for small frontiers (same three monoids)
@@ -55,12 +58,15 @@ constexpr uint32_t PULL_LONG = 4096;          // rows longer than this go to the
 // T(j) for the columns j the mask lets through.  LOR / LAND / ANY need no atomics: T(j) starts at the monoid's
 // identity-like value and every store is idempotent (LOR: "a product was true", LAND: "a product was false",
 // ANY: any product).  Work is proportional to the frontier's out-edges; used when those are < nnz / 16.
-struct PushArgs {
-    const uint32_t *rowptr; const uint32_t *col; const void *aval; int64_t nin;    // CSR whose rows are the input positions k
+template <typename OT> struct PushArgsT {
+    const OT *rowptr; const uint32_t *col; const void *aval; int64_t nin;    // CSR whose rows are the input positions k
     const void *uval; const uint8_t *upres;
     const void *mval; const uint8_t *mpres; int mtc; int mask_comp, mask_struct;
     void *tval; uint8_t *tpres; int64_t nout;
     int add_op, mul_op, flip;
     uint32_t *list; int64_t *chunk_scan; unsigned long long *counters;           // frontier list, chunk offsets, {count, edges}
 };
-GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bool *done, std::string *err);
+using PushArgs = PushArgsT<uint32_t>;
+using PushArgsWide = PushArgsT<int64_t>;
+template <typename OT> GrB_Info spmv_masked_push_try(int xt, int zt, PushArgsT<OT> &a, int64_t nnz_total, bool *done, std::string *err);
+template <typename OT> GrB_Info spmv_masked_pull_dispatch(int xt, int zt, const PullArgsT<OT> &a, std::string *err);

@@ -89,6 +89,3 @@ void spmv_hot2_prep(const Hot2Args &h);
 bool spmv_run_dispatch(int xt, int add, int mul, const RunArgs &a, Hot2Args *hot, size_t table_limit);
 bool spmv_run_generic(int xt, int zt, const RunArgs &a);
 
-// ---- masked pull kernels (spmv_pull.cu)
-struct PullArgs;
-GrB_Info spmv_masked_pull_dispatch(int xt, int zt, const PullArgs &a, std::string *err);

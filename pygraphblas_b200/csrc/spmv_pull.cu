@@ -26,8 +26,8 @@ template <typename ZT> __device__ __forceinline__ bool pull_settled(int add, ZT 
         default: return false;
     }
 }
-template <typename XT, typename ZT>
-__device__ __forceinline__ ZT pull_product(const PullArgs &p, const XT *aval, const XT *uval, uint32_t k, uint32_t c) {
+template <typename XT, typename ZT, typename OT>
+__device__ __forceinline__ ZT pull_product(const PullArgsT<OT> &p, const XT *aval, const XT *uval, OT k, uint32_t c) {
     const XT a = gload<XT>(aval + k), u = gload<XT>(uval + c);
     return p.flip ? MulApply<XT, ZT>::f(p.mul_op, u, a) : MulApply<XT, ZT>::f(p.mul_op, a, u);
 }
@@ -35,9 +35,9 @@ __device__ __forceinline__ ZT pull_product(const PullArgs &p, const XT *aval, co
 // Warp batches of 32 rows, their entries flattened: lane i owns row base+i (mask, accumulators, result) while
 // the entries of all 32 rows are walked 32 at a time, so short rows cost one slot per entry instead of one
 // warp iteration per row.  Rows advance in rounds of at most `cap` entries each; a row whose result is settled
-// leaves the batch at the end of the round.
-template <typename XT, typename ZT>
-__global__ void __launch_bounds__(256) spmv_masked_pull_kernel(const PullArgs p) {
+// leaves the batch at the end of the round.  OT: the type of the row offsets (spmv_args.cuh); a row's length fits 32 bits.
+template <typename XT, typename ZT, typename OT>
+__global__ void __launch_bounds__(256) spmv_masked_pull_kernel(const PullArgsT<OT> p) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -53,9 +53,9 @@ __global__ void __launch_bounds__(256) spmv_masked_pull_kernel(const PullArgs p)
             if (p.mask_comp) m = !m;
             if (!m) p.tpres[mr] = 0;
         }
-        uint32_t pos = 0, rem = 0;
+        OT pos = 0; uint32_t rem = 0;
         if (m) {
-            pos = p.rowptr[mr]; rem = p.rowptr[mr + 1] - pos;
+            pos = p.rowptr[mr]; rem = (uint32_t)(p.rowptr[mr + 1] - pos);
             if (rem > PULL_LONG) { p.long_rows[atomicAdd(p.long_count, 1)] = (uint32_t)mr; rem = 0; m = false; }
         }
         int n_it = 0; bool sat = false; ZT first = (ZT)0;
@@ -67,17 +67,17 @@ __global__ void __launch_bounds__(256) spmv_masked_pull_kernel(const PullArgs p)
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
             const uint32_t off = incl - take, total = __shfl_sync(0xffffffffu, incl, 31);
-            const uint32_t delta = pos - off;                  // entry index = delta(owner) + flat position
+            const OT delta = pos - off;                        // entry index = delta(owner) + flat position
             for (uint32_t f0 = 0; f0 < total; f0 += 32) {
                 const uint32_t f = f0 + lane;
                 int own = 0;                                   // first lane whose inclusive end exceeds f
 #pragma unroll
                 for (int step = 16; step > 0; step >>= 1) { const uint32_t t = __shfl_sync(0xffffffffu, incl, own + step - 1); if (t <= f) own += step; }
-                const uint32_t k = __shfl_sync(0xffffffffu, delta, own) + f;
+                const OT k = __shfl_sync(0xffffffffu, delta, own) + f;
                 bool has = false; ZT v = (ZT)0;
                 if (f < total) {
                     const uint32_t c = __ldg(p.col + k);
-                    if (!p.upres || __ldg(p.upres + c)) { v = pull_product<XT, ZT>(p, aval, uval, k, c); has = true; }
+                    if (!p.upres || __ldg(p.upres + c)) { v = pull_product<XT, ZT, OT>(p, aval, uval, k, c); has = true; }
                 }
                 const unsigned hasmask = __ballot_sync(0xffffffffu, has);
                 const unsigned satmask = __ballot_sync(0xffffffffu, has && monoid_saturated<ZT>(add, v));
@@ -100,8 +100,8 @@ __global__ void __launch_bounds__(256) spmv_masked_pull_kernel(const PullArgs p)
     }
 }
 // Long rows (hubs): one 1024-thread CTA per row, 1024 entries per iteration, early exit CTA-wide.
-template <typename XT, typename ZT>
-__global__ void __launch_bounds__(1024) spmv_pull_long_kernel(const PullArgs p) {
+template <typename XT, typename ZT, typename OT>
+__global__ void __launch_bounds__(1024) spmv_pull_long_kernel(const PullArgsT<OT> p) {
     __shared__ int s_n[32]; __shared__ int s_sat[32]; __shared__ ZT s_first[32];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const XT *aval = static_cast<const XT *>(p.aval), *uval = static_cast<const XT *>(p.uval);
@@ -110,15 +110,15 @@ __global__ void __launch_bounds__(1024) spmv_pull_long_kernel(const PullArgs p) 
     const int nlong = *p.long_count;
     for (int w = blockIdx.x; w < nlong; w += gridDim.x) {
         const uint32_t r = p.long_rows[w];
-        const uint32_t rs = p.rowptr[r], re = p.rowptr[r + 1];
+        const OT rs = p.rowptr[r], re = p.rowptr[r + 1];
         int n_it = 0; bool sat = false; ZT first = (ZT)0;
-        for (uint32_t b0 = rs; b0 < re; b0 += 1024) {
-            const uint32_t k = b0 + threadIdx.x;
+        for (OT b0 = rs; b0 < re; b0 += 1024) {
+            const OT k = b0 + threadIdx.x;
             int stop = 0;
             if (k < re) {
                 const uint32_t c = __ldg(p.col + k);
                 if (!p.upres || __ldg(p.upres + c)) {
-                    const ZT v = pull_product<XT, ZT>(p, aval, uval, k, c);
+                    const ZT v = pull_product<XT, ZT, OT>(p, aval, uval, k, c);
                     if (n_it == 0) first = v;
                     n_it = min(2, n_it + 1);
                     if (monoid_saturated<ZT>(add, v)) { sat = true; stop = pull_settled<ZT>(add, v); }
@@ -140,20 +140,22 @@ __global__ void __launch_bounds__(1024) spmv_pull_long_kernel(const PullArgs p) 
         __syncthreads();
     }
 }
-GrB_Info spmv_masked_pull_dispatch(int xt, int zt, const PullArgs &a, std::string *err) {
+template <typename OT> GrB_Info spmv_masked_pull_dispatch(int xt, int zt, const PullArgsT<OT> &a, std::string *err) {
     const int grid = grid_for(a.nrows, 256, 8), lgrid = grid_for(a.long_cap, 1, 2);
     bool ok;
     GB_FOR_DOMAINS(xt, zt, ok,
-        spmv_masked_pull_kernel<XT_, ZT_><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED();
-        if (a.has_long) { spmv_pull_long_kernel<XT_, ZT_><<<lgrid, 1024, 0, G.stream>>>(a); GB_LAUNCHED(); });
+        spmv_masked_pull_kernel<XT_, ZT_, OT><<<grid, 256, 0, G.stream>>>(a); GB_LAUNCHED();
+        if (a.has_long) { spmv_pull_long_kernel<XT_, ZT_, OT><<<lgrid, 1024, 0, G.stream>>>(a); GB_LAUNCHED(); });
     return ok ? GrB_SUCCESS : gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
 }
+template GrB_Info spmv_masked_pull_dispatch<uint32_t>(int, int, const PullArgs &, std::string *);
+template GrB_Info spmv_masked_pull_dispatch<int64_t>(int, int, const PullArgsWide &, std::string *);
 
 
 // ------------------------------------------------------------------ push
 constexpr int PUSH_CHUNK = 1024;
 // size of the frontier and of its out-edge set: one atomic pair per CTA
-__global__ void __launch_bounds__(256) push_stats_kernel(const PushArgs a) {
+template <typename OT> __global__ void __launch_bounds__(256) push_stats_kernel(const PushArgsT<OT> a) {
     __shared__ unsigned long long s_c[8], s_d[8];
     unsigned long long cnt = 0, deg = 0;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.nin; k += (int64_t)gridDim.x * blockDim.x)
@@ -167,7 +169,7 @@ __global__ void __launch_bounds__(256) push_stats_kernel(const PushArgs a) {
     }
 }
 // the frontier as a list (order irrelevant): warp-aggregated append
-__global__ void __launch_bounds__(256) push_frontier_kernel(const PushArgs a) {
+template <typename OT> __global__ void __launch_bounds__(256) push_frontier_kernel(const PushArgsT<OT> a) {
     const int lane = threadIdx.x & 31;
     for (int64_t base = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) - lane; base < a.nin; base += (int64_t)gridDim.x * blockDim.x) {
         const int64_t k = base + lane;
@@ -180,7 +182,7 @@ __global__ void __launch_bounds__(256) push_frontier_kernel(const PushArgs a) {
         if (in) a.list[pos + __popc(m & ((1u << lane) - 1u))] = (uint32_t)k;
     }
 }
-__global__ void push_chunks_kernel(const PushArgs a, int64_t count) {
+template <typename OT> __global__ void push_chunks_kernel(const PushArgsT<OT> a, int64_t count) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= count; i += (int64_t)gridDim.x * blockDim.x) {
         int64_t c = 0;
         if (i < count) { const uint32_t k = a.list[i]; c = ((int64_t)(a.rowptr[k + 1] - a.rowptr[k]) + PUSH_CHUNK - 1) / PUSH_CHUNK; }
@@ -191,8 +193,8 @@ template <typename ZT> __global__ void push_init_kernel(ZT *tval, uint8_t *tpres
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) { tval[i] = init; tpres[i] = 0; }
 }
 // one warp per chunk of <= PUSH_CHUNK entries of a frontier row
-template <typename XT, typename ZT>
-__global__ void __launch_bounds__(256) push_kernel(const PushArgs a, int64_t count) {
+template <typename XT, typename ZT, typename OT>
+__global__ void __launch_bounds__(256) push_kernel(const PushArgsT<OT> a, int64_t count) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const int64_t nchunks = a.chunk_scan[count];
@@ -202,10 +204,10 @@ __global__ void __launch_bounds__(256) push_kernel(const PushArgs a, int64_t cou
         int64_t lo = 0, hi = count;                              // owner: last i with chunk_scan[i] <= c
         while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if (a.chunk_scan[mid] <= c) lo = mid; else hi = mid; }
         const uint32_t k = a.list[lo];
-        const uint32_t rs = a.rowptr[k] + (uint32_t)(c - a.chunk_scan[lo]) * PUSH_CHUNK;
-        const uint32_t re = min(a.rowptr[k + 1], rs + (uint32_t)PUSH_CHUNK);
+        const OT rs = a.rowptr[k] + (uint32_t)(c - a.chunk_scan[lo]) * PUSH_CHUNK;      // a row's length fits 32 bits
+        const OT re = min(a.rowptr[k + 1], rs + (OT)PUSH_CHUNK);
         const XT uk = gload<XT>(uval + k);
-        for (uint32_t e = rs + lane; e < re; e += 32) {
+        for (OT e = rs + lane; e < re; e += 32) {
             const uint32_t j = __ldg(a.col + e);
             bool m = a.mpres ? a.mpres[j] != 0 : true;
             if (m && !a.mask_struct) m = mask_value_true(a.mtc, a.mval, (int64_t)j);
@@ -220,14 +222,14 @@ __global__ void __launch_bounds__(256) push_kernel(const PushArgs a, int64_t cou
         }
     }
 }
-template <typename XT, typename ZT> static void push_launch(const PushArgs &a, int64_t count, int64_t chunk_bound) {
+template <typename XT, typename ZT, typename OT> static void push_launch(const PushArgsT<OT> &a, int64_t count, int64_t chunk_bound) {
     const ZT init = a.add_op == OP_LAND ? (ZT)1 : (ZT)0;
     push_init_kernel<ZT><<<grid_for(a.nout), 256, 0, G.stream>>>(static_cast<ZT *>(a.tval), a.tpres, a.nout, init); GB_LAUNCHED();
     if (count > 0) {
-        push_kernel<XT, ZT><<<grid_for(chunk_bound * 32), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
+        push_kernel<XT, ZT, OT><<<grid_for(chunk_bound * 32), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
     }
 }
-GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bool *done, std::string *err) {
+template <typename OT> GrB_Info spmv_masked_push_try(int xt, int zt, PushArgsT<OT> &a, int64_t nnz_total, bool *done, std::string *err) {
     *done = false;
     // LOR / LAND results are normalised only when the monoid type is BOOL (every builtin); ANY stores the product as is
     if ((a.add_op == OP_LOR || a.add_op == OP_LAND) && zt != TC_BOOL) return GrB_SUCCESS;
@@ -236,7 +238,7 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     GB_TRY(counters.alloc(4, err));
     a.counters = counters;
     CU_TRY(cudaMemsetAsync(a.counters, 0, 32, G.stream), err);
-    push_stats_kernel<<<grid_for(a.nin, 256 * 4, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    push_stats_kernel<OT><<<grid_for(a.nin, 256 * 4, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     unsigned long long h[2] = {0, 0};
     CU_TRY(cudaMemcpyAsync(h, a.counters, 16, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
@@ -246,18 +248,20 @@ GrB_Info spmv_masked_push_try(int xt, int zt, PushArgs &a, int64_t nnz_total, bo
     GB_TRY(list.alloc((size_t)count + 1, err));
     a.list = list;
     if (count > 0) {
-        push_frontier_kernel<<<grid_for(a.nin), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+        push_frontier_kernel<OT><<<grid_for(a.nin), 256, 0, G.stream>>>(a); GB_LAUNCHED();
     }
     GB_TRY(chunk_scan.alloc((size_t)count + 2, err));
     a.chunk_scan = chunk_scan;
     if (count > 0) {
-        push_chunks_kernel<<<grid_for(count + 1), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
+        push_chunks_kernel<OT><<<grid_for(count + 1), 256, 0, G.stream>>>(a, count); GB_LAUNCHED();
         GB_TRY(dev_exclusive_scan(a.chunk_scan, count + 1, err));
     } else CU_TRY(cudaMemsetAsync(a.chunk_scan, 0, 16, G.stream), err);
     const int64_t chunk_bound = edges / PUSH_CHUNK + count + 1;
     bool ok;
-    GB_FOR_DOMAINS(xt, zt, ok, push_launch<XT_, ZT_>(a, count, chunk_bound));
+    GB_FOR_DOMAINS(xt, zt, ok, push_launch<XT_, ZT_, OT>(a, count, chunk_bound));
     CU_TRY(cudaGetLastError(), err);
     *done = ok;
     return GrB_SUCCESS;
 }
+template GrB_Info spmv_masked_push_try<uint32_t>(int, int, PushArgs &, int64_t, bool *, std::string *);
+template GrB_Info spmv_masked_push_try<int64_t>(int, int, PushArgsWide &, int64_t, bool *, std::string *);

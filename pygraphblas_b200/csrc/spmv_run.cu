@@ -2,16 +2,18 @@
 #include "spmv_run.cuh"
 #include <cub/device/device_radix_sort.cuh>
 
-// ---- run plan (cached per CSR)
-__global__ void plan_nonempty_kernel(const uint32_t *rowptr, int64_t nrows, int64_t *flag, uint8_t *pres) {
+// ---- run plan (cached per CSR).  OT: the type of the row offsets read (uint32_t: rowptr32; int64_t: rowptr, the wide route)
+template <typename OT>
+__global__ void plan_nonempty_kernel(const OT *rowptr, int64_t nrows, int64_t *flag, uint8_t *pres) {
     for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
         const int ne = rowptr[r + 1] > rowptr[r];
         flag[r] = ne; pres[r] = (uint8_t)ne;
     }
 }
-__global__ void plan_rows_kernel(const uint32_t *rowptr, const int64_t *rank, int64_t nrows, uint32_t *nzrow, uint32_t *headw) {
+template <typename OT>
+__global__ void plan_rows_kernel(const OT *rowptr, const int64_t *rank, int64_t nrows, uint32_t *nzrow, uint32_t *headw) {
     for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
-        const uint32_t rs = rowptr[r];
+        const OT rs = rowptr[r];
         if (rowptr[r + 1] > rs) { nzrow[rank[r]] = (uint32_t)r; atomicOr(&headw[rs >> 5], 1u << (rs & 31)); }
     }
 }
@@ -32,23 +34,23 @@ __global__ void plan_base_kernel(const int64_t *scan, int64_t nruns, uint32_t *r
 }
 // the row that starts last inside a run always holds the run's last entry: it is the run's "open" row
 // (possibly ending exactly at the run's end), completed by the fix-up kernel
-__global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzrow, const uint32_t *rowptr, int64_t nruns,
+template <typename OT>
+__global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzrow, const OT *rowptr, int64_t nruns,
                                   int32_t *tail_row, uint32_t *tail_last) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nruns; k += (int64_t)gridDim.x * blockDim.x) {
         int32_t tr = -1; uint32_t tl = 0;
         if (run_base[k + 1] > run_base[k]) {
             const uint32_t r = nzrow[run_base[k + 1] - 1];
-            const uint32_t re = rowptr[r + 1];
-            tr = (int32_t)r; tl = (re - 1) / RUN;
+            const OT re = rowptr[r + 1];
+            tr = (int32_t)r; tl = (uint32_t)((re - 1) / RUN);
         }
         tail_row[k] = tr; tail_last[k] = tl;
     }
 }
 
-GrB_Info spmv_run_plan(Csr &c, std::string *err) {
-    if (c.run.headw) return GrB_SUCCESS;
-    if (!c.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "mxv: matrices with >= 2^32 entries are not supported");
+template <typename OT> static GrB_Info spmv_run_plan_t(Csr &c, const OT *rowptr, std::string *err) {
     RunPlan p;                 // moved into c only once complete
+    p.wide = sizeof(OT) == 8;
     const int64_t nwords = ceil_div(c.nnz, 32);
     p.nruns = ceil_div(c.nnz, RUN);
     DevBuf<int64_t> flag, cnt;
@@ -62,19 +64,19 @@ GrB_Info spmv_run_plan(Csr &c, std::string *err) {
     GB_TRY(p.tail_last.alloc((size_t)p.nruns, err));
     CU_TRY(cudaMemsetAsync(p.headw, 0, ((size_t)nwords + 8) * 4, G.stream), err);
     CU_TRY(cudaMemsetAsync(flag + c.nrows, 0, 8, G.stream), err);
-    plan_nonempty_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr32, c.nrows, flag, p.pres_tmpl); GB_LAUNCHED();
+    plan_nonempty_kernel<OT><<<grid_for(c.nrows), 256, 0, G.stream>>>(rowptr, c.nrows, flag, p.pres_tmpl); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(flag, c.nrows + 1, err));
     int64_t nz = 0;
     CU_TRY(cudaMemcpyAsync(&nz, flag + c.nrows, 8, cudaMemcpyDeviceToHost, G.stream), err);
     CU_TRY(cudaStreamSynchronize(G.stream), err);
     p.nnzrows = nz;
     GB_TRY(p.nzrow.alloc((size_t)nz, err));
-    plan_rows_kernel<<<grid_for(c.nrows), 256, 0, G.stream>>>(c.rowptr32, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
+    plan_rows_kernel<OT><<<grid_for(c.nrows), 256, 0, G.stream>>>(rowptr, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
     CU_TRY(cudaMemsetAsync(cnt + p.nruns, 0, 8, G.stream), err);
     plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, p.lane, cnt); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
     plan_base_kernel<<<grid_for(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
-    plan_tails_kernel<<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, c.rowptr32, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
+    plan_tails_kernel<OT><<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, rowptr, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
     flag.reset(); cnt.reset();
     // per-call scratch lives with the plan: partials of the rows that straddle runs (8 bytes covers every type)
     GB_TRY(p.ws_head.alloc((size_t)p.nruns * 8 + 16, err));
@@ -84,6 +86,13 @@ GrB_Info spmv_run_plan(Csr &c, std::string *err) {
     CU_TRY(cudaGetLastError(), err);
     c.run = std::move(p);
     return GrB_SUCCESS;
+}
+// the plan of the route csr_wide picks: a plan built by the other route is built again (they are equal; B200_debug_wide tests both)
+GrB_Info spmv_run_plan(Csr &c, std::string *err) {
+    const bool wide = csr_wide(c);
+    if (c.run.headw && c.run.wide == wide) return GrB_SUCCESS;
+    c.run = RunPlan();
+    return wide ? spmv_run_plan_t<int64_t>(c, c.rowptr, err) : spmv_run_plan_t<uint32_t>(c, c.rowptr32, err);
 }
 
 // ---- hot-column plan (cached per CSR): the HOT_EXT most referenced columns are renamed to their rank, every other

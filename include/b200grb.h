@@ -234,9 +234,10 @@ uint64_t B200_kernel_launches(void);
  * the device (k = 0 switches it off); and the number of device blocks allocated and not yet freed */
 void B200_debug_fail_alloc(int64_t k);
 int64_t B200_debug_live_allocs(void);
-/* wide-route test seam: chunk > 0 puts every GrB_mxv / GrB_vxm and every transpose on the code that serves matrices with
- * 2^32 or more entries (64-bit entry offsets; transposes cut into chunks of `chunk` entries), whatever the matrix's size;
- * 0 switches it off.  The 32-bit row offsets stay built for the other operations */
+/* wide-route test seam: chunk > 0 puts every GrB_mxv / GrB_vxm, every transpose and the SpMM, dense-left and SDDMM routes of
+ * GrB_mxm on the code that serves matrices with 2^32 or more entries (64-bit entry offsets; transposes and SDDMM masks cut into
+ * chunks of `chunk` entries), whatever the matrix's size; 0 switches it off.  The 32-bit row offsets stay built for the other
+ * operations */
 void B200_debug_wide(int64_t chunk);
 /* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("tile (specialised, 8 items)",
  * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "spa-split", "masked-warp", "stream-L",

@@ -203,14 +203,19 @@ struct GBGlobal {
     int burble = 0;
     cudaEvent_t burble_e0 = nullptr, burble_e1 = nullptr;
     std::string last_kernel;      // kernel paths of the last GrB_mxv / GrB_vxm / GrB_mxm, separated by ';' (B200_debug_last_kernel)
-    int64_t debug_wide = 0;       // B200_debug_wide: > 0 puts every mxv / vxm / transpose on the wide route, transposes in chunks of this many entries
+    int64_t debug_wide = 0;       // B200_debug_wide: > 0 puts every mxv / vxm / transpose and the SpMM, dense-left and SDDMM
+                                  // routes of mxm on the wide route; transposes and SDDMM masks go in chunks of this many entries
     std::recursive_mutex mu;
 };
 extern GBGlobal G;
 static inline void gb_kernel_used(const char *k) { if (!G.last_kernel.empty()) G.last_kernel += ';'; G.last_kernel += k; }
-// the wide route of mxv / vxm (DESIGN.md section 3.1): 64-bit entry offsets, for a CSR without rowptr32 (nnz >= 2^32), and for
-// every CSR while B200_debug_wide is on
+// the wide route of mxv / vxm and of the dense-operand mxm (DESIGN.md sections 3.1 and 3.6): 64-bit entry offsets, for a CSR
+// without rowptr32 (nnz >= 2^32), and for every CSR while B200_debug_wide is on
 static inline bool csr_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide > 0; }
+// entries per chunk of the wide route's chunked passes (the transpose, the mask of SDDMM): 2^27, or B200_debug_wide's chunk,
+// at most 2^31 (the transpose's permutations are 32-bit)
+static constexpr int64_t TRANSPOSE_CHUNK = (int64_t)1 << 27;
+static inline int64_t wide_chunk() { return G.debug_wide > 0 ? std::min(G.debug_wide, (int64_t)1 << 31) : TRANSPOSE_CHUNK; }
 extern thread_local std::string tl_error;
 
 GrB_Info gb_fail(GrB_Info code, std::string *where, const char *fmt, ...);

@@ -166,9 +166,8 @@ __global__ void chunk_scatter_kernel(const uint32_t *keys, const uint32_t *perm,
 // column offsets of T), so every column of T still receives its rows in ascending order -- the same arrays as one sort.
 // Peak scratch: 16 bytes per chunk entry (row ids, two permutations, sorted keys) + the sort's own (about 8 bytes per chunk entry)
 // + 16 bytes per column of A when chunked: about 3.2 GB at TRANSPOSE_CHUNK = 2^27.  A single chunk runs the unchunked launches.
-static constexpr int64_t TRANSPOSE_CHUNK = (int64_t)1 << 27;
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err) {
-    const int64_t chunk = G.debug_wide > 0 ? std::min(G.debug_wide, (int64_t)1 << 31) : TRANSPOSE_CHUNK;     // 32-bit permutations
+    const int64_t chunk = wide_chunk();
     const bool chunked = a.nnz > chunk;
     t = Csr(); t.nrows = a.ncols; t.ncols = a.nrows; t.nnz = a.nnz;
     GB_TRY(t.rowptr.alloc((size_t)t.nrows + 1, err));

@@ -33,6 +33,17 @@ __global__ void sddmm_rowid_kernel(const uint32_t *rowptr, int64_t m, uint32_t *
         for (uint32_t q = rowptr[r] + lane; q < rowptr[r + 1]; q += 32) mrow[q] = (uint32_t)r;
 }
 
+// the wide route: warp per row of M, the row id of each of its entries in the chunk [q0, q1), at mrow[q - q0].  Reads the 64-bit
+// row offsets and keeps only a chunk's row ids; every row is visited once per chunk (16 bytes of offsets each).
+__global__ void sddmm_rowid_wide_kernel(const int64_t *rowptr, int64_t m, int64_t q0, int64_t q1, uint32_t *mrow) {
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    for (int64_t r = warp; r < m; r += nwarps) {
+        const int64_t e = min(rowptr[r + 1], q1);
+        for (int64_t q = max(rowptr[r], q0) + lane; q < e; q += 32) mrow[q - q0] = (uint32_t)r;
+    }
+}
+
 // The monoid's operator on two values of the fold.  A floating-point PLUS is the explicitly rounded add, which the compiler
 // never contracts with the multiply before it into a fused multiply-add: the oracle rounds the product and the sum separately,
 // and up to one chunk the result is its left-to-right fold bit for bit, whatever the values.
@@ -177,7 +188,7 @@ GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
     const int xt = mulop->xtype->code, zt = addop->ztype->code, add = addop->opcode, mul = mulop->opcode;
     const size_t zsz = tc_size(zt);
     gb_kernel_used("sddmm");
-    const Csr &M = Mask->dev;                           // on the device, with rowptr32 (GrB_mxm)
+    const Csr &M = Mask->dev;                           // on the device (GrB_mxm)
     const int64_t m = M.nrows, n = M.ncols, d = (int64_t)(f.tran0 ? A->nrows : A->ncols);
     SddmmOperand X, Y;
     GB_TRY(sddmm_operand(A, mul_reads_x(mul), xt, f.tran0 && d > 1, "x-transpose", X, err));
@@ -194,21 +205,32 @@ GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
         GB_TRY(ws_get(WS_WORDS, &tval, (size_t)M.nnz * zsz + 16, err));
         GB_TRY(ws_get(WS_FOUND, (void **)&found, (size_t)M.nnz + 16, err));
     }
+    // the wide route (csr_wide: nnz(M) >= 2^32, or B200_debug_wide) takes M in chunks of entries: the row ids of one chunk
+    // from the 64-bit row offsets, then the same kernel on that chunk's slice of M and T
+    const bool wide = csr_wide(M);
     if (M.nnz > 0 && d > 0) {
+        const int64_t chunk = !wide ? M.nnz : std::min(M.nnz, wide_chunk());
         uint32_t *mrow = nullptr;
-        GB_TRY(ws_array(WS_MASK_ROW, &mrow, (size_t)M.nnz, err));
-        sddmm_rowid_kernel<<<grid_for(m * 32), 256, 0, G.stream>>>(M.rowptr32, m, mrow); GB_LAUNCHED();
-        SddmmArgs p{};
-        p.mrow = mrow; p.mcol = M.col; p.mval = M.val; p.mtc = Mask->type->code; p.m_struct = f.mask_struct;
-        p.xval = X.val; p.xpres = X.pres; p.yval = Y.val; p.ypres = Y.pres;
-        p.d = d; p.nnz = M.nnz; p.add = add; p.mul = mul;
-        p.vec = (d * (int64_t)tc_size(xt)) % 16 == 0 && (uintptr_t)X.val % 16 == 0 && (uintptr_t)Y.val % 16 == 0;
-        p.tval = tval; p.found = found;
+        GB_TRY(ws_array(WS_MASK_ROW, &mrow, (size_t)chunk, err));
+        if (!wide) { sddmm_rowid_kernel<<<grid_for(m * 32), 256, 0, G.stream>>>(M.rowptr32, m, mrow); GB_LAUNCHED(); }
+        const size_t msz = tc_size(Mask->type->code);
         bool fast = false;
-        if (!sddmm_launch(xt, zt, p, &fast))
-            return gb_fail(GrB_DOMAIN_MISMATCH, err, "GrB_mxm: unsupported semiring domains (x=%d, z=%d)", xt, zt);
-        GB_LAUNCHED();
+        for (int64_t q0 = 0; q0 < M.nnz; q0 += chunk) {
+            const int64_t q1 = std::min(q0 + chunk, M.nnz);
+            if (wide) { sddmm_rowid_wide_kernel<<<grid_for(m * 32), 256, 0, G.stream>>>(M.rowptr, m, q0, q1, mrow); GB_LAUNCHED(); }
+            SddmmArgs p{};
+            p.mrow = mrow; p.mcol = M.col + q0; p.mval = M.val.get() ? (const uint8_t *)M.val.get() + q0 * msz : nullptr;
+            p.mtc = Mask->type->code; p.m_struct = f.mask_struct;
+            p.xval = X.val; p.xpres = X.pres; p.yval = Y.val; p.ypres = Y.pres;
+            p.d = d; p.nnz = q1 - q0; p.add = add; p.mul = mul;
+            p.vec = (d * (int64_t)tc_size(xt)) % 16 == 0 && (uintptr_t)X.val % 16 == 0 && (uintptr_t)Y.val % 16 == 0;
+            p.tval = (uint8_t *)tval + q0 * zsz; p.found = found ? found + q0 : nullptr;
+            if (!sddmm_launch(xt, zt, p, &fast))
+                return gb_fail(GrB_DOMAIN_MISMATCH, err, "GrB_mxm: unsupported semiring domains (x=%d, z=%d)", xt, zt);
+            GB_LAUNCHED();
+        }
         gb_kernel_used(fast ? "sddmm-fast" : "sddmm-generic");
+        if (wide) gb_kernel_used("offsets=64");
     } else if (found && M.nnz > 0) {
         CU_TRY(cudaMemsetAsync(found, 0, (size_t)M.nnz, G.stream), err);      // d = 0: no entry has a product
     }
@@ -226,8 +248,8 @@ GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum
     // algorithmic bytes: M (ids, row pointers, values when it is valued), X and Y once, T (ids, values, row pointers), and the
     // transposes built.  Left out: the gather, nnz(M) d b_Y -- rows of Y are read once per entry that names them, and how much of
     // that the caches absorb depends on M.
-    const double bytes = (double)M.nnz * 4 + (double)(m + 1) * 4 + (f.mask_struct ? 0.0 : (double)M.nnz * tc_size(Mask->type->code)) +
+    const double bytes = (double)M.nnz * 4 + (double)(m + 1) * (wide ? 8 : 4) + (f.mask_struct ? 0.0 : (double)M.nnz * tc_size(Mask->type->code)) +
                          operand_bytes + (double)T.nnz * (4 + tc_size(C->type->code)) + (double)(m + 1) * 8;
-    burble.note("sddmm", bytes);
+    burble.note(wide ? "sddmm, 64-bit offsets" : "sddmm", bytes);
     return matrix_writeback(C, Mask, accum, f, std::move(T), zt, /*masked=*/true, err);
 }

@@ -786,26 +786,28 @@ __global__ void __launch_bounds__(256) masked_dot_kernel(const GemmArgs p) {
 }
 
 // ------------------------------------------------------------------ compaction of a masked result (pattern of M, found flags) into CSR
-__global__ void row_found_count_kernel(const uint32_t *m_ptr, const uint8_t *found, int64_t nrows, int64_t *cnt) {
+// OT: the type of M's row offsets (uint32_t: rowptr32; int64_t: rowptr, the wide route of SDDMM)
+template <typename OT> __global__ void row_found_count_kernel(const OT *m_ptr, const uint8_t *found, int64_t nrows, int64_t *cnt) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < nrows; r += nwarps) {
         int c = 0;
-        for (uint32_t q = m_ptr[r] + lane; q < m_ptr[r + 1]; q += 32) c += found[q] != 0;
+        for (OT q = m_ptr[r] + lane; q < m_ptr[r + 1]; q += 32) c += found[q] != 0;
         for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
         if (lane == 0) cnt[r] = c;
     }
 }
-__global__ void row_found_fill_kernel(const uint32_t *m_ptr, const uint32_t *m_col, const uint8_t *found, const uint8_t *tval, int vsize,
+template <typename OT>
+__global__ void row_found_fill_kernel(const OT *m_ptr, const uint32_t *m_col, const uint8_t *found, const uint8_t *tval, int vsize,
                                       int64_t nrows, const int64_t *c_ptr, uint32_t *c_col, uint8_t *c_val) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < nrows; r += nwarps) {
         int64_t out = c_ptr[r];
-        for (uint32_t q0 = m_ptr[r]; q0 < m_ptr[r + 1]; q0 += 32) {
-            const uint32_t q = q0 + lane;
+        for (OT q0 = m_ptr[r]; q0 < m_ptr[r + 1]; q0 += 32) {
+            const OT q = q0 + lane;
             const bool f = q < m_ptr[r + 1] && found[q] != 0;
             const unsigned ball = __ballot_sync(0xffffffffu, f);
             if (f) {
@@ -1275,19 +1277,24 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
     return GrB_SUCCESS;
 }
 
-GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
+template <typename OT>
+static GrB_Info masked_compact_t(const Csr &M, const OT *m_ptr, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
     const int64_t nrows = M.nrows;
-    GB_TRY(csr_from_row_counts(nrows, M.ncols, vsize, T, err,
+    return csr_from_row_counts(nrows, M.ncols, vsize, T, err,
         [&](int64_t *rowptr) {
             CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-            if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, found, nrows, rowptr); GB_LAUNCHED(); }
+            if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, found, nrows, rowptr); GB_LAUNCHED(); }
             return GrB_SUCCESS;
         },
         [&](Csr &t) {
-            row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(M.rowptr32, M.col, found, (const uint8_t *)tval, (int)vsize,
+            row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, M.col, found, (const uint8_t *)tval, (int)vsize,
                                                                               nrows, t.rowptr, t.col, (uint8_t *)t.val); GB_LAUNCHED();
             return GrB_SUCCESS;
-        }));
+        });
+}
+GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
+    GB_TRY(csr_wide(M) ? masked_compact_t<int64_t>(M, M.rowptr.get(), found, tval, vsize, T, err)
+                       : masked_compact_t<uint32_t>(M, M.rowptr32.get(), found, tval, vsize, T, err));
     G.last_nnz_out = (uint64_t)T.nnz;
     return GrB_SUCCESS;
 }
@@ -1434,7 +1441,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     if (!Mask && f.mask_comp) return matrix_writeback(C, nullptr, accum, f, Csr(), zt, false, err);   // C<!NULL>: no product needed
     if (A->dn.valid && B->dn.valid && Mask && !f.mask_comp && !Mask->dn.valid) {                   // two dense operands under a sparse mask
         GB_TRY(matrix_ensure_device(Mask));
-        if (Mask->dev.rowptr32) return sddmm_mxm(C, Mask, accum, semiring, A, B, f, burble);
+        return sddmm_mxm(C, Mask, accum, semiring, A, B, f, burble);
     }
     if (B->dn.valid && !f.tran1) return spmm_mxm(C, Mask, accum, semiring, A, B, f, burble);         // dense X: DESIGN.md section 3.6
     if (A->dn.valid && !B->dn.valid && op_mirror(mul) >= 0 && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))

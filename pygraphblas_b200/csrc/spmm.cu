@@ -153,8 +153,9 @@ GrB_Info csr_to_dense(const Csr &c, size_t vsize, DevBuf<void> &val, DevBuf<uint
 }
 
 // ------------------------------------------------------------------ the SpMM kernels
-struct SpmmArgs {
-    const uint32_t *rowptr, *col; const void *aval;     // op(A): m rows, values of the multiply's x type
+// OT: the type of the row offsets (uint32_t: rowptr32; int64_t: rowptr, the wide route of matrices with >= 2^32 entries)
+template <typename OT> struct SpmmArgsT {
+    const OT *rowptr; const uint32_t *col; const void *aval;   // op(A): m rows, values of the multiply's x type
     const void *xval; const uint8_t *xpres;             // X: n x k row-major, values of the multiply's y type
     int64_t m, k;
     int add, mul;
@@ -166,8 +167,8 @@ struct SpmmArgs {
     void *pval; uint8_t *ppres; // partials: nseg x k
 };
 
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(256, 2) spmm_kernel(const SpmmArgs p) {
+template <typename XT, typename ZT, int ADD, int MUL, typename OT>
+__global__ void __launch_bounds__(256, 2) spmm_kernel(const SpmmArgsT<OT> p) {
     const int add = ADD >= 0 ? ADD : p.add, mul = MUL >= 0 ? MUL : p.mul;
     const int64_t item = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> p.gshift;
     if (item >= p.nitems) return;                       // lanes fold independently: no warp-wide operation follows
@@ -218,8 +219,8 @@ __global__ void __launch_bounds__(256, 2) spmm_kernel(const SpmmArgs p) {
 
 // thread per (long row, column): the partials of the row's segments folded pairwise, in place, in a fixed tree over the
 // segment order (deterministic; the rounding error of a long FP row grows with the log of its segment count, not linearly)
-template <typename ZT>
-__global__ void __launch_bounds__(256) spmm_combine_kernel(const SpmmArgs p, int64_t nseg) {
+template <typename ZT, typename OT>
+__global__ void __launch_bounds__(256) spmm_combine_kernel(const SpmmArgsT<OT> p, int64_t nseg) {
     ZT *pv = (ZT *)p.pval;
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < nseg * p.k; t += (int64_t)gridDim.x * blockDim.x) {
         const int64_t q = t / p.k, j = t - q * p.k;
@@ -239,7 +240,7 @@ __global__ void __launch_bounds__(256) spmm_combine_kernel(const SpmmArgs p, int
     }
 }
 
-__global__ void spmm_seg_count_kernel(const uint32_t *rowptr, int64_t m, int64_t *cnt) {
+template <typename OT> __global__ void spmm_seg_count_kernel(const OT *rowptr, int64_t m, int64_t *cnt) {
     for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < m; r += (int64_t)gridDim.x * blockDim.x) {
         const int64_t len = (int64_t)rowptr[r + 1] - rowptr[r];
         cnt[r] = len > SPMM_SEG ? ceil_div(len, SPMM_SEG) : 0;
@@ -251,42 +252,43 @@ __global__ void spmm_seg_fill_kernel(const int64_t *segoff, int64_t m, uint32_t 
 }
 
 // the specialised semirings (the SpMV list, spmv_common.cuh) on x = z = T
-template <typename T> static bool spmm_launch_fast(int add, int mul, const SpmmArgs &p, dim3 grid) {
-#define GB_SPMM_FAST(A, M) if (add == A && mul == M) { spmm_kernel<T, T, A, M><<<grid, 256, 0, G.stream>>>(p); return true; }
+template <typename T, typename OT> static bool spmm_launch_fast(int add, int mul, const SpmmArgsT<OT> &p, dim3 grid) {
+#define GB_SPMM_FAST(A, M) if (add == A && mul == M) { spmm_kernel<T, T, A, M, OT><<<grid, 256, 0, G.stream>>>(p); return true; }
     GB_SPMV_FAST_PAIRS(T, GB_SPMM_FAST)
 #undef GB_SPMM_FAST
     return false;
 }
-static bool spmm_launch(int xt, int zt, const SpmmArgs &p, dim3 grid, bool *fast) {
+template <typename OT> static bool spmm_launch(int xt, int zt, const SpmmArgsT<OT> &p, dim3 grid, bool *fast) {
     *fast = false;
     if (xt == zt) switch (xt) {
-        case TC_FP32: *fast = spmm_launch_fast<float>(p.add, p.mul, p, grid); break;
-        case TC_FP64: *fast = spmm_launch_fast<double>(p.add, p.mul, p, grid); break;
-        case TC_INT32: *fast = spmm_launch_fast<int32_t>(p.add, p.mul, p, grid); break;
-        case TC_INT64: *fast = spmm_launch_fast<int64_t>(p.add, p.mul, p, grid); break;
-        case TC_UINT32: *fast = spmm_launch_fast<uint32_t>(p.add, p.mul, p, grid); break;
-        case TC_UINT64: *fast = spmm_launch_fast<uint64_t>(p.add, p.mul, p, grid); break;
-        case TC_BOOL: *fast = spmm_launch_fast<bool>(p.add, p.mul, p, grid); break;
+        case TC_FP32: *fast = spmm_launch_fast<float, OT>(p.add, p.mul, p, grid); break;
+        case TC_FP64: *fast = spmm_launch_fast<double, OT>(p.add, p.mul, p, grid); break;
+        case TC_INT32: *fast = spmm_launch_fast<int32_t, OT>(p.add, p.mul, p, grid); break;
+        case TC_INT64: *fast = spmm_launch_fast<int64_t, OT>(p.add, p.mul, p, grid); break;
+        case TC_UINT32: *fast = spmm_launch_fast<uint32_t, OT>(p.add, p.mul, p, grid); break;
+        case TC_UINT64: *fast = spmm_launch_fast<uint64_t, OT>(p.add, p.mul, p, grid); break;
+        case TC_BOOL: *fast = spmm_launch_fast<bool, OT>(p.add, p.mul, p, grid); break;
         default: break;
     }
     if (*fast) return true;
     bool matched = false;
-    GB_FOR_DOMAINS(xt, zt, matched, (spmm_kernel<XT_, ZT_, -1, -1><<<grid, 256, 0, G.stream>>>(p)));
+    GB_FOR_DOMAINS(xt, zt, matched, (spmm_kernel<XT_, ZT_, -1, -1, OT><<<grid, 256, 0, G.stream>>>(p)));
     return matched;
 }
-static bool spmm_combine(int zt, const SpmmArgs &p, int64_t nseg) {
+template <typename OT> static bool spmm_combine(int zt, const SpmmArgsT<OT> &p, int64_t nseg) {
     const int grid = grid_for(nseg * p.k);
     bool matched = false;
-    GB_FOR_DOMAINS(zt, zt, matched, (spmm_combine_kernel<ZT_><<<grid, 256, 0, G.stream>>>(p, nseg)));
+    GB_FOR_DOMAINS(zt, zt, matched, (spmm_combine_kernel<ZT_, OT><<<grid, 256, 0, G.stream>>>(p, nseg)));
     return matched;
 }
 
-// T (m x k, type zt, presence per entry) = a (+).(x) X
-static GrB_Info spmm_product(const Csr &a, const void *aval, const void *xval, const uint8_t *xpres, int64_t k, int xt, int zt, int add, int mul,
-                             void *tval, uint8_t *tpres, std::string *err) {
+// T (m x k, type zt, presence per entry) = a (+).(x) X, reading a's row offsets through rowptr (of type OT)
+template <typename OT>
+static GrB_Info spmm_product_t(const Csr &a, const OT *rowptr, const void *aval, const void *xval, const uint8_t *xpres, int64_t k, int xt,
+                               int zt, int add, int mul, void *tval, uint8_t *tpres, std::string *err) {
     const int64_t m = a.nrows;
-    SpmmArgs p{};
-    p.rowptr = a.rowptr32; p.col = a.col; p.aval = aval; p.xval = xval; p.xpres = xpres;
+    SpmmArgsT<OT> p{};
+    p.rowptr = rowptr; p.col = a.col; p.aval = aval; p.xval = xval; p.xpres = xpres;
     p.m = m; p.k = k; p.add = add; p.mul = mul;
     while ((1 << p.gshift) < k && p.gshift < 5) ++p.gshift;
     p.tval = tval; p.tpres = tpres;
@@ -294,7 +296,7 @@ static GrB_Info spmm_product(const Csr &a, const void *aval, const void *xval, c
     DevBuf<int64_t> segoff; DevBuf<uint32_t> segrow; DevBuf<void> pval; DevBuf<uint8_t> ppres;
     GB_TRY(segoff.alloc((size_t)m + 1, err));
     CU_TRY(cudaMemsetAsync(segoff.get() + m, 0, 8, G.stream), err);
-    spmm_seg_count_kernel<<<grid_for(m), 256, 0, G.stream>>>(a.rowptr32, m, segoff); GB_LAUNCHED();
+    spmm_seg_count_kernel<<<grid_for(m), 256, 0, G.stream>>>(rowptr, m, segoff); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(segoff, m + 1, err));
     int64_t nseg = 0; GB_TRY(read_i64(segoff.get() + m, &nseg, err));
     if (nseg > 0) {
@@ -312,12 +314,19 @@ static GrB_Info spmm_product(const Csr &a, const void *aval, const void *xval, c
         return gb_fail(GrB_DOMAIN_MISMATCH, err, "GrB_mxm: unsupported semiring domains (x=%d, z=%d)", xt, zt);
     GB_LAUNCHED();
     gb_kernel_used(fast ? "spmm-fast" : "spmm-generic");
+    if (sizeof(OT) == 8) gb_kernel_used("offsets=64");
     if (nseg > 0) {
         spmm_combine(zt, p, nseg); GB_LAUNCHED();
         gb_kernel_used("spmm-split");
     }
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
+}
+// the wide route (csr_wide: nnz >= 2^32, or B200_debug_wide) reads the 64-bit row offsets; the kernels are otherwise the same
+static GrB_Info spmm_product(const Csr &a, const void *aval, const void *xval, const uint8_t *xpres, int64_t k, int xt, int zt, int add, int mul,
+                             void *tval, uint8_t *tpres, std::string *err) {
+    return csr_wide(a) ? spmm_product_t<int64_t>(a, a.rowptr.get(), aval, xval, xpres, k, xt, zt, add, mul, tval, tpres, err)
+                       : spmm_product_t<uint32_t>(a, a.rowptr32.get(), aval, xval, xpres, k, xt, zt, add, mul, tval, tpres, err);
 }
 
 // C<Mask> = accum(C, T) for a dense T (m x k).  With no mask or a dense-form mask, C is viewed as a vector of m*k positions and
@@ -369,7 +378,6 @@ GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     gb_kernel_used("spmm");
     Csr *pa; GB_TRY(source_csr(A, f.tran0, &pa));
     const Csr &a = *pa;
-    if (!a.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
     const int64_t m = a.nrows, n = a.ncols, k = (int64_t)B->ncols;
     // operands cast to the multiply's input types, as in the CSR path
     DevBuf<void> a_cast, x_cast;
@@ -383,9 +391,10 @@ GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     if (m > 0 && k > 0) GB_TRY(spmm_product(a, aval, xval, B->dn.pres, k, xt, zt, add, mul, tval, tpres, err));
     a_cast.reset(); x_cast.reset();
     // algorithmic bytes: A (ids, values, row pointers), X once, T (values and presence)
-    const double bytes = (double)a.nnz * (4 + tc_size(A->type->code)) + (double)(m + 1) * 4 +
+    const bool wide = csr_wide(a);
+    const double bytes = (double)a.nnz * (4 + tc_size(A->type->code)) + (double)(m + 1) * (wide ? 8 : 4) +
                          (double)(n * k) * (tc_size(B->type->code) + (B->dn.pres ? 1 : 0)) + (double)(m * k) * (tc_size(zt) + 1);
-    burble.note("spmm", bytes);
+    burble.note(wide ? "spmm, 64-bit offsets" : "spmm", bytes);
     return spmm_writeback(C, Mask, accum, f, std::move(tval), std::move(tpres), zt, err);
 }
 
@@ -418,7 +427,6 @@ GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp a
     gb_kernel_used("spmm-left");
     if (f.tran1) GB_TRY(matrix_ensure_device(B)); else GB_TRY(matrix_ensure_transpose(B));
     const Csr &b = f.tran1 ? B->dev : B->devT;
-    if (!b.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
     const int64_t m = b.nrows, n = b.ncols, k = (int64_t)(f.tran0 ? A->ncols : A->nrows);
     // operands cast to the multiply's input types, as in the CSR path: op(B)' takes the swapped multiply's x, X its y
     DevBuf<void> b_cast, x_cast;
@@ -454,8 +462,9 @@ GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp a
     }
     // algorithmic bytes: the right route's (op(B)', X once, T), plus the transposes (each reads and writes its array)
     const double xb = (double)(n * k) * (tc_size(A->type->code) + (A->dn.pres ? 1 : 0)), tb = (double)(m * k) * (tc_size(zt) + 1);
-    const double bytes = (double)b.nnz * (4 + tc_size(B->type->code)) + (double)(m + 1) * 4 + xb + tb + (xtr ? 2 * xb : 0.0) +
+    const bool wide = csr_wide(b);
+    const double bytes = (double)b.nnz * (4 + tc_size(B->type->code)) + (double)(m + 1) * (wide ? 8 : 4) + xb + tb + (xtr ? 2 * xb : 0.0) +
                          (m > 1 ? 2 * tb : 0.0);
-    burble.note("spmm-left", bytes);
+    burble.note(wide ? "spmm-left, 64-bit offsets" : "spmm-left", bytes);
     return spmm_writeback(C, Mask, accum, f, std::move(tval), std::move(tpres), zt, err);
 }

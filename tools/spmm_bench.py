@@ -29,7 +29,14 @@ of fp64 numpy on 10^6 sampled edges plus the edges of the 16 longest mask rows. 
 which leaves out the gather, nnz(M) d b_Y (reported beside it); --sddmm --profile splits one call into row ids, kernel,
 transposes and write-back.
 
-    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile] [--left | --sddmm] [--ds 8,32,128]"""
+--wide measures the three routes on 64-bit row offsets (the wide route of matrices with 2^32 or more entries): (1) on the
+Kronecker graph A = kron(G, J) of 2^32 + 2^26 entries (n = 2^24), A (+).(x) X at k = 8 and 32, X (+).(x) A at k = 32 and SDDMM
+under A at d = 32, in FP32 when the card has the free memory for A and its transpose (8 B per entry each), else in UINT8 --
+time and algorithmic bytes over time, with (m + 1) 8 bytes of row offsets in the byte models; (2) the same three calls on the
+R-MAT graph at --scale, on the narrow and the forced-wide route (B200_debug_wide) alternated, outputs compared bit for bit:
+the cost of 64-bit offsets where both routes run.
+
+    python tools/spmm_bench.py [--scale 22] [--scale-csr 20] [--reps 10] [--warmup 2] [--profile] [--left | --sddmm | --wide] [--ds 8,32,128]"""
 import argparse
 import os
 import subprocess
@@ -41,7 +48,7 @@ import scipy.sparse as sp
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import pygraphblas_b200 as gb
-from pygraphblas_b200 import FP32, Matrix, Vector
+from pygraphblas_b200 import FP32, Matrix, Vector, descriptor
 from bench import cached_graph
 
 HBM_BPS = 3.35e12
@@ -440,9 +447,9 @@ def profile_sddmm(scale, d=32):
     fresh = lambda: Matrix.sparse(FP32, n, n)
     groups = {"row ids": ("sddmm_rowid",), "kernel": ("sddmm_kernel",), "transposes": ("dense_transpose",),
               "compaction": ("row_found", "scan", "Scan"), "write-back": ("mat_finalize", "cast_", "rowptr32")}
-    for name, f in (("desc=ST1, empty C", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.ST1, out=fresh())),
+    for name, f in (("desc=ST1, empty C", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=descriptor.ST1, out=fresh())),
                     ("desc=S, Y given d x n, empty C", lambda: X.mxm(Yt, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.S, out=fresh())),
-                    ("desc=ST1, C holds the last result", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=gb.descriptor.ST1, out=C))):
+                    ("desc=ST1, C holds the last result", lambda: X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=M, desc=descriptor.ST1, out=C))):
         f(); gb.lib.B200_device_synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             f(); gb.lib.B200_device_synchronize()
@@ -460,6 +467,102 @@ def profile_sddmm(scale, d=32):
         print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=8))
 
 
+def _bits_equal(a, b):
+    return all(np.array_equal(np.asarray(x).view(np.uint8), np.asarray(y).view(np.uint8)) for x, y in zip(a, b))
+
+
+def wide_kron(stream, reps, warmup):
+    """The three routes on kron(G, J), 2^32 + 2^26 entries: every call takes the wide route (no rowptr32)."""
+    from wide_spmv_bench import factor
+    NG = NJ = 4096
+    G, J = factor(1, NG, (1 << 16) + (1 << 10)), factor(2, NJ, 1 << 16)
+    nnz, n = G.nnz * J.nnz, NG * NJ
+    free = torch.cuda.mem_get_info()[0]
+    # FP32: A and A' at 8 B per entry, the partials of the split rows at k = 32 (~2.5 B per entry), the transpose's scratch and
+    # the dense blocks
+    fp32 = free > nnz * 18.5 + 8e9
+    typ, b = (FP32, 4) if fp32 else (gb.UINT8, 1)
+    sr = typ.PLUS_TIMES
+    print({"case": "wide-kron", "type": typ.name, "nnz": nnz, "n": n, "free_GB": round(free / 1e9, 1)}, flush=True)
+    mk = lambda S: Matrix.from_csr(S.indptr, S.indices, S.data.astype(typ.dtype), S.shape[0], S.shape[1], typ)
+    A, Gm, Jm = Matrix.sparse(typ, n, n), mk(G), mk(J)
+    gb.base._check(gb.lib.GrB_Matrix_kronecker_BinaryOp(A._matrix[0], gb.ffi.NULL, gb.ffi.NULL, typ.TIMES.get_op(),
+                                                        Gm._matrix[0], Jm._matrix[0], gb.ffi.NULL))
+    del Gm, Jm
+    rng = np.random.default_rng(5)
+    held = []
+
+    def report(name, ms, nbytes):
+        print({"case": name, "type": typ.name, "median_ms": round(ms, 2), "GEdge_per_s": round(nnz / ms / 1e6, 1),
+               "alg_GB_per_s": round(nbytes / ms / 1e6, 1), "kernels": last_kernel()}, flush=True)
+
+    for k in (8, 32):
+        X = Matrix.from_numpy(rng.integers(0, 4, (n, k)).astype(typ.dtype), typ=typ)
+        call = lambda: (held.clear(), held.append(A.mxm(X, semiring=sr)))
+        ms = alternate(stream, {"spmm": call}, reps, warmup)["spmm"]
+        report(f"wide-kron spmm k={k}", ms, nnz * (4 + b) + (n + 1) * 8 + n * k * b + n * k * (b + 1))
+        held.clear(); del X
+    d = 32
+    X = Matrix.from_numpy(rng.integers(0, 4, (n, d)).astype(typ.dtype), typ=typ)
+    Y = Matrix.from_numpy(rng.integers(0, 4, (n, d)).astype(typ.dtype), typ=typ)
+
+    def sddmm():
+        held.clear()                             # the previous T (as large as A) is freed before the next is formed
+        C = Matrix.sparse(typ, n, n)
+        X.mxm(Y, semiring=sr, mask=A, out=C, desc=descriptor.ST1)
+        held.append(C)
+    ms = alternate(stream, {"sddmm": sddmm}, reps, warmup)["sddmm"]
+    report(f"wide-kron sddmm d={d}", ms, nnz * 4 + (n + 1) * 8 + 2 * n * d * b + nnz * (4 + b) + (n + 1) * 8)
+    held.clear(); del X, Y
+    k = 32
+    X = Matrix.from_numpy(rng.integers(0, 4, (k, n)).astype(typ.dtype), typ=typ)
+    X.mxm(A, semiring=sr)                        # builds and caches A' (the chunked transpose), outside the timed calls
+    call = lambda: (held.clear(), held.append(X.mxm(A, semiring=sr)))
+    ms = alternate(stream, {"left": call}, reps, warmup)["left"]
+    xb, tb = n * k * b, n * k * (b + 1)
+    report(f"wide-kron left k={k}", ms, nnz * (4 + b) + (n + 1) * 8 + xb + tb + 2 * xb + 2 * tb)
+    held.clear()
+
+
+def wide_vs_narrow(stream, scale, reps, warmup):
+    """The three routes on the R-MAT graph, narrow and forced wide, alternated call by call; outputs compared bit for bit."""
+    n, indptr, indices, vals = graph(scale, quarter=False)
+    nnz = len(indices)
+    A = {w: Matrix.from_csr(indptr, indices, vals, n, n, FP32) for w in (False, True)}
+    k = d = 32
+    X = Matrix.from_numpy(xblock(n, k, False), typ=FP32)
+    Xl = Matrix.from_numpy(np.ascontiguousarray(xblock(n, k, False, seed=7).T), typ=FP32)
+    Y = Matrix.from_numpy(xblock(n, d, False, seed=9), typ=FP32)
+    out, kern = {}, {}
+
+    def arm(name, wide, f):
+        def g():
+            gb.lib.B200_debug_wide(1 << 30 if wide else 0)
+            try:
+                out[(name, wide)] = f(A[wide])
+            finally:
+                gb.lib.B200_debug_wide(0)
+            kern[(name, wide)] = last_kernel()
+        return g
+
+    def sddmm(a):
+        C = Matrix.sparse(FP32, n, n)
+        X.mxm(Y, semiring=FP32.PLUS_TIMES, mask=a, out=C, desc=descriptor.ST1)
+        return C
+    # (call, its result's arrays: the dense form's values and presence, or the CSR tuples)
+    calls = {"spmm k=32": (lambda a: a.mxm(X, semiring=FP32.PLUS_TIMES), Matrix.to_numpy),
+             "left k=32": (lambda a: Xl.mxm(a, semiring=FP32.PLUS_TIMES), Matrix.to_numpy),
+             "sddmm d=32": (sddmm, Matrix.to_arrays)}
+    for name, (f, arrays) in calls.items():
+        ms = alternate(stream, {w: arm(name, w, f) for w in (False, True)}, reps, warmup)
+        same = _bits_equal(arrays(out[(name, False)]), arrays(out[(name, True)]))
+        for w in (False, True):
+            print({"case": f"s{scale} {name} {'wide' if w else 'narrow'}", "nnz": nnz, "median_ms": round(ms[w], 4),
+                   "wide_over_narrow": round(ms[True] / ms[False], 4), "kernels": kern[(name, w)], "outputs_bit_identical": same},
+                  flush=True)
+        out.clear()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=int, default=22)
@@ -470,11 +573,19 @@ def main():
     ap.add_argument("--left", action="store_true", help="the dense left operand, X (+).(x) A (the batched vxm)")
     ap.add_argument("--sddmm", action="store_true", help="two dense operands under a sparse mask, C<M> = X (+).(x) Y'")
     ap.add_argument("--ds", default="8,32,128", help="--sddmm: the inner dimensions d")
+    ap.add_argument("--wide", action="store_true", help="the three routes on 64-bit row offsets: a graph of 2^32 + 2^26 entries, "
+                                                        "and the R-MAT graph narrow against forced wide")
+    ap.add_argument("--skip-large", action="store_true", help="--wide: only the narrow / forced-wide comparison")
     a = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     print({"card": card})
     stream = lib_stream()
+    if a.wide:
+        wide_vs_narrow(stream, a.scale, a.reps, a.warmup)
+        if not a.skip_large:
+            wide_kron(stream, max(3, a.reps // 3), 1)
+        return
     if a.sddmm:
         if a.profile:
             profile_sddmm(a.scale)

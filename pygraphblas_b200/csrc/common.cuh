@@ -106,6 +106,8 @@ struct RunPlan {
     DevBuf<uint32_t> base;           // [nruns+1] row starts before the run (= rank of its first row start)
     DevBuf<int32_t> tail_row;        // [nruns] row still open at the end of the run (its last row start), or -1
     DevBuf<uint32_t> tail_last;      // [nruns] last run that row reaches
+    DevBuf<uint32_t> long_run;       // [nlong] ascending: the runs whose open row reaches more than FIX_LONG runs further
+    int64_t nlong = 0;
     DevBuf<uint32_t> nzrow;          // [nnzrows] ids of the non-empty rows, ascending
     DevBuf<uint8_t> pres_tmpl;       // [nrows] 1 where the row is non-empty
     int64_t nruns = 0, nnzrows = 0;

@@ -427,7 +427,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         const RunPlan &rp = c.run;
         ra.col = c.col; ra.aval = aval; ra.uval = uval; ra.headw = rp.headw; ra.lane_rank = rp.lane; ra.run_base = rp.base;
         ra.nzrow = rp.nzrow; ra.rowptr = c.rowptr32; ra.nruns = rp.nruns; ra.nnz = c.nnz; ra.tval = tval;
-        ra.tail_row = rp.tail_row; ra.tail_last = rp.tail_last;
+        ra.tail_row = rp.tail_row; ra.tail_last = rp.tail_last; ra.long_run = rp.long_run; ra.nlong = rp.nlong;
         ra.add_op = add; ra.mul_op = kmul; ra.flip = kflip;
         ra.head_val = rp.ws_head; ra.tail_val = rp.ws_tail;            // scratch kept with the plan (the library serialises calls)
         if (sparse_u) { ra.upres = u->dpres; ra.tpres = tpres; ra.head_has = rp.ws_head_has; ra.tail_has = rp.ws_tail_has; }

@@ -13,7 +13,13 @@ struct RunArgs {
     int add_op, mul_op, flip;                                  // run-time operator codes (kernels instantiated with ADD = MUL = -1)
     const uint8_t *upres;                                      // SPARSE kernels: presence bytes of u ...
     uint8_t *tpres; uint8_t *head_has; uint8_t *tail_has;      // ... and of everything they produce
+    const uint32_t *long_run; int64_t nlong;                   // runs whose open row reaches more than FIX_LONG runs further
 };
+// the fix-up folds an open row with one thread when it reaches at most FIX_LONG runs past its tail run (a power of two: the
+// thread loads every partial at once and folds them by a tree), and with a whole warp, FIX_BATCH independent loads per lane
+// per trip, when it reaches further (the plan's long_run list)
+constexpr int FIX_LONG = 8;
+constexpr int FIX_BATCH = 8;
 
 // hot-table run kernel (spmv_run.cuh).  The host fills u_hot .. tpres and the two requests; spmv_run_launch lays out the
 // table tiers, runs the prep kernel and the hot-table kernel, and fills in the layout and the cluster size it used.

@@ -33,10 +33,11 @@ __global__ void plan_base_kernel(const int64_t *scan, int64_t nruns, uint32_t *r
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k <= nruns; k += (int64_t)gridDim.x * blockDim.x) run_base[k] = (uint32_t)scan[k];
 }
 // the row that starts last inside a run always holds the run's last entry: it is the run's "open" row
-// (possibly ending exactly at the run's end), completed by the fix-up kernel
+// (possibly ending exactly at the run's end), completed by the fix-up kernel.  is_long[k]: that row reaches more than
+// FIX_LONG runs past k (the fix-up gives it a warp)
 template <typename OT>
 __global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzrow, const OT *rowptr, int64_t nruns,
-                                  int32_t *tail_row, uint32_t *tail_last) {
+                                  int32_t *tail_row, uint32_t *tail_last, int64_t *is_long) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nruns; k += (int64_t)gridDim.x * blockDim.x) {
         int32_t tr = -1; uint32_t tl = 0;
         if (run_base[k + 1] > run_base[k]) {
@@ -45,7 +46,13 @@ __global__ void plan_tails_kernel(const uint32_t *run_base, const uint32_t *nzro
             tr = (int32_t)r; tl = (uint32_t)((re - 1) / RUN);
         }
         tail_row[k] = tr; tail_last[k] = tl;
+        is_long[k] = tr >= 0 && (int64_t)tl - k > FIX_LONG;
     }
+}
+// the long runs in ascending order, from the exclusive scan of is_long
+__global__ void plan_long_kernel(const int64_t *scan, int64_t nruns, uint32_t *long_run) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nruns; k += (int64_t)gridDim.x * blockDim.x)
+        if (scan[k + 1] > scan[k]) long_run[scan[k]] = (uint32_t)k;
 }
 
 template <typename OT> static GrB_Info spmv_run_plan_t(Csr &c, const OT *rowptr, std::string *err) {
@@ -76,7 +83,13 @@ template <typename OT> static GrB_Info spmv_run_plan_t(Csr &c, const OT *rowptr,
     plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, p.lane, cnt); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
     plan_base_kernel<<<grid_for(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
-    plan_tails_kernel<OT><<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, rowptr, p.nruns, p.tail_row, p.tail_last); GB_LAUNCHED();
+    plan_tails_kernel<OT><<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, rowptr, p.nruns, p.tail_row, p.tail_last, cnt); GB_LAUNCHED();
+    CU_TRY(cudaMemsetAsync(cnt + p.nruns, 0, 8, G.stream), err);
+    GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
+    CU_TRY(cudaMemcpyAsync(&p.nlong, cnt + p.nruns, 8, cudaMemcpyDeviceToHost, G.stream), err);
+    CU_TRY(cudaStreamSynchronize(G.stream), err);
+    GB_TRY(p.long_run.alloc((size_t)p.nlong + 1, err));
+    plan_long_kernel<<<grid_for(p.nruns), 256, 0, G.stream>>>(cnt, p.nruns, p.long_run); GB_LAUNCHED();
     flag.reset(); cnt.reset();
     // per-call scratch lives with the plan: partials of the rows that straddle runs (8 bytes covers every type)
     GB_TRY(p.ws_head.alloc((size_t)p.nruns * 8 + 16, err));
@@ -173,6 +186,7 @@ GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
 __global__ void __launch_bounds__(256) spmv_hot2_prep_kernel(const uint32_t *hperm, const uint8_t *u, uint8_t *u_hot, int vsize, uint32_t henc,
                                                             uint32_t t0, uint32_t t1, uint32_t slice, int lc,
                                                             uint4 *tval16, int64_t tval_n16, const uint4 *tmpl16, uint4 *tpres16, int64_t pres_n16) {
+    pdl_launch_dependents();                              // the hot-table kernel waits for this grid before it reads u_hot or writes T
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
     const uint32_t past = (slice << lc) - t1;             // slots of the slices that hold no rank
     for (int64_t i = tid; i < henc; i += nth) {

@@ -193,6 +193,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
                  "@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
+// programmatic dependent launch: a grid launched with cudaLaunchAttributeProgrammaticStreamSerialization may start once every
+// CTA of the grid before it has passed pdl_launch_dependents (or exited); pdl_wait then blocks until that grid has completed
+// and its memory operations are visible.  Without the attribute pdl_wait returns at once.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
@@ -240,6 +246,9 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
     if (threadIdx.x == 0) mbar_init(s_bar + HOT2_WARPS, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
+    if (lane == 0 && run < p.nruns) issue(run);   // A's encoded columns and values: the prep kernel does not write them
+    pdl_wait();                               // the prep kernel is done: u_hot is filled and T cleared
+    pdl_launch_dependents();                  // the fix-up may launch; it waits for this grid before it reads a partial
     const uint32_t tab_n = t0 + slice;
     if (threadIdx.x == 0 && tab_n) {          // the table: the replicated tier and this CTA's slice, bulk copies of <= 16 KB
         const unsigned char *src = static_cast<const unsigned char *>(h.u_hot);
@@ -250,7 +259,6 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         src += rb + (size_t)cluster_ctarank() * sb; dst += rb;
         for (uint32_t off = 0; off < sb; off += 16384u) tma_bulk_g2s(dst + off, src + off, min(16384u, sb - off), s_bar + HOT2_WARPS);
     }
-    if (lane == 0 && run < p.nruns) issue(run);
     if (tab_n) mbar_wait(s_bar + HOT2_WARPS, 0);
     cluster_sync_all();                       // every table of the cluster is in
 
@@ -313,30 +321,73 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
     cluster_sync_all();                       // no peer reads this CTA's table any more
 }
 
-// rows that continue past their run: tail partial (+) head partials of the following runs, 8 lanes per open row.
-// Every run after `run` up to tail_last starts inside that row, so its head partial exists.
+// rows that continue past their run: tail partial (+) head partials of the following runs.  Every run after `run` up to
+// tail_last starts inside that row, so its head partial exists.  The first ceil(nlong / 8) CTAs give each row of the plan's
+// long_run list a warp; the others take one thread per run and skip those rows.  The order of every fold depends on the plan
+// alone (deterministic).
 template <typename ZT, int ADD_C, bool SPARSE>
 __global__ void __launch_bounds__(256) spmv_run_fixup_kernel(const RunArgs p) {
     const int ADD = ADD_C >= 0 ? ADD_C : p.add_op;
-    const int sub = threadIdx.x & 7;
-    const int64_t run = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
-    const int32_t r = run < p.nruns ? __ldg(p.tail_row + run) : -1;
+    const ZT *head_val = static_cast<const ZT *>(p.head_val), *tail_val = static_cast<const ZT *>(p.tail_val);
+    const int64_t long_ctas = (p.nlong + 7) >> 3;
     Part<ZT> acc{(ZT)0, 0};
-    if (r >= 0) {
+    if ((int64_t)blockIdx.x < long_ctas) {
+        // a long row: lane l folds the head partials run + 1 + l + 32 k in order of k, FIX_BATCH loads in flight per trip, lane 0
+        // starting with the tail partial; then a fixed xor tree over the warp
+        const int64_t w = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+        if (w >= p.nlong) return;                                       // whole warps
+        const int lane = threadIdx.x & 31;
+        const int64_t run = __ldg(p.long_run + w);
+        const int32_t r = __ldg(p.tail_row + run);
         const int64_t last_run = __ldg(p.tail_last + run);
-        if (sub == 0) { acc.v = static_cast<const ZT *>(p.tail_val)[run]; acc.has = SPARSE ? (int)p.tail_has[run] : 1; }
-        for (int64_t t = run + 1 + sub; t <= last_run; t += 8) {
-            const Part<ZT> y{static_cast<const ZT *>(p.head_val)[t], SPARSE ? (int)p.head_has[t] : 1};
+        pdl_wait();
+        if (lane == 0) { acc.v = tail_val[run]; acc.has = SPARSE ? (int)p.tail_has[run] : 1; }
+        for (int64_t t0 = run + 1 + lane; t0 <= last_run; t0 += 32 * FIX_BATCH) {
+            Part<ZT> y[FIX_BATCH];
+#pragma unroll
+            for (int j = 0; j < FIX_BATCH; ++j) {
+                const int64_t t = t0 + 32 * j;
+                y[j].v = t <= last_run ? head_val[t] : (ZT)0;
+                y[j].has = t <= last_run ? (SPARSE ? (int)p.head_has[t] : 1) : 0;
+            }
+#pragma unroll
+            for (int j = 0; j < FIX_BATCH; ++j) acc = part_join<ZT>(ADD, acc, y[j]);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            Part<ZT> y; y.v = shfl_xor_t<ZT>(acc.v, o); y.has = __shfl_xor_sync(0xffffffffu, acc.has, o);
             acc = part_join<ZT>(ADD, acc, y);
         }
+        if (lane == 0) { static_cast<ZT *>(p.tval)[r] = acc.v; if (SPARSE) p.tpres[r] = (uint8_t)acc.has; }
+        return;
     }
+    // every other open row: one thread, all of its <= 1 + FIX_LONG partials loaded at once, folded by a fixed tree: the tail
+    // partial and head partial s (of run + 1 + s) as x0 = tail (+) h0, xs = hs; then (x0 + x4, x1 + x5, x2 + x6, x3 + x7),
+    // pairs of those, the last pair
+    const int64_t run = ((int64_t)blockIdx.x - long_ctas) * blockDim.x + threadIdx.x;
+    if (run >= p.nruns) return;
+    int32_t r = __ldg(p.tail_row + run);
+    const int64_t last_run = r >= 0 ? (int64_t)__ldg(p.tail_last + run) : 0;
+    if (last_run - run > FIX_LONG) r = -1;                              // a long row: its warp completes it
+    pdl_wait();
+    if (r < 0) return;
+    Part<ZT> x[FIX_LONG];
 #pragma unroll
-    for (int o = 4; o > 0; o >>= 1) {
-        Part<ZT> y; y.v = shfl_xor_t<ZT>(acc.v, o); y.has = __shfl_xor_sync(0xffffffffu, acc.has, o);
-        acc = part_join<ZT>(ADD, acc, y);
+    for (int s = 0; s < FIX_LONG; ++s) {
+        const int64_t t = run + 1 + s;
+        x[s].v = t <= last_run ? head_val[t] : (ZT)0;
+        x[s].has = t <= last_run ? (SPARSE ? (int)p.head_has[t] : 1) : 0;
     }
-    if (r >= 0 && sub == 0) { static_cast<ZT *>(p.tval)[r] = acc.v; if (SPARSE) p.tpres[r] = (uint8_t)acc.has; }
+    acc.v = tail_val[run]; acc.has = SPARSE ? (int)p.tail_has[run] : 1;
+    x[0] = part_join<ZT>(ADD, acc, x[0]);
+#pragma unroll
+    for (int o = FIX_LONG / 2; o > 0; o >>= 1) {
+#pragma unroll
+        for (int s = 0; s < o; ++s) x[s] = part_join<ZT>(ADD, x[s], x[s + o]);
+    }
+    static_cast<ZT *>(p.tval)[r] = x[0].v; if (SPARSE) p.tpres[r] = (uint8_t)x[0].has;
 }
+static inline unsigned fixup_ctas(const RunArgs &a) { return (unsigned)((a.nlong + 7) / 8 + ceil_div(a.nruns, 256)); }
 
 // shared memory the hot-table kernel can use for its table, after the warp stages and barriers
 template <typename XT> static inline uint32_t hot2_table_entries(bool need_a, uint32_t henc, size_t limit_bytes) {
@@ -405,8 +456,9 @@ static void hot2_launch(const RunArgs &a, Hot2Args &h, size_t table_limit) {
     spmv_hot2_prep(h);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)ctas); cfg.blockDim = dim3(HOT2_WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = G.stream;
-    cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {(unsigned)C, 1, 1};
-    cfg.attrs = at; cfg.numAttrs = 1;
+    cudaLaunchAttribute at[2]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {(unsigned)C, 1, 1};
+    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 2;
     cudaLaunchKernelEx(&cfg, kernel, a, (const Hot2Args)h); GB_LAUNCHED();
 }
 
@@ -414,18 +466,25 @@ template <typename XT, typename ZT, int ADD, int MUL>
 static void spmv_run_launch(const RunArgs &a, Hot2Args *hot, size_t table_limit) {
     if constexpr (ADD >= 0) {
         if (hot && !a.upres) {
+            // prep -> hot-table kernel -> fix-up as programmatic dependent launches: each grid starts its prologue (plan
+            // loads, the first stage copy) while the one before it drains
             hot2_launch<XT, ZT, ADD, MUL>(a, *hot, table_limit);
-            spmv_run_fixup_kernel<ZT, ADD, false><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+            cudaLaunchConfig_t cfg{};
+            cfg.gridDim = dim3(fixup_ctas(a)); cfg.blockDim = dim3(256); cfg.stream = G.stream;
+            cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+            at[0].val.programmaticStreamSerializationAllowed = 1;
+            cfg.attrs = at; cfg.numAttrs = 1;
+            cudaLaunchKernelEx(&cfg, spmv_run_fixup_kernel<ZT, ADD, false>, a); GB_LAUNCHED();
             return;
         }
     }
     if (a.upres) {
         spmv_run_kernel<XT, ZT, ADD, MUL, true><<<(unsigned)ceil_div(a.nruns, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-        spmv_run_fixup_kernel<ZT, ADD, true><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+        spmv_run_fixup_kernel<ZT, ADD, true><<<fixup_ctas(a), 256, 0, G.stream>>>(a); GB_LAUNCHED();
         return;
     }
     spmv_run_kernel<XT, ZT, ADD, MUL, false><<<(unsigned)ceil_div(a.nruns, 8), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    spmv_run_fixup_kernel<ZT, ADD, false><<<(unsigned)ceil_div(a.nruns * 8, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
+    spmv_run_fixup_kernel<ZT, ADD, false><<<fixup_ctas(a), 256, 0, G.stream>>>(a); GB_LAUNCHED();
 }
 
 // the run kernels of the specialised semiring (add, mul) on T (spmv_common.cuh); false when it is not one

@@ -239,7 +239,7 @@ int64_t B200_debug_live_allocs(void);
  * chunks of `chunk` entries), whatever the matrix's size; 0 switches it off.  The 32-bit row offsets stay built for the other
  * operations */
 void B200_debug_wide(int64_t chunk);
-/* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("tile (specialised, 8 items)",
+/* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("run",
  * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "spa-split", "masked-warp", "stream-L",
  * "dot", ...); recorded whether the burble is on or not, valid until the next such call.  Host-decided variants follow
  * their entry as "key=value" tokens: "filter=exact" or "filter=bloom" after each "stream-S" / "stream-M" / "stream-L"

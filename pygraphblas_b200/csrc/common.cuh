@@ -94,11 +94,6 @@ public:
     void adopt(T *p) { reset(); p_ = p; }     // takes a dmalloc block handed over as a raw pointer (vector_write's result)
 };
 
-// SpMV tile plan (spmv.cu): first row of every TILE-sized slice of the nnz range
-struct TilePlan {
-    DevBuf<uint32_t> row;            // [ntiles+1]
-    int64_t ntiles = 0;
-};
 // run plan (spmv_run.cu, warp-independent kernels): entries cut into warp-sized runs of 256
 struct RunPlan {
     DevBuf<uint32_t> headw;          // [ceil(nnz/32)] bit q = entry q starts a row
@@ -134,7 +129,6 @@ struct CsrFields {
     DevBuf<uint32_t> col;            // [nnz]
     DevBuf<void> val;                // [nnz] of the matrix type
     // cached SpMV plans, each either complete or absent
-    TilePlan tile;
     RunPlan run;
     HotPlan hot;
     bool valid = false;
@@ -147,7 +141,7 @@ struct Csr : CsrFields {
     Csr &operator=(Csr &&o) noexcept { if (this != &o) { CsrFields::operator=(std::move(o)); o.clear(); } return *this; }
     void clear() { static_cast<CsrFields &>(*this) = CsrFields(); }
     // the cached SpMV plans and scratch (dropped whenever the structure changes)
-    void drop_plans() { tile = TilePlan(); run = RunPlan(); hot = HotPlan(); }
+    void drop_plans() { run = RunPlan(); hot = HotPlan(); }
 };
 
 // per-object storage hints of SuiteSparse's GxB_*_Option_set/get: recorded and reported back, without effect on the HBM
@@ -240,7 +234,6 @@ static inline void gb_thread_enter() {
 // kernel-choice switches read from the environment ONCE (GrB_init) and again only on B200_reload_tunables()
 // (tests flip them between calls); nothing on a call path touches getenv
 struct Tunables {
-    int spmv_run = -1;         // B200GRB_SPMV_RUN     -1 default choice, 0 never, 1 always the run kernel
     int spmv_hot_kb = -1;      // B200GRB_SPMV_HOT     -1 default (on when the gathers are concentrated), 0 off, >0 table cap in KB
     bool no_pull = false, no_push = false, force_push = false;
     int spmv_cluster = 2;      // B200GRB_SPMV_CLUSTER thread-block cluster size of the hot-table kernel (1 / 2 / 4 / 8 / 16)

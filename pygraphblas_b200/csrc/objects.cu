@@ -36,7 +36,6 @@ static Tunables g_tun; static bool g_tun_loaded = false;
 static void tunables_load() {
     Tunables t;
     auto geti = [](const char *k, int d) { const char *e = getenv(k); return e ? atoi(e) : d; };
-    t.spmv_run = geti("B200GRB_SPMV_RUN", -1);
     t.spmv_hot_kb = geti("B200GRB_SPMV_HOT", -1);
     t.no_pull = getenv("B200GRB_NO_PULL") != nullptr; t.no_push = getenv("B200GRB_NO_PUSH") != nullptr;
     t.force_push = getenv("B200GRB_FORCE_PUSH") != nullptr;

@@ -7,295 +7,22 @@
 // the matrix type), vectors are dense value arrays + one presence byte per position
 // (no presence array at all when every position is present).
 //
-// This file: the host logic of both calls (operand casts, kernel choice, write-back) and the tile kernel.
+// This file: the host logic of both calls (operand casts, kernel choice, write-back).
 // Kernel choice, in order (DESIGN.md section 3.1):
 //   mask + LOR/LAND/ANY monoid  -> masked push (small frontier, spmv_pull.cu) or masked pull with early exit
-//   nnz >= 4096                 -> run kernel (spmv_run*.cu): 256-entry runs per warp on a cached run plan,
+//   nnz == 0                    -> no kernel but clearing T's presence
+//   otherwise                   -> run kernel (spmv_run*.cu): 256-entry runs per warp on a cached run plan,
 //                                  compile-time semirings (+ shared-memory hot-column table), run-time
-//                                  operator codes, dense or sparse u
-//   otherwise                   -> tile kernel below: the nnz range is cut into tiles of SPMV_TILE = 2048
-//                                  entries, one CTA per tile, item-centric segmented reduction; rows that straddle
-//                                  tiles leave head / tail partials that a fix-up kernel combines in a fixed order.
+//                                  operator codes, dense or sparse u; rows that straddle runs are
+//                                  combined by a fix-up kernel in a fixed order
 // Every path is nnz-split (R-MAT hub rows cannot serialise a warp) and deterministic for a given matrix.
 //
 // Algorithmic bytes per call (DESIGN.md): nnz*(4 + sizeof(a)) + (nrows+1)*4
 //   + ncols*sizeof(u) + nrows*(sizeof(t) + 1).
 #include "spmv_args.cuh"
 
-static constexpr int SPMV_THREADS = 256;
-static constexpr int SPMV_WARPS = SPMV_THREADS / 32;
-static constexpr int SPMV_PER_THREAD = 8;                         // entries per thread of the tile kernel
-static constexpr int SPMV_TILE = SPMV_THREADS * SPMV_PER_THREAD;
-
-struct SpmvArgs {
-    const uint32_t *rowptr; const uint32_t *col; const void *aval;
-    const uint32_t *tile_row; int64_t ntiles; int64_t nrows; int64_t nnz;
-    const void *uval; const uint8_t *upres;
-    void *tval; uint8_t *tpres;
-    void *head_val; uint8_t *head_has; void *tail_val; uint8_t *tail_has; int32_t *tail_row;
-    int add_op, mul_op;
-    int flip;      // 0: z = mul(a, u) (mxv)   1: z = mul(u, a) (vxm)   (run-time-operator kernels only)
-    int tile;      // entries per tile (SPMV_TILE)
-};
-
-// ---- plan: tile_row[t] = row holding entry t*tile (tile_row[0] = 0, tile_row[ntiles] = nrows)
-__global__ void spmv_plan_kernel(const uint32_t *rowptr, int64_t nrows, int64_t ntiles, int tile, uint32_t *tile_row) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t > ntiles) return;
-    if (t == 0) { tile_row[0] = 0; return; }
-    if (t == ntiles) { tile_row[t] = (uint32_t)nrows; return; }
-    const uint32_t x = (uint32_t)(t * tile);
-    int64_t lo = 0, hi = nrows;           // first r in [0, nrows] with rowptr[r] > x
-    while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (rowptr[mid] > x) hi = mid; else lo = mid + 1; }
-    tile_row[t] = (uint32_t)(lo - 1);
-}
-
-static GrB_Info spmv_plan(Csr &c, std::string *err) {
-    if (c.tile.row) return GrB_SUCCESS;
-    if (!c.rowptr32) return gb_fail(GrB_INVALID_VALUE, err, "mxv: matrices with >= 2^32 entries are not supported");
-    TilePlan p;
-    p.ntiles = ceil_div(c.nnz, SPMV_TILE);
-    GB_TRY(p.row.alloc((size_t)p.ntiles + 1, err));
-    const int64_t n = p.ntiles + 1;
-    spmv_plan_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, G.stream>>>(c.rowptr32, c.nrows, p.ntiles, SPMV_TILE, p.row); GB_LAUNCHED();
-    CU_TRY(cudaGetLastError(), err);
-    c.tile = std::move(p);
-    return GrB_SUCCESS;
-}
-
-
-// One tile of SPMV_THREADS * IT consecutive entries per CTA:
-//
-//   1. every thread streams its IT consecutive entries (128-bit loads), issues all its gathers of u
-//      back to back and keeps the products in registers;
-//   2. the rows of the tile are walked thread-per-row (coalesced rowptr reads): empty rows are
-//      written out as "no entry", the others mark their first entry in shared memory;
-//   3. item-centric segmented reduction: each thread folds its items between row marks (rows that
-//      begin and end inside a thread are final), then a segmented suffix scan over the threads
-//      (shuffles inside a warp, 8 aggregates across warps) completes the rows that span threads.
-//      Work per thread is constant whatever the row lengths: hub rows and runs of short rows cost
-//      the same;
-//   4. what sticks out of the tile goes to the per-tile head / tail slots for the fix-up kernel.
-//
-// ADD/MUL >= 0: compile-time semiring (flip already folded into MUL by the host); -1: run-time codes.
-// SPARSE: u has a presence array (entries with absent u(k) do not contribute).
-// Everything after the column / value words of a tile are in registers: gather u, mark rows, fold,
-// scan, write.  `sync` is the barrier of the 256 threads that share s_head / s_wv / s_wflag.
-template <typename XT, typename ZT, int ADD, int MUL, bool SPARSE, int IT, typename Sync>
-__device__ __forceinline__ void spmv_tile_finish(const SpmvArgs &p, const uint32_t tile, const int tid, const int tlen, const int nvalid,
-                                                 uint32_t (&c)[IT], XT (&a)[IT], int32_t *s_head, ZT *s_wv, int *s_wflag, Sync &&sync) {
-    constexpr int TILE = SPMV_THREADS * IT;
-    constexpr bool NEED_A = MUL < 0 || mul_reads_x(MUL);
-    constexpr bool NEED_U = MUL < 0 || mul_reads_y(MUL);
-    const int add = ADD >= 0 ? ADD : p.add_op;
-    const int mul = MUL >= 0 ? MUL : p.mul_op;
-    const int lane = tid & 31, warp = tid >> 5;
-    const int loc0 = tid * IT;
-    const int64_t tstart = (int64_t)tile * TILE;
-    const XT *uval = static_cast<const XT *>(p.uval);
-    ZT *tval = static_cast<ZT *>(p.tval);
-
-    const uint32_t r0 = p.tile_row[tile];
-    const uint32_t r1 = (uint32_t)min((int64_t)p.tile_row[tile + 1], p.nrows - 1);
-    uint32_t pre_rs = 0, pre_re = 0;                                      // row pointers of this thread's first row
-    if (r0 + tid <= r1) { pre_rs = p.rowptr[r0 + tid]; pre_re = p.rowptr[r0 + tid + 1]; }
-#pragma unroll
-    for (int j = 0; j < IT; j += 4) *reinterpret_cast<int4 *>(&s_head[loc0 + j]) = make_int4(-1, -1, -1, -1);
-    if (tid == 0) { p.tail_row[tile] = -1; p.head_has[tile] = 0; p.tail_has[tile] = 0; }
-    uint8_t hs[SPARSE ? IT : 1]; XT uv[IT];
-    if (SPARSE) {
-#pragma unroll
-        for (int j = 0; j < IT; ++j) hs[j] = __ldg(p.upres + c[j]);
-    }
-    if (NEED_U) {
-#pragma unroll
-        for (int j = 0; j < IT; ++j) {
-            uv[j] = gload<XT>(uval + c[j]);
-        }
-    }
-    sync();                                                               // head marks are clear
-
-    // ---- (2) rows of the tile: empty ones are final, the others mark their first entry
-    {
-        const uint32_t ts32 = (uint32_t)tstart;                           // nnz < 2^32
-        uint32_t rs = pre_rs, re = pre_re;
-        for (uint32_t r = r0 + tid; r <= r1; r += SPMV_THREADS) {
-            if (r != r0 + tid) { rs = p.rowptr[r]; re = p.rowptr[r + 1]; }
-            if (rs == re) { p.tpres[r] = 0; tval[r] = (ZT)0; }
-            else if (rs >= ts32 && rs - ts32 < (uint32_t)tlen) s_head[rs - ts32] = (int32_t)(r - r0);
-        }
-    }
-    ZT prod[IT];
-#pragma unroll
-    for (int j = 0; j < IT; ++j) {
-        const XT av = NEED_A ? a[j] : (XT)1;
-        const XT uu = NEED_U ? uv[j] : (XT)1;
-        if (MUL >= 0) prod[j] = MulApply<XT, ZT>::f(mul, av, uu);
-        else prod[j] = p.flip ? MulApply<XT, ZT>::f(mul, uu, av) : MulApply<XT, ZT>::f(mul, av, uu);
-    }
-    sync();                                                               // head marks are complete
-
-    // ---- (3a) fold this thread's items between row marks
-    int32_t h[IT];
-#pragma unroll
-    for (int j = 0; j < IT; j += 4) {
-        const int4 t4 = *reinterpret_cast<const int4 *>(&s_head[loc0 + j]);
-        h[j] = t4.x; h[j + 1] = t4.y; h[j + 2] = t4.z; h[j + 3] = t4.w;
-    }
-    Part<ZT> acc{(ZT)0, 0}, lead{(ZT)0, 0};
-    bool seen = false; int32_t cur = -1;
-    if (!SPARSE && nvalid == IT) {
-        // every item contributes: presence is structural, no per-item flags
-#pragma unroll
-        for (int j = 0; j < IT; ++j) {
-            if (h[j] >= 0) {
-                if (!seen) lead = acc;
-                else { tval[r0 + cur] = acc.v; p.tpres[r0 + cur] = 1; }      // row began and ended in this thread
-                seen = true; cur = h[j]; acc.v = prod[j]; acc.has = 1;
-            } else if (j == 0) { acc.v = prod[0]; acc.has = 1; }
-            else acc.v = MulApply<ZT, ZT>::f(add, acc.v, prod[j]);
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < IT; ++j) {
-            if (h[j] >= 0) {
-                if (!seen) lead = acc;
-                else { tval[r0 + cur] = acc.v; p.tpres[r0 + cur] = (uint8_t)acc.has; }
-                seen = true; cur = h[j]; acc.has = 0;
-            }
-            const Part<ZT> it{prod[j], (j < nvalid && (!SPARSE || hs[SPARSE ? j : 0])) ? 1 : 0};
-            acc = part_join<ZT>(add, acc, it);
-        }
-    }
-    if (!seen) { lead = acc; acc.has = 0; }                               // no mark: everything continues an earlier row
-
-    // ---- (3b) segmented suffix scan of the leads: X_t = lead_t (+) (stop_t ? nothing : X_{t+1}); stop = thread has a mark
-    Part<ZT> x = lead; int stop = seen ? 1 : 0;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        Part<ZT> y; y.v = shfl_down_t<ZT>(x.v, d); y.has = __shfl_down_sync(0xffffffffu, x.has, d);
-        const int ystop = __shfl_down_sync(0xffffffffu, stop, d);
-        if (lane + d < 32) { if (!stop) x = part_join<ZT>(add, x, y); stop |= ystop; }
-    }
-    if (lane == 0) { s_wv[warp] = x.v; s_wflag[warp] = x.has | (stop << 1); }
-    sync();
-    Part<ZT> carry{(ZT)0, 0}; int carry_stop = 0;                         // what the following warps add to a row open at this warp's end
-    for (int w = SPMV_WARPS - 1; w > warp; --w) {
-        Part<ZT> y; y.v = s_wv[w]; const int f = s_wflag[w]; y.has = f & 1;
-        if (f >> 1) { carry = y; carry_stop = 1; } else carry = part_join<ZT>(add, y, carry);
-    }
-    if (!stop) { x = part_join<ZT>(add, x, carry); stop |= carry_stop; }
-    Part<ZT> nxt; nxt.v = shfl_down_t<ZT>(x.v, 1); nxt.has = __shfl_down_sync(0xffffffffu, x.has, 1);   // S_t = X_{t+1}
-    int nxt_stop = __shfl_down_sync(0xffffffffu, stop, 1);
-    if (lane == 31) { nxt = carry; nxt_stop = carry_stop; }
-
-    // ---- (4) rows still open at the end of a thread, and what sticks out of the tile
-    if (seen) {
-        const Part<ZT> total = part_join<ZT>(add, acc, nxt);
-        if (nxt_stop) { tval[r0 + cur] = total.v; p.tpres[r0 + cur] = (uint8_t)total.has; }
-        else { static_cast<ZT *>(p.tail_val)[tile] = total.v; p.tail_has[tile] = (uint8_t)total.has; p.tail_row[tile] = (int32_t)(r0 + cur); }
-    }
-    if (tid == 0 && h[0] < 0) {                                           // the tile starts inside a row of an earlier tile
-        static_cast<ZT *>(p.head_val)[tile] = x.v; p.head_has[tile] = (uint8_t)x.has;
-    }
-}
-
-// General path: one CTA per tile, loads straight from global memory into registers.
-template <typename XT, typename ZT, int ADD, int MUL, bool SPARSE, int IT>
-__global__ void __launch_bounds__(SPMV_THREADS) spmv_tile_kernel(const SpmvArgs p) {
-    constexpr int TILE = SPMV_THREADS * IT;
-    constexpr bool NEED_A = MUL < 0 || mul_reads_x(MUL);
-    __shared__ __align__(16) int32_t s_head[TILE];     // row (relative to the tile's first row) starting at this entry, or -1
-    __shared__ ZT s_wv[SPMV_WARPS];
-    __shared__ int s_wflag[SPMV_WARPS];
-    const int tid = threadIdx.x;
-    const uint32_t tile = blockIdx.x;
-    const int64_t tstart = (int64_t)tile * TILE;
-    const int tlen = (int)min((int64_t)TILE, p.nnz - tstart);            // valid entries in this tile
-    const int loc0 = tid * IT;
-    const int nvalid = min(max(tlen - loc0, 0), IT);                     // valid entries of this thread
-    const uint32_t *colp = p.col + tstart + loc0;
-    const XT *avalp = static_cast<const XT *>(p.aval) + tstart + loc0;
-    uint32_t c[IT]; XT a[IT];
-    if (nvalid == IT) {
-#pragma unroll
-        for (int g = 0; g < IT / 4; ++g) {
-            load4<uint32_t>(colp + g * 4, &c[g * 4]);
-            if (NEED_A) load4<XT>(avalp + g * 4, &a[g * 4]);
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < IT; ++j) {
-            c[j] = j < nvalid ? colp[j] : 0u;                            // 0 is always a valid column to gather
-            if (NEED_A) a[j] = j < nvalid ? avalp[j] : (XT)1;
-        }
-    }
-    spmv_tile_finish<XT, ZT, ADD, MUL, SPARSE, IT>(p, tile, tid, tlen, nvalid, c, a, s_head, s_wv, s_wflag, [] { __syncthreads(); });
-}
-
-// ---- fix-up: rows that straddle tiles = tail partial of the tile they start in
-//      (+) head partials of the following tiles, combined by one warp in a fixed order
-template <typename ZT, int ADD>
-__global__ void __launch_bounds__(256) spmv_fixup_kernel(const SpmvArgs p) {
-    const int add = ADD >= 0 ? ADD : p.add_op;
-    const int lane = threadIdx.x & 31;
-    const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (t >= p.ntiles) return;
-    const int32_t r = p.tail_row[t];
-    if (r < 0) return;
-    const int64_t re = p.rowptr[r + 1];
-    const int64_t last_tile = (re - 1) / p.tile;
-    Part<ZT> acc{(ZT)0, 0};
-    if (lane == 0 && p.tail_has[t]) { acc.v = static_cast<const ZT *>(p.tail_val)[t]; acc.has = 1; }
-    for (int64_t tt = t + 1 + lane; tt <= last_tile; tt += 32) if (p.head_has[tt]) {
-        const Part<ZT> y{static_cast<const ZT *>(p.head_val)[tt], 1};
-        acc = part_join<ZT>(add, acc, y);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        Part<ZT> y; y.v = shfl_xor_t<ZT>(acc.v, o); y.has = __shfl_xor_sync(0xffffffffu, acc.has, o);
-        acc = part_join<ZT>(add, acc, y);
-    }
-    if (lane == 0) { static_cast<ZT *>(p.tval)[r] = acc.v; p.tpres[r] = (uint8_t)(acc.has != 0); }
-}
-
 __global__ void clear_presence_kernel(uint8_t *p, int64_t n) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) p[k] = 0;
-}
-
-template <typename XT, typename ZT, int ADD, int MUL, bool SPARSE>
-static void spmv_launch(const SpmvArgs &a) {
-    spmv_tile_kernel<XT, ZT, ADD, MUL, SPARSE, SPMV_PER_THREAD><<<(unsigned)a.ntiles, SPMV_THREADS, 0, G.stream>>>(a); GB_LAUNCHED();
-    spmv_fixup_kernel<ZT, ADD><<<(unsigned)ceil_div(a.ntiles * 32, 256), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-}
-
-// compile-time specialised semirings (spmv_common.cuh: BASELINE.json north_star PLUS_TIMES, LOR_LAND, MIN_PLUS, PLUS_SECOND,
-// and the ones the reference's demos use) for dense u; everything else runs the same kernel with run-time operator codes.
-template <typename T> static bool spmv_fast(int add, int mul, const SpmvArgs &a) {
-#define GB_FAST(A, M) if (add == A && mul == M) { spmv_launch<T, T, A, M, false>(a); return true; }
-    GB_SPMV_FAST_PAIRS(T, GB_FAST)
-#undef GB_FAST
-    return false;
-}
-
-static GrB_Info spmv_dispatch(int xt, int zt, int add, int mul, bool sparse_u, const SpmvArgs &a, std::string *err) {
-    if (spmv_is_fast(xt, zt, add, mul, sparse_u)) {
-        bool ok = false;
-        switch (xt) {
-            case TC_FP32:  ok = spmv_fast<float>(add, mul, a); break;
-            case TC_FP64:  ok = spmv_fast<double>(add, mul, a); break;
-            case TC_INT32: ok = spmv_fast<int32_t>(add, mul, a); break;
-            case TC_INT64: ok = spmv_fast<int64_t>(add, mul, a); break;
-            case TC_UINT32: ok = spmv_fast<uint32_t>(add, mul, a); break;
-            case TC_UINT64: ok = spmv_fast<uint64_t>(add, mul, a); break;
-            case TC_BOOL:  ok = spmv_fast<bool>(add, mul, a); break;
-            default: break;
-        }
-        return ok ? GrB_SUCCESS : gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
-    }
-    bool ok;
-    GB_FOR_DOMAINS(xt, zt, ok, if (sparse_u) spmv_launch<XT_, ZT_, -1, -1, true>(a); else spmv_launch<XT_, ZT_, -1, -1, false>(a));
-    return ok ? GrB_SUCCESS : gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
 }
 
 // w<mask> = accum(w, A' (+).(x) u) with `flip` selecting mul(u,a) (vxm) and `use_transpose`
@@ -342,9 +69,8 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const Tunables &tn = tunables();
     std::string hot_note;                    // the burble line names the cluster; it is printed when `burble` is destroyed
     GbBurble burble(fn);
-    // wide route (csr_wide: nnz >= 2^32, or B200_debug_wide): 64-bit row offsets in the plan, pull and push kernels, no tile kernel
+    // wide route (csr_wide: nnz >= 2^32, or B200_debug_wide): 64-bit row offsets in the run plan, pull and push kernels
     const bool wide = csr_wide(c);
-    if (!wide) GB_TRY(spmv_plan(c, err));
 
     DevBuf<void> a_cast, u_cast;
     const void *aval = c.val, *uval = u->dval;
@@ -393,35 +119,34 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
             PushArgs ps{}; PushArgsWide psw{};
             GB_TRY(wide ? push(psw, o.rowptr.get()) : push(ps, o.rowptr32.get()));
         }
-        PullArgs pa{}; PullArgsWide paw{};
-        pa.rowptr = c.rowptr32; pa.col = c.col; pa.aval = aval; pa.nrows = c.nrows; pa.uval = uval; pa.upres = u->dpres;
-        pa.mval = mask->dval; pa.mpres = mask->dpres; pa.mtc = mask->type->code; pa.mask_comp = f.mask_comp; pa.mask_struct = f.mask_struct;
-        pa.tval = tval; pa.tpres = tpres; pa.add_op = add; pa.mul_op = kmul; pa.flip = kflip;
         // rows longer than PULL_LONG: at most nnz / PULL_LONG of them
-        pa.long_cap = c.nnz / (int64_t)PULL_LONG + 1; pa.has_long = c.nnz > (int64_t)PULL_LONG;
+        const int64_t long_cap = c.nnz / (int64_t)PULL_LONG + 1;
         DevBuf<uint32_t> long_rows; DevBuf<int> long_count;
-        GB_TRY(long_rows.alloc((size_t)pa.long_cap + 1, err));
+        GB_TRY(long_rows.alloc((size_t)long_cap + 1, err));
         GB_TRY(long_count.alloc(4, err));
-        pa.long_rows = long_rows; pa.long_count = long_count;
-        CU_TRY(cudaMemsetAsync(pa.long_count, 0, sizeof(int), G.stream), err);
-        if (!pushed && wide) {
-            paw.rowptr = c.rowptr; paw.col = pa.col; paw.aval = pa.aval; paw.nrows = pa.nrows; paw.uval = pa.uval; paw.upres = pa.upres;
-            paw.mval = pa.mval; paw.mpres = pa.mpres; paw.mtc = pa.mtc; paw.mask_comp = pa.mask_comp; paw.mask_struct = pa.mask_struct;
-            paw.tval = pa.tval; paw.tpres = pa.tpres; paw.add_op = pa.add_op; paw.mul_op = pa.mul_op; paw.flip = pa.flip;
-            paw.has_long = pa.has_long; paw.long_cap = pa.long_cap; paw.long_rows = pa.long_rows; paw.long_count = pa.long_count;
-            GB_TRY(spmv_masked_pull_dispatch(xt, zt, paw, err));
-        } else if (!pushed) GB_TRY(spmv_masked_pull_dispatch(xt, zt, pa, err));
+        CU_TRY(cudaMemsetAsync(long_count, 0, sizeof(int), G.stream), err);
+        auto pull = [&](auto &pa, const auto *rowptr) {
+            pa.rowptr = rowptr; pa.col = c.col; pa.aval = aval; pa.nrows = c.nrows; pa.uval = uval; pa.upres = u->dpres;
+            pa.mval = mask->dval; pa.mpres = mask->dpres; pa.mtc = mask->type->code; pa.mask_comp = f.mask_comp; pa.mask_struct = f.mask_struct;
+            pa.tval = tval; pa.tpres = tpres; pa.add_op = add; pa.mul_op = kmul; pa.flip = kflip;
+            pa.long_cap = long_cap; pa.has_long = c.nnz > (int64_t)PULL_LONG; pa.long_rows = long_rows; pa.long_count = long_count;
+            return spmv_masked_pull_dispatch(xt, zt, pa, err);
+        };
+        PullArgs pa{}; PullArgsWide paw{};
+        if (!pushed) GB_TRY(wide ? pull(paw, c.rowptr.get()) : pull(pa, c.rowptr32.get()));
     }
-    // dense u + specialised semiring: warp-independent run kernel on the cached run plan
-    const bool run_ok = !use_pull && (fast_sr || xt == zt || zt == TC_BOOL);     // specialised or run-time operators; dense or sparse u
-    bool use_run = run_ok && c.nnz >= 4096;
-    if (tn.spmv_run >= 0) use_run = run_ok && c.nnz > 0 && tn.spmv_run != 0;
-    if (wide) use_run = run_ok && c.nnz > 0;          // the wide route has no tile kernel: B200GRB_SPMV_RUN does not apply
     const char *kernel_name = "pull";
     int hot_cluster = 0, hot_ctas = 0; uint32_t hot_t0 = 0, hot_t1 = 0, hot_henc = 0;      // cluster size, grid and tiers of the hot-table launch
     if (use_pull) {
         if (pushed) kernel_name = "push";
-    } else if (use_run) {
+    } else if (c.nnz == 0) {
+        clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
+        kernel_name = "empty";
+    } else {
+        // the run kernel on the cached run plan: compile-time specialised semirings, or run-time operator codes on the (x, z)
+        // domains GB_FOR_DOMAINS lists; dense or sparse u
+        bool domains_ok; GB_FOR_DOMAINS(xt, zt, domains_ok, (void)0);      // the specialised semirings are among them
+        if (!domains_ok) return gb_fail(GrB_DOMAIN_MISMATCH, err, "mxv: unsupported semiring domains (x=%d, z=%d)", xt, zt);
         GB_TRY(spmv_run_plan(c, err));
         RunArgs ra{};
         const RunPlan &rp = c.run;
@@ -457,24 +182,6 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         const bool ok = fast_sr ? spmv_run_dispatch(xt, add, kmul, ra, hot_kb > 0 ? &hot : nullptr, (size_t)hot_kb << 10) : spmv_run_generic(xt, zt, ra);
         if (!ok) return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
         if (hot_kb > 0) { hot_cluster = hot.cluster; hot_ctas = hot.ctas; hot_t0 = hot.t0; hot_t1 = hot.t1; hot_henc = hot.henc; }
-    } else if (c.nnz == 0) {
-        clear_presence_kernel<<<grid_for(n), 256, 0, G.stream>>>(tpres, n); GB_LAUNCHED();
-        kernel_name = "empty";
-    } else {
-        kernel_name = fast ? "tile (specialised, 8 items)" : "tile (run-time operators)";
-        SpmvArgs a{};
-        a.rowptr = c.rowptr32; a.col = c.col; a.aval = aval; a.tile_row = c.tile.row; a.ntiles = c.tile.ntiles;
-        a.nrows = c.nrows; a.nnz = c.nnz; a.uval = uval; a.upres = u->dpres; a.tval = tval; a.tpres = tpres;
-        a.add_op = add; a.mul_op = kmul; a.flip = kflip; a.tile = SPMV_TILE;
-        const size_t nt = (size_t)c.tile.ntiles;
-        DevBuf<void> head_val, tail_val; DevBuf<uint8_t> head_has, tail_has; DevBuf<int32_t> tail_row;
-        GB_TRY(head_val.alloc(nt * zsz + 16, err));
-        GB_TRY(tail_val.alloc(nt * zsz + 16, err));
-        GB_TRY(head_has.alloc(nt, err));
-        GB_TRY(tail_has.alloc(nt, err));
-        GB_TRY(tail_row.alloc(nt, err));
-        a.head_val = head_val; a.tail_val = tail_val; a.head_has = head_has; a.tail_has = tail_has; a.tail_row = tail_row;
-        GB_TRY(spmv_dispatch(xt, zt, add, kmul, sparse_u, a, err));
     }
     gb_kernel_used(kernel_name);
     if (wide) gb_kernel_used("offsets=64");

@@ -1,4 +1,4 @@
-// Shared by the SpMV translation units (spmv.cu: tile kernel + host logic; spmv_run*.cu: run kernels;
+// Shared by the SpMV translation units (spmv.cu: host logic; spmv_run*.cu: run kernels;
 // spmv_pull.cu: masked pull kernels).  Split only to keep nvcc's per-file time down.
 #pragma once
 #include "common.cuh"
@@ -62,7 +62,7 @@ template <typename T> __device__ __forceinline__ T shfl_idx_t(T v, int src) {
     else { int x = (int)v; x = __shfl_sync(0xffffffffu, x, src); return (T)x; }
 }
 
-// ---- the semirings with compile-time kernels (tile and run kernels; dense u, x = z): F(ADD, MUL) for each.  The numeric list
+// ---- the semirings with compile-time run kernels (dense u, x = z): F(ADD, MUL) for each.  The numeric list
 //      serves FP32, FP64, INT32, INT64, UINT32 and UINT64, the BOOL list BOOL; every other semiring runs with operator codes.
 #define GB_SPMV_FAST_NUM(F) F(OP_PLUS, OP_TIMES) F(OP_MIN, OP_PLUS) F(OP_PLUS, OP_SECOND) F(OP_PLUS, OP_FIRST) \
                             F(OP_PLUS, OP_PAIR) F(OP_MIN, OP_FIRST) F(OP_MIN, OP_SECOND)

@@ -9,14 +9,14 @@
 // Dense-u kernel for the specialised semirings: warp-independent RUNS.
 //
 // The entries are cut into runs of 256 (one warp, 8 consecutive entries per lane).  A cached plan gives
-// every lane what the tile kernel has to discover with shared-memory marks, a row pass and barriers:
+// every lane where its rows start, so that no lane has to find them out at call time:
 //   run_headw   one bit per entry: "this entry starts a row"
 //   run_base    number of row starts before the run;  run_lane: row starts inside the run before the lane
 //   nzrow       ids of the non-empty rows (row start rank -> row id);  pres_tmpl: the output's presence
 // so a warp needs no shared memory and no barrier: stream 8 entries, gather, fold between the row-start
 // bits (rows inside a lane are final), one segmented suffix scan over the 32 lanes, and the two partial
 // rows sticking out of the run go to per-run slots that spmv_run_fixup_kernel combines in a fixed order
-// (deterministic).  ~3.5x fewer instructions per entry than the tile kernel.
+// (deterministic).
 // HOT: persistent CTAs, hot_n most referenced entries of the (relabelled) u in a shared-memory table.
 
 

@@ -119,7 +119,7 @@ def test_mxv_kernels(kind):
     # u built on the host: its upload (vector_ensure_device, dense staging) runs under injection too
     k = _sweep(lambda: (_mat(S, FP32), Vector.from_lists(np.arange(len(u)), u, len(u), FP32)),
                lambda A, v: A.mxv(v, semiring=FP32.PLUS_TIMES), _close_vec(S.astype(np.float64), u.astype(np.float64)))
-    assert k > (10 if kind != "tile" else 2)
+    assert k > 10
 
 
 def test_mxv_hot_table(monkeypatch, capfd):

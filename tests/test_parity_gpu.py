@@ -318,13 +318,13 @@ def test_rmat_masked_mxm_large_ST1_and_valued_mask():
     assert np.array_equal(Bp, R2.indptr) and np.array_equal(Bj, R2.indices) and np.array_equal(Bx, R2.data.astype(np.int64))
 
 
-@pytest.mark.parametrize("mode", [{}, {"B200GRB_SPMV_HOT": "64"}, {"B200GRB_SPMV_HOT": "0"}, {"B200GRB_SPMV_RUN": "0"}])
+@pytest.mark.parametrize("mode", [{}, {"B200GRB_SPMV_HOT": "64"}, {"B200GRB_SPMV_HOT": "0"}])
 def test_large_spmv_all_kernel_variants(mode):
     """Large dense-u SpMV through every kernel variant (hot-table run kernel with TMA-staged runs at two table
-    sizes, plain run kernel, tile kernel): exact against the oracle on small-integer data, for specialised and
+    sizes, plain run kernel): exact against the oracle on small-integer data, for specialised and
     run-time semirings."""
     import os
-    old = {k: os.environ.get(k) for k in ("B200GRB_SPMV_HOT", "B200GRB_SPMV_RUN")}
+    old = {k: os.environ.get(k) for k in ("B200GRB_SPMV_HOT",)}
     os.environ.update(mode)
     gb.lib.B200_reload_tunables()                 # the switches are read at GrB_init and on request only
     try:

@@ -576,7 +576,7 @@ def _hyper_expect(form, t):
     elif form == "mxm":
         assert any(k.startswith("esc-") or k == "spa" for k in e), t
     else:
-        assert any(k.startswith("tile") or k.startswith("run") for k in e), t
+        assert any(k.startswith("run") for k in e), t
     REACHED.add(f"hyper-{form}")
 
 

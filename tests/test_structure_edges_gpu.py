@@ -13,7 +13,7 @@ Values are drawn from the edge pools of util.rand_edge_values; FP PLUS / TIMES f
 that every fold order gives the same bits.  Results are compared with the rules of test_value_edges_gpu.py: bit-exact,
 NaN matches NaN, +-0 match under MIN / MAX, and an ANY result must be one of its entry's products.
 
-The last sections run call sequences that reuse cached state (the tile / run / hot plans and the cached transpose of a
+The last sections run call sequences that reuse cached state (the run / hot plans and the cached transpose of a
 matrix, the grow-only workspaces, mxv formed in place in w's buffers) and check every step against the oracle."""
 import functools
 
@@ -160,21 +160,16 @@ def spmv_route(S, sr, vxm, env, sparse_u=False, upres=None, masked=False):
             if not (edges * 16 > c.nnz or count * 32 > o.shape[0]) or "B200GRB_FORCE_PUSH" in env:
                 return "push"
         return "pull"
-    use_run = c.nnz >= 4096
-    if "B200GRB_SPMV_RUN" in env:
-        use_run = c.nnz > 0 and int(env["B200GRB_SPMV_RUN"]) != 0
-    if use_run:
-        hot_kb = int(env.get("B200GRB_SPMV_HOT", -1))
-        hot = False
-        if fast and need_u and (hot_kb if hot_kb >= 0 else 128) > 0 and c.nnz >= (1 << 20) and c.shape[1] >= (1 << 16):
-            henc, cover = _hot_stats(key)
-            hot = henc >= 16 and (hot_kb >= 0 or cover >= 0.25)
-        if hot:
-            return "run+hot-table (TMA-staged)"
-        return "run (sparse u)" if sparse_u else "run"
     if c.nnz == 0:
         return "empty"
-    return "tile (specialised, 8 items)" if fast else "tile (run-time operators)"
+    hot_kb = int(env.get("B200GRB_SPMV_HOT", -1))
+    hot = False
+    if fast and need_u and (hot_kb if hot_kb >= 0 else 128) > 0 and c.nnz >= (1 << 20) and c.shape[1] >= (1 << 16):
+        henc, cover = _hot_stats(key)
+        hot = henc >= 16 and (hot_kb >= 0 or cover >= 0.25)
+    if hot:
+        return "run+hot-table (TMA-staged)"
+    return "run (sparse u)" if sparse_u else "run"
 
 
 def flops_per_row(SA, SB):
@@ -396,10 +391,10 @@ def run_gemm(SA, SB, SM, desc, label, env=None, srs=GEMM_SRS, c_init=False, accu
     return routes
 
 
-# ================================================================== SpMV: tile
+# ================================================================== SpMV: small matrices
 def tile_pattern(items, tail):
-    """Rows laid out against tiles of T = 256 * items entries: three leading empty rows; a row covering two whole tiles
-    and more; a row ending at the last entry of tile 2; empty rows on that boundary; a row of one entry (ending at the
+    """Rows laid out against tiles of T = 256 * items entries (items runs of the run kernel): three leading empty rows; a
+    row covering two whole tiles and more; a row ending at the last entry of tile 2; empty rows on that boundary; a row of one entry (ending at the
     first entry of tile 3); a row ending at the end of tile 3; 3000 empty rows; a row of 7; then rows up to
     nnz = 6 T + tail (tail in -1, 0, 1); five trailing empty rows."""
     T = 256 * items
@@ -421,9 +416,8 @@ def tile_pattern(items, tail):
 @pytest.mark.parametrize("items", [8])
 def test_tile_boundaries(items, tail):
     S = tile_pattern(items, tail)
-    env = {"B200GRB_SPMV_RUN": 0}
-    routes = run_spmv(S, f"tile-{items}-{tail}", env)
-    assert f"tile (specialised, {items} items)" in routes and "tile (run-time operators)" in routes, routes
+    routes = run_spmv(S, f"tile-{items}-{tail}")
+    assert routes == {"run"}, routes
     side(f"tile-{items}-nnz{tail:+d}")
 
 
@@ -437,7 +431,7 @@ def test_tile_degenerate_shapes(shape):
         S = csr([0] * 2499 + [1], 777, cols={2499: [776]})
         assert S.indices[-1] == 776 and row_span(S, 2499) == (0, 1)
     routes = run_spmv(S, f"tile-{shape}")
-    assert all(r.startswith("tile") for r in routes), routes
+    assert routes == {"run"}, routes
     side(f"tile-{shape}")
 
 
@@ -446,7 +440,7 @@ def run_pattern(tail, natural=False):
     """Rows laid out against runs of 256 entries and lane groups of 8: two leading empty rows; a row over three runs
     ending at a position = 7 (mod 8); rows starting at = 7, 0 and 1 (mod 8); a row ending at the end of run 3; 2000
     empty rows; a row covering exactly two whole runs; filler rows up to nnz = k * 256 + tail; trailing empty rows.
-    natural: nnz = 4096 + tail, the size at which the run kernel is chosen without the switch."""
+    natural: nnz = 4096 + tail."""
     lens = [0, 0, 3 * RUN + 7, 1, 1, 4 * RUN - (3 * RUN + 9)] + [0] * 2000 + [2 * RUN]
     total = (4096 if natural else 8 * RUN) + tail
     while sum(lens) + 100 < total:
@@ -464,17 +458,17 @@ def run_pattern(tail, natural=False):
 @pytest.mark.parametrize("tail", [-1, 0, 1])
 def test_run_boundaries(tail, u):
     S = run_pattern(tail)
-    routes = run_spmv(S, f"run-{tail}-{u}", {"B200GRB_SPMV_RUN": 1}, sparse_u=0.6 if u == "sparse" else None)
+    routes = run_spmv(S, f"run-{tail}-{u}", sparse_u=0.6 if u == "sparse" else None)
     assert routes == ({"run"} if u == "dense" else {"run (sparse u)"}), routes
     side(f"run-nnz{tail:+d}")
 
 
 @pytest.mark.parametrize("tail", [-1, 0])
 def test_run_threshold(tail):
-    """nnz = 4095: the tile kernel; nnz = 4096: the run kernel, without any switch."""
+    """nnz = 4095 and nnz = 4096: the run kernel on both sides, with no size threshold."""
     S = run_pattern(tail, natural=True)
     routes = run_spmv(S, f"run-threshold{tail}", forms=("mxv",))
-    assert all(r.startswith("tile") for r in routes) if tail < 0 else routes == {"run"}, routes
+    assert routes == {"run"}, routes
     side("run-threshold-below" if tail < 0 else "run-threshold-at")
 
 
@@ -896,7 +890,7 @@ def test_gemm_into_operand(path):
 
 
 SPMV_WB_PATHS = {"run": (lambda: run_pattern(0, natural=True), {}), "hot": (lambda: hot_pattern(1 << 16, (1 << 20) + 1), {}),
-                 "tile": (lambda: tile_pattern(8, 1), {"B200GRB_SPMV_RUN": 0})}
+                 "tile": (lambda: tile_pattern(8, 1), {})}
 WB_SPMV_SRS = [("PLUS", "TIMES", "INT32"), ("MIN", "PLUS", "FP32"), ("PLUS", "TIMES", "FP64"), ("MAX", "MINUS", "INT64"),
                ("LOR", "LAND", "BOOL")]
 
@@ -907,7 +901,7 @@ def test_spmv_writeback(path, variant):
     desc, accum, w_init, mspec = WB_VARIANTS[variant]
     build, env = SPMV_WB_PATHS[path]
     routes = run_spmv(build(), f"wb-{path}-{variant}", env, srs=WB_SPMV_SRS, mask=mspec, desc=desc, accum=accum, w_init=w_init)
-    fam = {"run": "run", "hot": "run+hot", "tile": "tile"}[path]
+    fam = {"run": "run", "hot": "run+hot", "tile": "run"}[path]
     assert any(r.startswith(fam) for r in routes), routes
     side(f"wb-spmv-{path}-{variant}")
 
@@ -973,7 +967,7 @@ def _check_mxv(A, model, sr, env, label, forms=("mxv", "vxm", "T0")):
     return kinds
 
 
-SEQ_PATHS = {"tile": (lambda: tile_pattern(8, 0), {"B200GRB_SPMV_RUN": 0}),
+SEQ_PATHS = {"tile": (lambda: tile_pattern(8, 0), {}),
              "run": (lambda: run_pattern(1, natural=True), {}),
              "hot": (lambda: hot_pattern(1 << 16, (1 << 20) + 1), {})}
 SEQ_SRS = [("PLUS", "TIMES", "INT64"), ("MAX", "TIMES", "INT32"), ("PLUS", "TIMES", "FP32"), ("LOR", "LAND", "BOOL")]
@@ -1030,14 +1024,13 @@ def test_plans_dropped_when_matrix_changes(path):
     side(f"seq-{path}")
 
 
-def test_alternating_semirings_share_tile_plan():
-    """Specialised and run-time-operator semirings alternate on one matrix: every call reuses the one cached tile plan,
+def test_alternating_semirings_share_run_plan():
+    """Specialised and run-time-operator semirings alternate on one matrix: every call reuses the one cached run plan,
     and every result equals the model."""
     S = tile_pattern(8, 1)
-    env = {"B200GRB_SPMV_RUN": 0}
     srs = [("PLUS", "TIMES", "INT32"), ("MAX", "TIMES", "INT32")] * 3 + [("PLUS", "TIMES", "FP64"), ("MAX", "MINUS", "FP64")] * 2
-    routes = run_spmv(S, "alternate", env, srs=srs, forms=("mxv",))
-    assert routes == {"tile (specialised, 8 items)", "tile (run-time operators)"}, routes
+    routes = run_spmv(S, "alternate", srs=srs, forms=("mxv",))
+    assert routes == {"run"}, routes
     side("seq-alternate")
 
 
@@ -1101,7 +1094,7 @@ def test_mxv_in_place_sequences(inplace):
 
 
 # ------------------------------------------------------------------ every entry, variant and boundary side was reached
-ALL_ENTRIES = {"tile (specialised, 8 items)", "tile (run-time operators)", "run", "run (sparse u)", "run+hot-table (TMA-staged)",
+ALL_ENTRIES = {"run", "run (sparse u)", "run+hot-table (TMA-staged)",
                "pull", "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot",
                "filter=exact", "filter=bloom", "mxv=in-place"}
 ALL_SIDES = (

@@ -90,7 +90,7 @@ def rmat17():
 
 # SpMV paths: pattern, the switches, the expected kernel, the semirings it serves
 SPMV = {
-    "tile-8": dict(shape="small", env={}, kernel="tile", only=None),
+    "tile-8": dict(shape="small", env={}, kernel="run", only=None),          # a matrix smaller than 8 runs
     "run": dict(shape="run", env={}, kernel="run", only=None),
     "run-sparse-u": dict(shape="run", env={}, kernel="run (sparse u)", only=None, sparse_u=True),
     "hot": dict(shape="rmat", env={"B200GRB_SPMV_HOT": 128}, kernel="run+hot-table (TMA-staged)", only=spmv_specialised),
@@ -104,7 +104,7 @@ HOT_T = ["BOOL", "INT32", "UINT64", "FP32", "FP64"]
 @functools.lru_cache(maxsize=None)
 def spmv_pattern(shape):
     if shape == "small":
-        return pattern(11, 300, 400, 6)                       # 1800 entries: the tile kernel
+        return pattern(11, 300, 400, 6)                       # 1800 entries: the run kernel on a small matrix
     if shape == "run":
         return pattern(12, 3000, 2500, 6)                     # 18000 entries: the run kernel
     if shape == "rmat":
@@ -120,8 +120,6 @@ def spmv_pattern(shape):
 
 def _spmv_expect(path, cfg, typ, add, mul, vxm):
     k = cfg["kernel"]
-    if path == "tile-8":
-        return None                                            # specialised (8 items) or run-time operators: checked by prefix
     if path == "hot" and mul == ("SECOND" if vxm else "FIRST"):
         return "run"                                           # the multiply ignores u: no gathers for the hot table to serve
     return k
@@ -160,10 +158,7 @@ def run_spmv_path(path, typ):
                     calls += 1
                     want_k = _spmv_expect(path, cfg, typ, sr[0], sr[1], vxm)
                     form = "vxm" if vxm else "mxv"
-                    if want_k is None:
-                        assert len(ks) == 1 and ks[0].startswith("tile"), (path, sr, form, ks)
-                    else:
-                        assert entries(ks) == [want_k], (path, sr, form, ks)
+                    assert entries(ks) == [want_k], (path, sr, form, ks)
                     gI, gX = w.to_arrays()
                     ref = (orc.vxm(orc.SpVec(w.type.name, n_out), mo, None, sr, uo, Ao, "S" if mo else "") if vxm else
                            orc.mxv(orc.SpVec(w.type.name, n_out), mo, None, sr, Ao, uo, "S" if mo else ""))
@@ -320,7 +315,7 @@ def test_mixed_types(path, case):
         wv = util.rand_edge_values(rng, ctyp, nrows, 0.5)
         w = Vector.from_lists(np.flatnonzero(wp), wv[wp], nrows, util.g_type(ctyp))
         A.mxv(u, semiring=semiring(*sr), out=w, accum=accum)
-        assert _kernels()[0].startswith("tile" if path == "tile-8" else "run"), last_kernel()
+        assert _kernels()[0].startswith("run"), last_kernel()
         gI, gX = w.to_arrays()
         ref = orc.mxv(orc.SpVec(ctyp, nrows, np.flatnonzero(wp), wv[wp]), None, acc, sr, o_csr(otyp, S, av),
                       orc.SpVec(otyp, ncols, np.arange(ncols), uv))
@@ -404,7 +399,7 @@ def test_fp_sums_within_error_bound(path, typ, scale):
         with tunables(**cfg["env"]):
             w = A.mxv(u, semiring=s)
             ks = _kernels()
-        assert entries(ks) == [_spmv_expect(path, cfg, typ, "PLUS", "TIMES", False)] if path != "tile-8" else ks[0].startswith("tile"), ks
+        assert entries(ks) == [_spmv_expect(path, cfg, typ, "PLUS", "TIMES", False)], ks
         gI, gX = w.to_arrays()
         Ar = np.repeat(np.arange(nrows), np.diff(S.indptr))
         keep = upres[S.indices]
@@ -439,7 +434,7 @@ def test_fp_sums_within_error_bound(path, typ, scale):
 
 
 # ------------------------------------------------------------------ every path of the table was reached
-ALL_PATHS = {"tile (specialised, 8 items)", "tile (run-time operators)", "run", "run (sparse u)", "run+hot-table (TMA-staged)", "pull",
+ALL_PATHS = {"run", "run (sparse u)", "run+hot-table (TMA-staged)", "pull",
              "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot"}
 
 

@@ -143,10 +143,7 @@ def test_wide_equals_narrow(case):
     wI = np.flatnonzero(rng.random(n_out) < 0.5) if o.get("accum") else np.zeros(0, np.int64)
     wX = values(seed_of("wide-w", name), zt, len(wI), pool if zt == typ else "edge", 1)
     w0 = (wI, wX, n_out)
-    env = dict(o.get("env", {}))
-    if not o.get("mask"):
-        env.setdefault("B200GRB_SPMV_RUN", 1)      # the narrow route takes the run kernel at every size, as the wide one does
-    with tunables(**env):
+    with tunables(**o.get("env", {})):
         nI, nX, nks = _call(S, av, sr, form, o, uv, upres, mask, w0, typ)
         with wide(7 if S.nnz < 20000 else S.nnz // 5 + 1):      # transposes in thousands of chunks, or in 5 for the large shapes
             gI, gX, gks = _call(S, av, sr, form, o, uv, upres, mask, w0, typ)

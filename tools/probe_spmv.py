@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Which part of the SpMV tile kernel costs what: same graph, semirings that drop the gather / the value stream."""
+"""Which part of the SpMV run kernel costs what: same graph, semirings that drop the gather / the value stream."""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -18,11 +18,8 @@ sp_ = gb.ffi.new("void**"); gb.lib.B200_get_stream(sp_)
 stream = torch.cuda.ExternalStream(int(gb.ffi.cast("uintptr_t", sp_[0])))
 
 def run(label, sr, env):
-    keep_run = os.environ.get("B200GRB_SPMV_RUN")
-    for k in ("B200GRB_SPMV_HOT", "B200GRB_SPMV_RUN", "B200GRB_SPMV_CLUSTER", "B200GRB_SPMV_HOT_REPL"):
+    for k in ("B200GRB_SPMV_HOT", "B200GRB_SPMV_CLUSTER", "B200GRB_SPMV_HOT_REPL"):
         os.environ.pop(k, None)
-    if keep_run is not None and "B200GRB_SPMV_RUN" not in env:
-        os.environ["B200GRB_SPMV_RUN"] = keep_run
     os.environ.update(env)
     gb.lib.B200_reload_tunables()
     for _ in range(5):

@@ -74,24 +74,30 @@ template <typename T> static inline GrB_Info dalloc(T **p, size_t count, std::st
 
 // Owner of one dmalloc block, released at scope exit (stream-ordered after the kernels already enqueued).  It converts
 // to the raw pointer, so it can stand wherever a device pointer is read.  DevBuf<void> takes an exact byte count.
+// A borrowed block (borrow) belongs to someone else -- another container, a communicator's cudaMalloc region -- and is
+// never freed here.
 template <typename T> class DevBuf {
     T *p_ = nullptr;
+    bool borrowed_ = false;
 public:
     DevBuf() = default;                 // move-only: declaring the moves deletes the copies
-    DevBuf(DevBuf &&o) noexcept : p_(o.p_) { o.p_ = nullptr; }
-    DevBuf &operator=(DevBuf &&o) noexcept { if (this != &o) { reset(); p_ = o.p_; o.p_ = nullptr; } return *this; }
+    DevBuf(DevBuf &&o) noexcept : p_(o.p_), borrowed_(o.borrowed_) { o.p_ = nullptr; o.borrowed_ = false; }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) { reset(); p_ = o.p_; borrowed_ = o.borrowed_; o.p_ = nullptr; o.borrowed_ = false; }
+        return *this;
+    }
     ~DevBuf() { reset(); }
     GrB_Info alloc(size_t count, std::string *err) {
         reset();
         if constexpr (std::is_void<T>::value) return dmalloc(&p_, count, err);
         else return dalloc(&p_, count, err);
     }
+    void borrow(T *p) { reset(); p_ = p; borrowed_ = true; }
+    bool borrowed() const { return borrowed_; }
     T *get() const { return p_; }
     operator T *() const { return p_; }
     template <typename U> explicit operator U *() const { return (U *)p_; }
-    T *release() { T *q = p_; p_ = nullptr; return q; }
-    void reset() { dfree(p_); p_ = nullptr; }
-    void adopt(T *p) { reset(); p_ = p; }     // takes a dmalloc block handed over as a raw pointer (vector_write's result)
+    void reset() { if (!borrowed_) dfree(p_); p_ = nullptr; borrowed_ = false; }
 };
 
 // run plan (spmv_run.cu, warp-independent kernels): entries cut into warp-sized runs of 256
@@ -148,14 +154,19 @@ struct Csr : CsrFields {
 // layout (always CSR by row / dense + presence) -- the API is format-agnostic, results do not depend on them
 struct GBObjOpts { double hyper = 0.0625; int format = 0 /* GxB_BY_ROW */; int sparsity = 15 /* GxB_AUTO_SPARSITY */; };
 
-// Dense device form of a matrix (DESIGN.md section 3.6): nrows x ncols values of the matrix type, row-major, and one presence byte
-// per entry (pres NULL: every entry present).  Only B200_Matrix_import_dense and the SpMM result of GrB_mxm create one.  While it
-// is held it is authoritative: the CSR and the host tuples beside it are caches built from it on demand, and any modification
-// drops it (matrix_invalidate_device).  nrows * ncols <= 2^31-1, so the flattened form is a legal vector.
+// Dense device form: values of the container's type, one per position, and one presence byte per position (pres NULL: every
+// position present).  It is the device form of every vector, and of a dense matrix (DESIGN.md section 3.6): nrows x ncols
+// positions, row-major, created only by B200_Matrix_import_dense and the SpMM result of GrB_mxm.  A matrix's dense form is
+// authoritative while it is held: the CSR and the host tuples beside it are caches built from it on demand, and any
+// modification drops it (matrix_invalidate_device).  nrows * ncols <= 2^31-1, so the flattened form is a legal vector.
+// A view (a communicator's result, a stack-built operand) borrows its buffers: dropping the form frees nothing.
 struct DenseForm {
     DevBuf<void> val;
     DevBuf<uint8_t> pres;
     bool valid = false;
+    static DenseForm borrow(void *val, uint8_t *pres) {
+        DenseForm d; d.val.borrow(val); d.pres.borrow(pres); d.valid = true; return d;
+    }
 };
 
 struct GB_Matrix_opaque {
@@ -177,9 +188,8 @@ struct GB_Vector_opaque {
     // host form: sorted unique (index, value)
     std::vector<uint64_t> hi; std::vector<uint8_t> hx; bool host_valid;
     std::vector<uint64_t> pi; std::vector<uint8_t> px;
-    // device form: dense values + presence bytes (present == nullptr: all present)
-    void *dval = nullptr; uint8_t *dpres = nullptr; bool dev_valid = false; int64_t dev_nvals = -1;
-    bool borrowed = false;     // dval / dpres belong to a communicator (dist.cu): never freed through the vector
+    // device form, and its entry count when known (-1: count the presence bytes)
+    DenseForm dv; int64_t dev_nvals = -1;
     // overlapped host copies (B200_Vector_set_dense / export_dense with where = 2): the copy streams' hand-shakes with the compute stream
     cudaEvent_t ev_h2d = nullptr, ev_d2h = nullptr, ev_use = nullptr;
     bool h2d_pending = false, d2h_pending = false, use_recorded = false;
@@ -272,12 +282,12 @@ GrB_Info matrix_ensure_device(GrB_Matrix A);
 GrB_Info matrix_ensure_transpose(GrB_Matrix A);     // builds A->devT on the device
 void matrix_invalidate_device(GrB_Matrix A);
 void matrix_adopt_device(GrB_Matrix A, Csr &&c);    // A takes ownership of c, host form dropped
-void matrix_adopt_dense(GrB_Matrix A, DevBuf<void> &&val, DevBuf<uint8_t> &&pres);   // A takes a dense form, every other form dropped
+void matrix_adopt_dense(GrB_Matrix A, DenseForm &&d);   // A takes a dense form, every other form dropped
 bool matrix_known_empty(const GrB_Matrix A);        // A has no entries, as far as can be told without reading the device
 GrB_Info vector_ensure_host(GrB_Vector v);
 GrB_Info vector_ensure_device(GrB_Vector v);
 void vector_invalidate_device(GrB_Vector v);
-void vector_adopt_device(GrB_Vector v, void *vals, uint8_t *pres);
+void vector_adopt_device(GrB_Vector v, DenseForm &&d);   // v takes d as its device form, host form dropped
 void vector_mark_used(GrB_Vector v);               // after the kernels reading v were enqueued (lets the next overlapped import of v start early)
 bool gb_valid_matrix(const GrB_Matrix A);
 bool gb_valid_vector(const GrB_Vector v);
@@ -298,13 +308,12 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
                           Csr &&T, int ttc, bool t_already_masked, std::string *err);
 // fold of n values (presence bytes optional) with a builtin monoid operator on the device (vector_ops.cu)
 GrB_Info dev_reduce_values(const void *val, const uint8_t *pres, int vtc, int64_t n, int op, int mtc, Sc *out, bool *has, std::string *err);
-// w<mask> = accum(w, T) on the device (vector_ops.cu).  T = (tval, tpres) of type ttc over w->n positions
-// (tpres NULL: every position present; t_scalar: tval is ONE value standing for all positions).  region
-// (NULL = everything) limits the write to the positions it flags, GrB_assign style.  own_val / own_pres hold
-// T's buffers when the caller hands them over (w may then adopt them); empty when T is borrowed.
+// w<mask> = accum(w, T) on the device (vector_ops.cu).  T (val, pres) is of type ttc over w->n positions
+// (pres NULL: every position present; t_scalar: val is ONE value standing for all positions).  region
+// (NULL = everything) limits the write to the positions it flags, GrB_assign style.  w may adopt the buffers of a T
+// that owns them; a borrowed T (another vector's form) is only read.  T is consumed.
 GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const DescFlags &f,
-                      const void *tval, const uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region,
-                      DevBuf<void> &&own_val = DevBuf<void>(), DevBuf<uint8_t> &&own_pres = DevBuf<uint8_t>());
+                      DenseForm &&T, int ttc, bool t_scalar, const uint8_t *region);
 
 // positional operators (positional.cu).  What a positional operator returns, decoded: the index of the first or the second
 // operand (`second`), its row or its column (`col`), plus `off` (0, or 1 for the ...1 forms)

@@ -126,7 +126,7 @@ extern "C" GrB_Info GxB_Matrix_memoryUsage(size_t *size, const GrB_Matrix A) {
 extern "C" GrB_Info GxB_Vector_memoryUsage(size_t *size, const GrB_Vector v) {
     if (!size) return gb_fail(GrB_NULL_POINTER, nullptr, "GxB_Vector_memoryUsage: NULL");
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GxB_Vector_memoryUsage: invalid vector");
-    *size = sizeof(*v) + v->hi.size() * (8 + v->type->size) + (v->dev_valid ? (size_t)v->n * (1 + v->type->size) : 0);
+    *size = sizeof(*v) + v->hi.size() * (8 + v->type->size) + (v->dv.valid ? (size_t)v->n * (1 + v->type->size) : 0);
     return GrB_SUCCESS;
 }
 
@@ -208,5 +208,5 @@ extern "C" GrB_Info GxB_Vector_Option_set(GrB_Vector v, GxB_Option_Field field, 
 }
 extern "C" GrB_Info GxB_Vector_Option_get(GrB_Vector v, GxB_Option_Field field, ...) {
     if (!gb_valid_vector(v)) return gb_fail(GrB_UNINITIALIZED_OBJECT, nullptr, "GxB_Vector_Option_get: invalid vector");
-    va_list ap; va_start(ap, field); const GrB_Info r = object_option_get(v->opts, field, !v->dev_valid, ap); va_end(ap); return r;
+    va_list ap; va_start(ap, field); const GrB_Info r = object_option_get(v->opts, field, !v->dv.valid, ap); va_end(ap); return r;
 }

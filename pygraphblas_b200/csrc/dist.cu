@@ -72,7 +72,6 @@ extern "C" GrB_Info B200_Comm_create(B200_Comm *comm, int rank, int world, GrB_I
     // the borrowed view handed out by B200_Comm_result
     GrB_Info r = GrB_Vector_new(&c->view, type, n);
     if (r != GrB_SUCCESS) { cudaFree(c->region); delete c; return r; }
-    c->view->borrowed = true;
     *comm = c;
     return GrB_SUCCESS;
 }
@@ -111,10 +110,7 @@ extern "C" GrB_Info B200_Comm_free(B200_Comm *comm) {
         for (int p = 0; p < c->world; ++p) if (p != c->rank && c->peer[p]) cudaIpcCloseMemHandle(c->peer[p]);
         cudaFree(c->region);
     }
-    if (c->view) {
-        if (c->view->borrowed) { c->view->dval = nullptr; c->view->dpres = nullptr; c->view->dev_valid = false; c->view->borrowed = false; }
-        GrB_Vector_free(&c->view);           // frees what the view owns
-    }
+    GrB_Vector_free(&c->view);               // frees only what the view came to own, never the region it borrows
     c->magic = GB_FREED; delete c; *comm = nullptr;
     return GrB_SUCCESS;
 }
@@ -215,12 +211,10 @@ __global__ void __launch_bounds__(256) comm_fold_kernel(PeerPtrs part, int world
 static inline int cgrid(size_t bytes) { return (int)std::max<size_t>(1, std::min<size_t>((bytes / 16 + 255) / 256, (size_t)G.num_sms * 4)); }
 static inline int pgrid(size_t bytes) { return (int)std::max<size_t>(1, std::min<size_t>((bytes / 16 + 2047) / 2048, (size_t)G.num_sms * 2)); }
 
+// the view borrows buffer `which`; buffers it came to own (an import into it, a write with it as output) are freed
 static void comm_set_view(B200_Comm c, int which) {
     unsigned char *b = comm_buf(c, c->region, which);
-    vector_invalidate_device(c->view);       // buffers the view came to own (an import into it, a write with it as output) are freed
-    c->view->use_recorded = false;
-    c->view->dval = b; c->view->dpres = b + c->val_bytes; c->view->dev_valid = true; c->view->dev_nvals = -1; c->view->borrowed = true;
-    c->view->host_valid = false; c->view->hi.clear(); c->view->hx.clear(); c->view->pi.clear(); c->view->px.clear();
+    vector_adopt_device(c->view, DenseForm::borrow(b, b + c->val_bytes));
 }
 
 // flags-only round on slot `slot`: raise mine everywhere, wait for everybody's
@@ -273,14 +267,14 @@ extern "C" GrB_Info B200_Comm_allgather(B200_Comm c, const GrB_Vector slice, GrB
                                                             (unsigned long long)row0, (unsigned long long)slice->n);
     GbBurble burble("B200_Comm_allgather");
     GB_TRY(vector_ensure_device(slice));
-    const uint8_t *pres = slice->dpres; DevBuf<uint8_t> ones;
+    const uint8_t *pres = slice->dv.pres; DevBuf<uint8_t> ones;
     if (!pres) {                                                           // a full slice: its presence is all ones
         GB_TRY(ones.alloc((size_t)slice->n + 16, &c->err));
         fill_bytes_kernel<<<cgrid(slice->n), 256, 0, G.stream>>>(ones, (int64_t)slice->n + 16, 1); GB_LAUNCHED();
         pres = ones;
     }
     const int which = (int)((c->step + 1) & 1);
-    GrB_Info r = comm_push_and_wait(c, slice->dval, pres, row0, slice->n, which);
+    GrB_Info r = comm_push_and_wait(c, slice->dv.val, pres, row0, slice->n, which);
     ones.reset();
     burble.note("peer push (NVLink stores) + flag wait", (double)slice->n * (c->esize + 1) * (c->world - 1));
     return r;
@@ -302,8 +296,8 @@ extern "C" GrB_Info B200_Comm_allreduce(B200_Comm c, const GrB_Vector partial, G
     GB_TRY(vector_ensure_device(partial));
     // 1. publish the partial in the exchange region and tell everybody (flag slot 1)
     unsigned char *mine = comm_buf(c, c->region, 2);
-    CU_TRY(cudaMemcpyAsync(mine, partial->dval, (size_t)c->n * c->esize, cudaMemcpyDeviceToDevice, G.stream), &c->err);
-    if (partial->dpres) CU_TRY(cudaMemcpyAsync(mine + c->val_bytes, partial->dpres, (size_t)c->n, cudaMemcpyDeviceToDevice, G.stream), &c->err);
+    CU_TRY(cudaMemcpyAsync(mine, partial->dv.val, (size_t)c->n * c->esize, cudaMemcpyDeviceToDevice, G.stream), &c->err);
+    if (partial->dv.pres) CU_TRY(cudaMemcpyAsync(mine + c->val_bytes, partial->dv.pres, (size_t)c->n, cudaMemcpyDeviceToDevice, G.stream), &c->err);
     else { fill_bytes_kernel<<<cgrid(c->n), 256, 0, G.stream>>>(mine + c->val_bytes, (int64_t)c->n, 1); GB_LAUNCHED(); }
     const unsigned long long step = c->step + 1;
     comm_signal_wait(c, 1, step);

@@ -342,11 +342,11 @@ extern "C" GrB_Info GxB_Matrix_diag(GrB_Matrix C, const GrB_Vector v, int64_t k,
     Csr T;
     GB_TRY(csr_from_row_counts((int64_t)dim, (int64_t)dim, vsize, T, err,
         [&](int64_t *rowptr) {
-            diag_build_kernel<<<grid_for((int64_t)dim + 1), 256, 0, G.stream>>>(v->dpres, (int64_t)v->n, k, (int64_t)dim, rowptr); GB_LAUNCHED();
+            diag_build_kernel<<<grid_for((int64_t)dim + 1), 256, 0, G.stream>>>(v->dv.pres, (int64_t)v->n, k, (int64_t)dim, rowptr); GB_LAUNCHED();
             return GrB_SUCCESS;
         },
         [&](Csr &t) {
-            diag_fill_kernel<<<grid_for((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dval, (int)vsize, (int64_t)v->n, k, (int64_t)dim, t.rowptr, t.col,
+            diag_fill_kernel<<<grid_for((int64_t)dim), 256, 0, G.stream>>>((const uint8_t *)v->dv.val, (int)vsize, (int64_t)v->n, k, (int64_t)dim, t.rowptr, t.col,
                                                                            (uint8_t *)t.val); GB_LAUNCHED();
             return GrB_SUCCESS;
         }));
@@ -385,7 +385,7 @@ extern "C" GrB_Info GxB_Vector_diag(GrB_Vector v, const GrB_Matrix A, int64_t k,
     CU_TRY(cudaMemsetAsync(oval, 0, (size_t)len * vsize, G.stream), err);
     if (len > 0) { diag_extract_kernel<<<grid_for(len), 256, 0, G.stream>>>(A->dev.rowptr, A->dev.col, (const uint8_t *)A->dev.val, (int)vsize, nr, nc, k, len, (uint8_t *)oval, opres); GB_LAUNCHED(); }
     DescFlags plain{};
-    return vector_write(v, nullptr, nullptr, plain, oval, opres, A->type->code, false, nullptr, std::move(oval), std::move(opres));
+    return vector_write(v, nullptr, nullptr, plain, DenseForm{std::move(oval), std::move(opres)}, A->type->code, false, nullptr);
 }
 
 // ================================================================== GrB_Matrix_kronecker_BinaryOp:  C<Mask> = accum(C, kron(op(A), op(B)))
@@ -482,7 +482,7 @@ static GrB_Info slice_vector(const Csr &a, GrB_Type type, int along, uint64_t in
         GB_LAUNCHED();
     }
     GB_TRY(GrB_Vector_new(out, type, (GrB_Index)n));
-    vector_adopt_device(*out, val.release(), pres.release());
+    vector_adopt_device(*out, DenseForm{std::move(val), std::move(pres)});
     return GrB_SUCCESS;
 }
 __global__ void vec_flags_kernel(const uint8_t *pres, int64_t n, int64_t *flag) {
@@ -512,7 +512,7 @@ static GrB_Info vector_as_slice_csr(GrB_Vector v, int along, uint64_t index, int
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
     DevBuf<int64_t> pos;
     GB_TRY(pos.alloc((size_t)n + 1, err));
-    vec_flags_kernel<<<grid_for(n + 1), 256, 0, G.stream>>>(v->dpres, n, pos); GB_LAUNCHED();
+    vec_flags_kernel<<<grid_for(n + 1), 256, 0, G.stream>>>(v->dv.pres, n, pos); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(pos, n + 1, err));
     GB_TRY(read_i64(pos + n, &T.nnz, err));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
@@ -520,11 +520,11 @@ static GrB_Info vector_as_slice_csr(GrB_Vector v, int along, uint64_t index, int
     if (along == 0) {
         GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
         row_only_ptr_kernel<<<grid_for(nrows + 1), 256, 0, G.stream>>>(nrows, (int64_t)index, T.nnz, T.rowptr); GB_LAUNCHED();
-        if (T.nnz > 0) { vec_to_row_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, pos, 0, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
+        if (T.nnz > 0) { vec_to_row_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dv.val, v->dv.pres, (int)vsize, n, pos, 0, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
         pos.reset();
     } else {
         T.rowptr = std::move(pos);       // one entry per present position: the scan IS the row pointer
-        if (T.nnz > 0) { vec_to_col_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dval, v->dpres, (int)vsize, n, T.rowptr, (uint32_t)index, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
+        if (T.nnz > 0) { vec_to_col_kernel<<<grid_for(n), 256, 0, G.stream>>>((const uint8_t *)v->dv.val, v->dv.pres, (int)vsize, n, T.rowptr, (uint32_t)index, T.col, (uint8_t *)T.val); GB_LAUNCHED(); }
     }
     GB_TRY(dev_build_rowptr32(T, err));
     CU_TRY(cudaGetLastError(), err);

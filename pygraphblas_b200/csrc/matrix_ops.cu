@@ -151,15 +151,15 @@ extern "C" GrB_Info GxB_Vector_select(GrB_Vector w, const GrB_Vector mask, const
     GB_TRY(select_args(op, thunk, u->type->code, a, fn));
     GB_NEED_DEVICE(&w->err, fn);
     GB_TRY(vector_ensure_device(u));
-    a.val = u->dval; a.tc = u->type->code; a.nrows = (int64_t)u->n;
+    a.val = u->dv.val; a.tc = u->type->code; a.nrows = (int64_t)u->n;
     // T keeps u's values and narrows its presence: a vector is a column, i = position, j = 0
     const size_t bytes = (size_t)u->n * u->type->size;
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     GB_TRY(tval.alloc(bytes + 16, &w->err));
     GB_TRY(tpres.alloc((size_t)u->n, &w->err));
-    CU_TRY(cudaMemcpyAsync(tval, u->dval, bytes, cudaMemcpyDeviceToDevice, G.stream), &w->err);
-    vec_select_kernel<<<grid_for(a.nrows), 256, 0, G.stream>>>(a, u->dpres, tpres); GB_LAUNCHED();
-    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, std::move(tval), std::move(tpres));
+    CU_TRY(cudaMemcpyAsync(tval, u->dv.val, bytes, cudaMemcpyDeviceToDevice, G.stream), &w->err);
+    vec_select_kernel<<<grid_for(a.nrows), 256, 0, G.stream>>>(a, u->dv.pres, tpres); GB_LAUNCHED();
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, u->type->code, false, nullptr);
 }
 
 // ------------------------------------------------------------------ apply:  T has A's pattern, z = f(a) / op(x, a) / op(a, y)
@@ -287,7 +287,7 @@ static GrB_Info mat_reduce_vector(GrB_Vector w, const GrB_Vector mask, const GrB
     GB_TRY(tpres.alloc((size_t)rows, &w->err));
     a.tval = tval; a.tpres = tpres;
     row_reduce_kernel<<<grid_for(a.nrows * 32), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    return vector_write(w, mask, accum, f, a.tval, a.tpres, a.mtc, false, nullptr, std::move(tval), std::move(tpres));
+    return vector_write(w, mask, accum, f, DenseForm{std::move(tval), std::move(tpres)}, a.mtc, false, nullptr);
 }
 extern "C" GrB_Info GrB_Matrix_reduce_Monoid(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Monoid monoid, const GrB_Matrix A, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;

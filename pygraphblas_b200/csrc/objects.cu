@@ -444,8 +444,7 @@ void vector_mark_used(GrB_Vector v) {
 }
 void vector_invalidate_device(GrB_Vector v) {
     vector_join_copies(v);
-    if (!v->borrowed) { dfree(v->dval); dfree(v->dpres); }       // a borrowed view (B200_Comm_result) does not own its buffers
-    v->borrowed = false; v->dval = nullptr; v->dpres = nullptr; v->dev_valid = false; v->dev_nvals = -1;
+    v->dv = DenseForm(); v->dev_nvals = -1;
 }
 void matrix_adopt_device(GrB_Matrix A, Csr &&c) {
     matrix_invalidate_device(A);
@@ -454,9 +453,9 @@ void matrix_adopt_device(GrB_Matrix A, Csr &&c) {
     A->pi.clear(); A->pj.clear(); A->px.clear();
     A->host_valid = false;
 }
-void matrix_adopt_dense(GrB_Matrix A, DevBuf<void> &&val, DevBuf<uint8_t> &&pres) {
+void matrix_adopt_dense(GrB_Matrix A, DenseForm &&d) {
     matrix_invalidate_device(A);
-    A->dn.val = std::move(val); A->dn.pres = std::move(pres); A->dn.valid = true;
+    A->dn = std::move(d); A->dn.valid = true;
     A->hi.clear(); A->hj.clear(); A->hx.clear(); A->hi.shrink_to_fit(); A->hj.shrink_to_fit(); A->hx.shrink_to_fit();
     A->pi.clear(); A->pj.clear(); A->px.clear();
     A->host_valid = false;
@@ -465,10 +464,10 @@ bool matrix_known_empty(const GrB_Matrix A) {
     if (A->host_valid) return A->hi.empty() && A->pi.empty();
     return A->dev.valid ? A->dev.nnz == 0 : !A->dn.valid;
 }
-void vector_adopt_device(GrB_Vector v, void *vals, uint8_t *pres) {
+void vector_adopt_device(GrB_Vector v, DenseForm &&d) {
     vector_invalidate_device(v);
     v->use_recorded = false;       // the new buffers are filled (and their pool blocks were last used) by work enqueued since
-    v->dval = vals; v->dpres = pres; v->dev_valid = true; v->dev_nvals = pres ? -1 : (int64_t)v->n;
+    v->dv = std::move(d); v->dv.valid = true; v->dev_nvals = v->dv.pres ? -1 : (int64_t)v->n;
     v->hi.clear(); v->hx.clear(); v->pi.clear(); v->px.clear(); v->host_valid = false;
 }
 
@@ -599,16 +598,16 @@ GrB_Info matrix_ensure_transpose(GrB_Matrix A) {
 
 GrB_Info vector_ensure_host(GrB_Vector v) {
     if (v->host_valid) return vector_flush_pending(v);
-    if (!v->dev_valid) { v->host_valid = true; return GrB_SUCCESS; }
+    if (!v->dv.valid) { v->host_valid = true; return GrB_SUCCESS; }
     vector_join_import(v);
     const size_t sz = v->type->size, n = (size_t)v->n;
     std::vector<uint8_t> vals(n * sz), pres;
-    CU_TRY(cudaMemcpyAsync(vals.data(), v->dval, n * sz, cudaMemcpyDeviceToHost, G.stream), &v->err);
-    if (v->dpres) { pres.resize(n); CU_TRY(cudaMemcpyAsync(pres.data(), v->dpres, n, cudaMemcpyDeviceToHost, G.stream), &v->err); }
+    CU_TRY(cudaMemcpyAsync(vals.data(), v->dv.val, n * sz, cudaMemcpyDeviceToHost, G.stream), &v->err);
+    if (v->dv.pres) { pres.resize(n); CU_TRY(cudaMemcpyAsync(pres.data(), v->dv.pres, n, cudaMemcpyDeviceToHost, G.stream), &v->err); }
     CU_TRY(cudaStreamSynchronize(G.stream), &v->err);
     v->hi.clear(); v->hx.clear();
     for (size_t i = 0; i < n; ++i)
-        if (!v->dpres || pres[i]) { v->hi.push_back(i); v->hx.insert(v->hx.end(), &vals[i * sz], &vals[i * sz] + sz); }
+        if (!v->dv.pres || pres[i]) { v->hi.push_back(i); v->hx.insert(v->hx.end(), &vals[i * sz], &vals[i * sz] + sz); }
     v->host_valid = true;
     return GrB_SUCCESS;
 }
@@ -625,17 +624,17 @@ GrB_Info vector_ensure_device(GrB_Vector v) {
     if (v->host_valid) GB_TRY(vector_flush_pending(v));
     vector_join_import(v);
     v->use_recorded = false;       // the caller enqueues work on v after the last recorded use
-    if (v->dev_valid) return GrB_SUCCESS;
+    if (v->dv.valid) return GrB_SUCCESS;
     if (v->n > DEV_DIM_MAX) return gb_fail(GrB_INVALID_VALUE, &v->err, "vector size %llu exceeds the 2^31-1 limit of the HBM layout", (unsigned long long)v->n);
     const size_t sz = v->type->size, n = (size_t)v->n, k = v->hi.size();
-    DevBuf<void> dval; DevBuf<uint8_t> dpres;        // committed to v only once filled
-    GB_TRY(dval.alloc(n * sz + 16, &v->err));
+    DenseForm d;        // committed to v only once filled
+    GB_TRY(d.val.alloc(n * sz + 16, &v->err));
     const bool full = k == n && n > 0;
-    if (!full) GB_TRY(dpres.alloc(n, &v->err));
+    if (!full) GB_TRY(d.pres.alloc(n, &v->err));
     if (n && k < n / 8) {
         // few entries (a BFS source, a seed set): ship the tuples and scatter them in HBM rather than two dense arrays
-        CU_TRY(cudaMemsetAsync(dval, 0, n * sz, G.stream), &v->err);
-        CU_TRY(cudaMemsetAsync(dpres, 0, n, G.stream), &v->err);
+        CU_TRY(cudaMemsetAsync(d.val, 0, n * sz, G.stream), &v->err);
+        CU_TRY(cudaMemsetAsync(d.pres, 0, n, G.stream), &v->err);
         if (k) {
             DevBuf<void> di, dx;
             GB_TRY(di.alloc(k * sizeof(uint64_t), &v->err));
@@ -643,20 +642,19 @@ GrB_Info vector_ensure_device(GrB_Vector v) {
             CU_TRY(cudaMemcpyAsync(di, v->hi.data(), k * sizeof(uint64_t), cudaMemcpyHostToDevice, G.stream), &v->err);
             CU_TRY(cudaMemcpyAsync(dx, v->hx.data(), k * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
             const int grid = (int)std::min<size_t>((k + 255) / 256, 4096);
-            vec_scatter_kernel<<<grid, 256, 0, G.stream>>>((const uint64_t *)di, (const uint8_t *)dx, (uint8_t *)dval, dpres, (int)sz, (int64_t)k);
+            vec_scatter_kernel<<<grid, 256, 0, G.stream>>>((const uint64_t *)di, (const uint8_t *)dx, (uint8_t *)d.val, d.pres, (int)sz, (int64_t)k);
             G.launches++;
             CU_TRY(cudaGetLastError(), &v->err);
         }
     } else if (n) {
         std::vector<uint8_t> vals(n * sz, 0), pres(full ? 0 : n, 0);
         for (size_t q = 0; q < k; ++q) { memcpy(&vals[v->hi[q] * sz], &v->hx[q * sz], sz); if (!full) pres[v->hi[q]] = 1; }
-        CU_TRY(cudaMemcpyAsync(dval, vals.data(), n * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
-        if (!full) CU_TRY(cudaMemcpyAsync(dpres, pres.data(), n, cudaMemcpyHostToDevice, G.stream), &v->err);
+        CU_TRY(cudaMemcpyAsync(d.val, vals.data(), n * sz, cudaMemcpyHostToDevice, G.stream), &v->err);
+        if (!full) CU_TRY(cudaMemcpyAsync(d.pres, pres.data(), n, cudaMemcpyHostToDevice, G.stream), &v->err);
         CU_TRY(cudaStreamSynchronize(G.stream), &v->err);      // the staging vectors die here
     }
     CU_TRY(cudaStreamSynchronize(G.stream), &v->err);
-    v->dval = dval.release(); v->dpres = dpres.release();
-    v->dev_valid = true; v->dev_nvals = (int64_t)v->hi.size();
+    v->dv = std::move(d); v->dv.valid = true; v->dev_nvals = (int64_t)v->hi.size();
     return GrB_SUCCESS;
 }
 
@@ -909,15 +907,14 @@ extern "C" GrB_Info GrB_Vector_dup(GrB_Vector *w, const GrB_Vector u) {
     } else {
         o->host_valid = false;
         const size_t sz = u->type->size, n = (size_t)u->n;
-        DevBuf<void> dval; DevBuf<uint8_t> dpres;
-        GrB_Info r = dval.alloc(n * sz + 16, &u->err);
-        if (r == GrB_SUCCESS && u->dpres) r = dpres.alloc(n, &u->err);
-        if (r == GrB_SUCCESS && cudaMemcpyAsync(dval, u->dval, n * sz, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+        GrB_Info r = o->dv.val.alloc(n * sz + 16, &u->err);
+        if (r == GrB_SUCCESS && u->dv.pres) r = o->dv.pres.alloc(n, &u->err);
+        if (r == GrB_SUCCESS && cudaMemcpyAsync(o->dv.val, u->dv.val, n * sz, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
             r = gb_fail(GrB_PANIC, &u->err, "GrB_Vector_dup: copy of the values failed");
-        if (r == GrB_SUCCESS && u->dpres && cudaMemcpyAsync(dpres, u->dpres, n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+        if (r == GrB_SUCCESS && u->dv.pres && cudaMemcpyAsync(o->dv.pres, u->dv.pres, n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
             r = gb_fail(GrB_PANIC, &u->err, "GrB_Vector_dup: copy of the presence failed");
-        if (r != GrB_SUCCESS) { delete o; return r; }
-        o->dval = dval.release(); o->dpres = dpres.release(); o->dev_valid = true; o->dev_nvals = u->dev_nvals;
+        if (r != GrB_SUCCESS) { delete o; return r; }      // frees what o was given
+        o->dv.valid = true; o->dev_nvals = u->dev_nvals;
     }
     *w = o; return GrB_SUCCESS;
 }
@@ -936,8 +933,8 @@ extern "C" GrB_Info GrB_Vector_nvals(GrB_Index *n, const GrB_Vector v) {
     if (!n) return gb_fail(GrB_NULL_POINTER, nullptr, "GrB_Vector_nvals: NULL"); GB_VECTOR_OK(v, "GrB_Vector_nvals");
     if (v->host_valid) { GB_TRY(vector_flush_pending(v)); *n = v->hi.size(); return GrB_SUCCESS; }
     if (v->dev_nvals < 0) {
-        if (!v->dpres) v->dev_nvals = (int64_t)v->n;
-        else { vector_join_import(v); GB_TRY(dev_count_present(v->dpres, (int64_t)v->n, &v->dev_nvals, &v->err)); }
+        if (!v->dv.pres) v->dev_nvals = (int64_t)v->n;
+        else { vector_join_import(v); GB_TRY(dev_count_present(v->dv.pres, (int64_t)v->n, &v->dev_nvals, &v->err)); }
     }
     *n = (GrB_Index)v->dev_nvals; return GrB_SUCCESS;
 }
@@ -969,7 +966,7 @@ extern "C" GrB_Info GrB_Vector_error(const char **error, const GrB_Vector v) {
 }
 static GrB_Info vector_host_writable(GrB_Vector v) {
     GB_TRY(vector_ensure_host(v));
-    if (v->dev_valid) vector_invalidate_device(v);
+    if (v->dv.valid) vector_invalidate_device(v);
     return GrB_SUCCESS;
 }
 static GrB_Info vector_set_element(GrB_Vector w, int src_tc, const void *x, GrB_Index i) {
@@ -1174,7 +1171,7 @@ extern "C" GrB_Info B200_Matrix_import_dense(GrB_Matrix *A, GrB_Type type, GrB_I
     if (r == GrB_SUCCESS && present) r = copy_in(pres, present, n, where, &m->err);
     if (r == GrB_SUCCESS && !where && cudaStreamSynchronize(G.stream) != cudaSuccess) r = GrB_PANIC;
     if (r != GrB_SUCCESS) { val.reset(); pres.reset(); GrB_Matrix_free(A); return r; }
-    matrix_adopt_dense(m, std::move(val), std::move(pres));
+    matrix_adopt_dense(m, DenseForm{std::move(val), std::move(pres)});
     return GrB_SUCCESS;
 }
 extern "C" GrB_Info B200_Matrix_export_dense(const GrB_Matrix A, void *x, uint8_t *present, int where) {
@@ -1206,11 +1203,13 @@ extern "C" GrB_Info B200_Vector_set_dense(GrB_Vector v, const void *x, const uin
     if (v->n > DEV_DIM_MAX) return gb_fail(GrB_INVALID_VALUE, &v->err, "vector size exceeds 2^31-1");
     const size_t sz = v->type->size, n = (size_t)v->n;
     if (where == 2) GB_TRY(vector_async_setup(v));
-    // a borrowed view (B200_Comm_result) gets buffers of its own: the communicator's region is neither written nor freed here
-    const bool fresh = v->borrowed || !v->dev_valid || !v->dval || (present && !v->dpres) || (!present && v->dpres);
-    if (v->borrowed || !v->dev_valid || !v->dval) { vector_invalidate_device(v); GB_TRY(dmalloc(&v->dval, n * sz + 16, &v->err)); }
-    if (present && !v->dpres) GB_TRY(dmalloc((void **)&v->dpres, n + 16, &v->err));
-    if (!present && v->dpres) { vector_join_copies(v); dfree(v->dpres); v->dpres = nullptr; }
+    // the buffers v owns are written in place; a borrowed view (B200_Comm_result) gets buffers of its own: the communicator's
+    // region is neither written nor freed here
+    const bool own = v->dv.valid && v->dv.val && !v->dv.val.borrowed();
+    const bool fresh = !own || (present && !v->dv.pres) || (!present && v->dv.pres);
+    if (!own) { vector_invalidate_device(v); GB_TRY(v->dv.val.alloc(n * sz + 16, &v->err)); }
+    if (present && !v->dv.pres) GB_TRY(v->dv.pres.alloc(n, &v->err));
+    if (!present && v->dv.pres) { vector_join_copies(v); v->dv.pres.reset(); }
     if (where == 2) {
         // pinned host memory, copied on the import stream so that it overlaps kernels already enqueued on the compute stream.
         // The copy may start once the last kernels that touch this vector are done (their event, recorded by the mxv / vxm that
@@ -1219,17 +1218,17 @@ extern "C" GrB_Info B200_Vector_set_dense(GrB_Vector v, const void *x, const uin
         if (v->use_recorded && !fresh) cudaStreamWaitEvent(G.h2d, v->ev_use, 0);
         else { cudaEventRecord(v->ev_use, G.stream); cudaStreamWaitEvent(G.h2d, v->ev_use, 0); }
         if (v->d2h_pending) cudaStreamWaitEvent(G.h2d, v->ev_d2h, 0);
-        CU_TRY(cudaMemcpyAsync(v->dval, x, n * sz, cudaMemcpyHostToDevice, G.h2d), &v->err);
-        if (present) CU_TRY(cudaMemcpyAsync(v->dpres, present, n, cudaMemcpyHostToDevice, G.h2d), &v->err);
+        CU_TRY(cudaMemcpyAsync(v->dv.val, x, n * sz, cudaMemcpyHostToDevice, G.h2d), &v->err);
+        if (present) CU_TRY(cudaMemcpyAsync(v->dv.pres, present, n, cudaMemcpyHostToDevice, G.h2d), &v->err);
         CU_TRY(cudaEventRecord(v->ev_h2d, G.h2d), &v->err);
         v->h2d_pending = true;
     } else {
         vector_join_copies(v);
-        GB_TRY(copy_in(v->dval, x, n * sz, where, &v->err));
-        if (present) GB_TRY(copy_in(v->dpres, present, n, where, &v->err));
+        GB_TRY(copy_in(v->dv.val, x, n * sz, where, &v->err));
+        if (present) GB_TRY(copy_in(v->dv.pres, present, n, where, &v->err));
     }
     v->use_recorded = false;       // this call wrote v: an earlier use no longer orders the next import
-    v->dev_valid = true; v->dev_nvals = present ? -1 : (int64_t)n;
+    v->dv.valid = true; v->dev_nvals = present ? -1 : (int64_t)n;
     v->hi.clear(); v->hx.clear(); v->pi.clear(); v->px.clear(); v->host_valid = false;
     return GrB_SUCCESS;
 }
@@ -1252,18 +1251,18 @@ extern "C" GrB_Info B200_Vector_export_dense(const GrB_Vector v, void *x, uint8_
         if (v->d2h_pending) cudaStreamWaitEvent(G.d2h, v->ev_d2h, 0);
         CU_TRY(cudaEventRecord(v->ev_d2h, G.stream), &v->err);
         CU_TRY(cudaStreamWaitEvent(G.d2h, v->ev_d2h, 0), &v->err);
-        if (x) CU_TRY(cudaMemcpyAsync(x, v->dval, n * sz, cudaMemcpyDeviceToHost, G.d2h), &v->err);
+        if (x) CU_TRY(cudaMemcpyAsync(x, v->dv.val, n * sz, cudaMemcpyDeviceToHost, G.d2h), &v->err);
         if (present) {
-            if (v->dpres) CU_TRY(cudaMemcpyAsync(present, v->dpres, n, cudaMemcpyDeviceToHost, G.d2h), &v->err);
+            if (v->dv.pres) CU_TRY(cudaMemcpyAsync(present, v->dv.pres, n, cudaMemcpyDeviceToHost, G.d2h), &v->err);
             else memset(present, 1, n);
         }
         CU_TRY(cudaEventRecord(v->ev_d2h, G.d2h), &v->err);
         v->d2h_pending = true;
         return GrB_SUCCESS;
     }
-    if (x) GB_TRY(copy_out(x, v->dval, n * sz, where, &v->err));
+    if (x) GB_TRY(copy_out(x, v->dv.val, n * sz, where, &v->err));
     if (present) {
-        if (v->dpres) GB_TRY(copy_out(present, v->dpres, n, where, &v->err));
+        if (v->dv.pres) GB_TRY(copy_out(present, v->dv.pres, n, where, &v->err));
         else if (where) CU_TRY(cudaMemsetAsync(present, 1, n, G.stream), &v->err);
         else memset(present, 1, n);
     }
@@ -1273,9 +1272,9 @@ extern "C" GrB_Info B200_Vector_export_dense(const GrB_Vector v, void *x, uint8_
 extern "C" GrB_Info B200_Vector_device_ptrs(GrB_Vector v, void **values, uint8_t **present) {
     GB_LOCK; GB_VECTOR_OK(v, "B200_Vector_device_ptrs");
     GB_TRY(vector_ensure_device(v));
-    if (values) *values = v->dval;
-    if (present) *present = v->dpres;
+    if (values) *values = v->dv.val;
+    if (present) *present = v->dv.pres;
     // the caller may write through these pointers: the host form is no longer authoritative
-    v->hi.clear(); v->hx.clear(); v->host_valid = false; if (v->dpres) v->dev_nvals = -1;
+    v->hi.clear(); v->hx.clear(); v->host_valid = false; if (v->dv.pres) v->dev_nvals = -1;
     return GrB_SUCCESS;
 }

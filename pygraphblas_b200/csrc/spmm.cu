@@ -351,21 +351,16 @@ static GrB_Info spmm_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Bi
             GB_TRY(matrix_ensure_device(C));
             GB_TRY(csr_to_dense(C->dev, C->type->size, cval, cpres, err));
         }
-        w.host_valid = false; w.dev_valid = true; w.borrowed = true; w.dev_nvals = -1;
-        w.dval = C->dn.valid ? C->dn.val.get() : cval.get(); w.dpres = C->dn.valid ? C->dn.pres.get() : cpres.get();
+        w.host_valid = false;
+        w.dv = C->dn.valid ? DenseForm::borrow(C->dn.val, C->dn.pres) : DenseForm::borrow(cval, cpres);
     }
     GB_Vector_opaque mv{};
     if (Mask) {
         mv.magic = GB_MAGIC; mv.type = Mask->type; mv.n = (uint64_t)(m * k); mv.host_valid = false;
-        mv.dval = Mask->dn.val; mv.dpres = Mask->dn.pres; mv.dev_valid = true; mv.dev_nvals = -1; mv.borrowed = true;
+        mv.dv = DenseForm::borrow(Mask->dn.val, Mask->dn.pres);
     }
-    void *tv = tval; uint8_t *tp = tpres;
-    const GrB_Info r = vector_write(&w, Mask ? &mv : nullptr, accum, f, tv, tp, zt, false, nullptr, std::move(tval), std::move(tpres));
-    if (!w.borrowed && w.dev_valid) {           // the write-back's result: C adopts it as its dense form
-        DevBuf<void> v; DevBuf<uint8_t> pr;
-        v.adopt(w.dval); pr.adopt(w.dpres);
-        matrix_adopt_dense(C, std::move(v), std::move(pr));
-    }
+    const GrB_Info r = vector_write(&w, Mask ? &mv : nullptr, accum, f, DenseForm{std::move(tval), std::move(tpres)}, zt, false, nullptr);
+    if (w.dv.valid && !w.dv.val.borrowed()) matrix_adopt_dense(C, std::move(w.dv));    // the write-back's result: C's dense form
     if (r != GrB_SUCCESS && !w.err.empty()) *err = w.err;
     return r;
 }

@@ -45,7 +45,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const int add = addop->opcode, mul = mulop->opcode;
     G.last_kernel.clear();
     if (!mask && f.mask_comp)      // w<!NULL>: nothing is let through, no product needed (vector_write clears w under REPLACE)
-        return vector_write(w, nullptr, accum, f, nullptr, nullptr, zt, false, nullptr);
+        return vector_write(w, nullptr, accum, f, DenseForm(), zt, false, nullptr);
 
     // ---- operands in HBM
     Csr *pc; GB_TRY(source_csr(A, use_transpose, &pc));
@@ -63,7 +63,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
                  mul == OP_LXOR || mul == OP_EQ || mul == OP_NE || mul == OP_ISEQ || mul == OP_ISNE)) kflip = false;     // commutative
     const bool need_a = kflip ? mul_reads_y(kmul) : mul_reads_x(kmul);
     const bool need_u = kflip ? mul_reads_x(kmul) : mul_reads_y(kmul);
-    const bool sparse_u = u->dpres != nullptr;
+    const bool sparse_u = u->dv.pres != nullptr;
     const bool fast_sr = !kflip && spmv_is_fast(xt, zt, add, kmul, false);      // a compile-time specialised semiring
     const bool fast = fast_sr && !sparse_u;
     const Tunables &tn = tunables();
@@ -73,12 +73,12 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     const bool wide = csr_wide(c);
 
     DevBuf<void> a_cast, u_cast;
-    const void *aval = c.val, *uval = u->dval;
+    const void *aval = c.val, *uval = u->dv.val;
     if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-    if (need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+    if (need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dv.val, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
     // run-time-operator kernels always read both operands: give them something readable of the right type
     if (!fast && !need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-    if (!fast && !need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+    if (!fast && !need_u && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dv.val, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
 
     const int64_t n = (int64_t)out_n;
     const size_t zsz = (size_t)tc_size(zt);
@@ -86,14 +86,14 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     // operand of this call, T is formed in place -- the iterated call `A.mxv(u, out=w)` then allocates nothing.
     void *tval = nullptr; uint8_t *tpres = nullptr;
     DevBuf<void> t_val; DevBuf<uint8_t> t_pres;      // T's own buffers when it is not formed in w's
-    const bool w_reusable = !need_final && w != u && w->dev_valid && w->dval && w->dpres && w->type->code == zt && !w->borrowed &&
-                            a_cast.get() != w->dval && u_cast.get() != w->dval;
+    const bool w_reusable = !need_final && w != u && w->dv.valid && w->dv.val && w->dv.pres && !w->dv.val.borrowed() &&
+                            w->type->code == zt && a_cast.get() != w->dv.val && u_cast.get() != w->dv.val;
     const bool in_place = w_reusable && (tn.mxv_inplace == 2 || (tn.mxv_inplace == 1 && !w->h2d_pending && !w->d2h_pending));
     if (in_place && tn.mxv_inplace == 2) {      // whatever the flags say: the kernels below start after w's last overlapped copies
         if (w->ev_h2d) { cudaStreamWaitEvent(G.stream, w->ev_h2d, 0); cudaStreamWaitEvent(G.stream, w->ev_d2h, 0); }
         w->h2d_pending = false; w->d2h_pending = false;
     }
-    if (in_place) { tval = w->dval; tpres = w->dpres; }
+    if (in_place) { tval = w->dv.val; tpres = w->dv.pres; }
     else {
         GB_TRY(t_val.alloc((size_t)n * zsz + 16, err));
         GB_TRY(t_pres.alloc((size_t)n, err));
@@ -106,13 +106,13 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
     if (use_pull) {
         // the run-time-operator kernel reads both operands: make sure both are of the operand type
         if (aval == c.val && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, c.val, A->type->code, c.nnz, err)); aval = a_cast; }
-        if (uval == u->dval && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dval, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
+        if (uval == u->dv.val && u->type->code != xt) { GB_TRY(dev_cast_values(u_cast, xt, u->dv.val, u->type->code, (int64_t)u->n, err)); uval = u_cast; }
         // few frontier edges: push along the rows of the other orientation (already in HBM) instead of pulling every row
         const Csr &o = use_transpose ? A->dev : A->devT;
         if (sparse_u && o.valid && (wide || o.rowptr32) && o.nnz == c.nnz && A->type->code == xt && !tn.no_push) {
             auto push = [&](auto &ps, const auto *rowptr) {
-                ps.rowptr = rowptr; ps.col = o.col; ps.aval = o.val; ps.nin = o.nrows; ps.uval = uval; ps.upres = u->dpres;
-                ps.mval = mask->dval; ps.mpres = mask->dpres; ps.mtc = mask->type->code; ps.mask_comp = f.mask_comp; ps.mask_struct = f.mask_struct;
+                ps.rowptr = rowptr; ps.col = o.col; ps.aval = o.val; ps.nin = o.nrows; ps.uval = uval; ps.upres = u->dv.pres;
+                ps.mval = mask->dv.val; ps.mpres = mask->dv.pres; ps.mtc = mask->type->code; ps.mask_comp = f.mask_comp; ps.mask_struct = f.mask_struct;
                 ps.tval = tval; ps.tpres = tpres; ps.nout = n; ps.add_op = add; ps.mul_op = kmul; ps.flip = kflip;
                 return spmv_masked_push_try(xt, zt, ps, c.nnz, &pushed, err);
             };
@@ -126,8 +126,8 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         GB_TRY(long_count.alloc(4, err));
         CU_TRY(cudaMemsetAsync(long_count, 0, sizeof(int), G.stream), err);
         auto pull = [&](auto &pa, const auto *rowptr) {
-            pa.rowptr = rowptr; pa.col = c.col; pa.aval = aval; pa.nrows = c.nrows; pa.uval = uval; pa.upres = u->dpres;
-            pa.mval = mask->dval; pa.mpres = mask->dpres; pa.mtc = mask->type->code; pa.mask_comp = f.mask_comp; pa.mask_struct = f.mask_struct;
+            pa.rowptr = rowptr; pa.col = c.col; pa.aval = aval; pa.nrows = c.nrows; pa.uval = uval; pa.upres = u->dv.pres;
+            pa.mval = mask->dv.val; pa.mpres = mask->dv.pres; pa.mtc = mask->type->code; pa.mask_comp = f.mask_comp; pa.mask_struct = f.mask_struct;
             pa.tval = tval; pa.tpres = tpres; pa.add_op = add; pa.mul_op = kmul; pa.flip = kflip;
             pa.long_cap = long_cap; pa.has_long = c.nnz > (int64_t)PULL_LONG; pa.long_rows = long_rows; pa.long_count = long_count;
             return spmv_masked_pull_dispatch(xt, zt, pa, err);
@@ -155,7 +155,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         ra.tail_row = rp.tail_row; ra.tail_last = rp.tail_last; ra.long_run = rp.long_run; ra.nlong = rp.nlong;
         ra.add_op = add; ra.mul_op = kmul; ra.flip = kflip;
         ra.head_val = rp.ws_head; ra.tail_val = rp.ws_tail;            // scratch kept with the plan (the library serialises calls)
-        if (sparse_u) { ra.upres = u->dpres; ra.tpres = tpres; ra.head_has = rp.ws_head_has; ra.tail_has = rp.ws_tail_has; }
+        if (sparse_u) { ra.upres = u->dv.pres; ra.tpres = tpres; ra.head_has = rp.ws_head_has; ra.tail_has = rp.ws_tail_has; }
         // hot-column table: on by default for large matrices whose gathers are concentrated (R-MAT-like);
         // B200GRB_SPMV_HOT=0 disables it, =<KB> caps the table size (and forces the kernel whatever the coverage)
         int hot_kb = tn.spmv_hot_kb >= 0 ? tn.spmv_hot_kb : 128;     // stage + table stay inside the 196 KB carve-out: the 228 KB one leaves no L1
@@ -204,7 +204,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         return GrB_SUCCESS;
     }
     // ---- w<mask> = accum(w, t)   (vector_ops.cu)
-    return vector_write(w, mask, accum, f, tval, tpres, zt, /*t_scalar=*/false, /*region=*/nullptr, std::move(t_val), std::move(t_pres));
+    return vector_write(w, mask, accum, f, DenseForm{std::move(t_val), std::move(t_pres)}, zt, /*t_scalar=*/false, /*region=*/nullptr);
 }
 
 // The value semiring the inner form runs on: the monoid of s, with FIRST (vxm) / SECOND (mxv) of the monoid's type
@@ -236,15 +236,15 @@ GrB_Info positional_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp 
         DevBuf<void> iota; DevBuf<uint8_t> pres;
         GB_TRY(iota.alloc((size_t)in_n * tc_size(zt) + 16, err));
         GB_TRY(pos_vector_values(iota, zt, nullptr, OP_ANY, (int64_t)in_n, false, ids_in, p.off, err));
-        const uint8_t *upres = u->dpres;
+        const uint8_t *upres = u->dv.pres;
         if (upres && w == u) {      // T may be formed in w's buffers: the kernels must not read the presence they write
             GB_TRY(pres.alloc((size_t)in_n, err));
             CU_TRY(cudaMemcpyAsync(pres, upres, (size_t)in_n, cudaMemcpyDeviceToDevice, G.stream), err);
             upres = pres;
         }
-        GB_Vector_opaque k{};      // u with the values k: borrows its buffers, never freed through the vector
+        GB_Vector_opaque k{};      // u with the values k
         k.magic = GB_MAGIC; k.type = s->add->op->ztype; k.n = in_n; k.host_valid = false;
-        k.dval = iota; k.dpres = (uint8_t *)upres; k.dev_valid = true; k.dev_nvals = u->dev_nvals; k.borrowed = true;
+        k.dv = DenseForm::borrow(iota, (uint8_t *)upres); k.dev_nvals = u->dev_nvals;
         GB_Semiring_opaque sr = value_semiring(s, vxm);
         GB_TRY(mxv_core(w, mask, accum, &sr, A, &k, f, use_transpose, vxm, fn));
         vector_mark_used(u);
@@ -262,16 +262,15 @@ GrB_Info positional_mxv(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp 
     // T = the values from the counts, with the counts' presence (its own copy: w may adopt T's buffers)
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     if (r == GrB_SUCCESS) r = tval.alloc((size_t)out_n * tc_size(zt) + 16, err);
-    if (r == GrB_SUCCESS) r = pos_vector_values(tval, zt, (const int64_t *)t->dval, add, (int64_t)out_n, zero, ids_out, p.off, err);
-    if (r == GrB_SUCCESS && t->dpres) {
+    if (r == GrB_SUCCESS) r = pos_vector_values(tval, zt, (const int64_t *)t->dv.val, add, (int64_t)out_n, zero, ids_out, p.off, err);
+    if (r == GrB_SUCCESS && t->dv.pres) {
         r = tpres.alloc((size_t)out_n, err);
-        if (r == GrB_SUCCESS && cudaMemcpyAsync(tpres, t->dpres, (size_t)out_n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
+        if (r == GrB_SUCCESS && cudaMemcpyAsync(tpres, t->dv.pres, (size_t)out_n, cudaMemcpyDeviceToDevice, G.stream) != cudaSuccess)
             r = gb_fail(GrB_PANIC, err, "%s: copy of the count presence failed", fn);
     }
     if (r == GrB_SUCCESS) {
         gb_kernel_used("positional=count");
-        void *tv = tval; uint8_t *tp = tpres;
-        r = vector_write(w, mask, accum, f, tv, tp, zt, false, nullptr, std::move(tval), std::move(tpres));
+        r = vector_write(w, mask, accum, f, DenseForm{std::move(tval), std::move(tpres)}, zt, false, nullptr);
     } else if (t->err.size()) *err = t->err;
     GrB_Vector_free(&t);
     return r;

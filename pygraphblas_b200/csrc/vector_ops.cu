@@ -120,29 +120,27 @@ static bool finalize_typed(const VecFinalizeArgs &g) {
 }
 
 GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const DescFlags &f,
-                      const void *tval, const uint8_t *tpres, int ttc, bool t_scalar, const uint8_t *region,
-                      DevBuf<void> &&own_val, DevBuf<uint8_t> &&own_pres) {
+                      DenseForm &&T, int ttc, bool t_scalar, const uint8_t *region) {
     std::string *err = &w->err;
     const int64_t n = (int64_t)w->n;
     const int wtc = w->type->code;
     if (!mask && f.mask_comp) {
         // w<!NULL>: the complement of "no mask" lets nothing through -- w keeps its entries, or loses all of
         // them under GrB_REPLACE (GraphBLAS C API 1.3 section 4.3; SuiteSparse's quick-mask exit)
-        own_val.reset(); own_pres.reset();
         if (f.replace) {
             vector_invalidate_device(w);
             w->hi.clear(); w->hx.clear(); w->pi.clear(); w->px.clear(); w->host_valid = true;
         }
         return GrB_SUCCESS;
     }
-    const bool need_final = mask != nullptr || accum != nullptr || region != nullptr || t_scalar || !own_val;
+    const bool need_final = mask != nullptr || accum != nullptr || region != nullptr || t_scalar || T.val.borrowed();
     if (!need_final) {      // w takes T's buffers
         if (wtc != ttc) {
             DevBuf<void> cv;
-            GB_TRY(dev_cast_values(cv, wtc, tval, ttc, n, err));
-            own_val = std::move(cv);
+            GB_TRY(dev_cast_values(cv, wtc, T.val, ttc, n, err));
+            T.val = std::move(cv);
         }
-        vector_adopt_device(w, own_val.release(), own_pres.release());
+        vector_adopt_device(w, std::move(T));
         CU_TRY(cudaGetLastError(), err);
         return GrB_SUCCESS;
     }
@@ -150,26 +148,25 @@ GrB_Info vector_write(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp ac
     if (!w_empty) GB_TRY(vector_ensure_device(w));
     if (mask) GB_TRY(vector_ensure_device(mask));
     VecFinalizeArgs fa{};
-    fa.n = n; fa.wval = w->dval; fa.wpres = w->dpres; fa.wtc = wtc; fa.w_exists = w_empty ? 0 : 1;
-    fa.tval = tval; fa.tpres = tpres; fa.ttc = ttc; fa.t_scalar = t_scalar ? 1 : 0;
-    if (mask) { fa.mval = mask->dval; fa.mpres = mask->dpres; fa.mtc = mask->type->code; fa.has_mask = 1; }
+    fa.n = n; fa.wval = w->dv.val; fa.wpres = w->dv.pres; fa.wtc = wtc; fa.w_exists = w_empty ? 0 : 1;
+    fa.tval = T.val; fa.tpres = T.pres; fa.ttc = ttc; fa.t_scalar = t_scalar ? 1 : 0;
+    if (mask) { fa.mval = mask->dv.val; fa.mpres = mask->dv.pres; fa.mtc = mask->type->code; fa.has_mask = 1; }
     fa.mask_comp = f.mask_comp; fa.mask_struct = f.mask_struct; fa.replace = f.replace;
     fa.accum_op = accum ? accum->opcode : -1;
     fa.accum_tc = accum ? accum->xtype->code : 0; fa.accum_ztc = accum ? accum->ztype->code : 0;
     fa.region = region;
-    DevBuf<void> oval; DevBuf<uint8_t> opres;
-    GB_TRY(oval.alloc((size_t)n * tc_size(wtc) + 16, err));
-    fa.oval = oval;
+    DenseForm out;
+    GB_TRY(out.val.alloc((size_t)n * tc_size(wtc) + 16, err));
+    fa.oval = out.val;
     // a full w stays full under an accumulator (and a mask that does not replace), and a full T over the whole
     // vector without a mask gives a full result: no presence bytes, and the next mxv sees a dense operand
     // (SSSP: v = min(v, A' min.+ v))
-    const bool w_full = !w_empty && w->dpres == nullptr;
-    const bool out_full = (w_full && !(mask && f.replace) && (accum != nullptr || (region != nullptr && tpres == nullptr))) ||
-                          (tpres == nullptr && !mask && !region);
-    if (!out_full) { GB_TRY(opres.alloc((size_t)n, err)); fa.opres = opres; }
+    const bool w_full = !w_empty && !w->dv.pres;
+    const bool out_full = (w_full && !(mask && f.replace) && (accum != nullptr || (region != nullptr && !T.pres))) ||
+                          (!T.pres && !mask && !region);
+    if (!out_full) { GB_TRY(out.pres.alloc((size_t)n, err)); fa.opres = out.pres; }
     if (!finalize_typed(fa)) { vec_finalize_kernel<<<grid_for(n), 256, 0, G.stream>>>(fa); GB_LAUNCHED(); }
-    own_val.reset(); own_pres.reset();
-    vector_adopt_device(w, oval.release(), opres.release());
+    vector_adopt_device(w, std::move(out));
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
@@ -229,14 +226,14 @@ static GrB_Info vec_ewise(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     const int64_t n = (int64_t)w->n;
     EwiseArgs a{};
     a.n = n; a.mode = mode; a.op = op->opcode; a.xtc = op->xtype->code; a.ztc = op->ztype->code;
-    a.uval = u->dval; a.upres = u->dpres; a.utc = u->type->code; a.vval = v->dval; a.vpres = v->dpres; a.vtc = v->type->code;
+    a.uval = u->dv.val; a.upres = u->dv.pres; a.utc = u->type->code; a.vval = v->dv.val; a.vpres = v->dv.pres; a.vtc = v->type->code;
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     GB_TRY(tval.alloc((size_t)n * tc_size(a.ztc) + 16, &w->err));
-    const bool t_full = mode == EW_ADD ? (!u->dpres || !v->dpres) : (!u->dpres && !v->dpres);
+    const bool t_full = mode == EW_ADD ? (!u->dv.pres || !v->dv.pres) : (!u->dv.pres && !v->dv.pres);
     if (!t_full) GB_TRY(tpres.alloc((size_t)n, &w->err));
     a.tval = tval; a.tpres = tpres;
     vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED();
-    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, a.ztc, false, nullptr, std::move(tval), std::move(tpres));
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, a.ztc, false, nullptr);
 }
 extern "C" GrB_Info GrB_Vector_eWiseAdd_BinaryOp(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_BinaryOp op,
                                                   const GrB_Vector u, const GrB_Vector v, const GrB_Descriptor desc) {
@@ -287,18 +284,18 @@ static GrB_Info vec_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryO
     const int64_t n = (int64_t)w->n;
     EwiseArgs a{};
     a.n = n; a.mode = mode; a.op = opcode; a.xtc = xtc; a.ztc = ztc; a.scalar = scalar;
-    a.uval = u->dval; a.upres = u->dpres; a.utc = u->type->code;
+    a.uval = u->dv.val; a.upres = u->dv.pres; a.utc = u->type->code;
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     GB_TRY(tval.alloc((size_t)n * tc_size(ztc) + 16, &w->err));
-    if (u->dpres) GB_TRY(tpres.alloc((size_t)n, &w->err));
+    if (u->dv.pres) GB_TRY(tpres.alloc((size_t)n, &w->err));
     a.tval = tval; a.tpres = tpres;
     if (mode == EW_UNARY ? uop_is_positional(opcode) : op_is_positional(opcode)) {
         // a vector is a column: position k is (k, 0), so the row operators give k and the column ones 0; T keeps u's presence
         const PosOp p = mode == EW_UNARY ? pos_unop(opcode) : pos_binop(opcode);
         GB_TRY(pos_vector_values(tval, ztc, nullptr, OP_ANY, n, p.col, nullptr, p.off, &w->err));
-        if (u->dpres) CU_TRY(cudaMemcpyAsync(tpres, u->dpres, (size_t)n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
+        if (u->dv.pres) CU_TRY(cudaMemcpyAsync(tpres, u->dv.pres, (size_t)n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
     } else { vec_ewise_kernel<<<grid_for(n), 256, 0, G.stream>>>(a); GB_LAUNCHED(); }
-    return vector_write(w, mask, accum, desc_flags(desc), a.tval, a.tpres, ztc, false, nullptr, std::move(tval), std::move(tpres));
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, ztc, false, nullptr);
 }
 extern "C" GrB_Info GrB_Vector_apply(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_UnaryOp op, const GrB_Vector u, const GrB_Descriptor desc) {
     GB_LOCK; GB_CHECK_INIT;
@@ -399,7 +396,7 @@ static GrB_Info vec_assign_scalar(GrB_Vector w, const GrB_Vector mask, const GrB
             region_mark_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), region); GB_LAUNCHED();
         }
     }
-    return vector_write(w, mask, accum, desc_flags(desc), tval, nullptr, wtc, true, region, std::move(tval));
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval)}, wtc, true, region);
 }
 
 extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Vector u, const GrB_Index *I, GrB_Index ni,
@@ -420,7 +417,7 @@ extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const
     const int utc = u->type->code;
     if (all) {
         if (w == u && !mask && !accum) return GrB_SUCCESS;
-        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr);
+        return vector_write(w, mask, accum, desc_flags(desc), DenseForm::borrow(u->dv.val, u->dv.pres), utc, false, nullptr);
     }
     DevBuf<void> tval; DevBuf<uint8_t> tpres, region;
     const size_t n = (size_t)w->n;
@@ -432,9 +429,9 @@ extern "C" GrB_Info GrB_Vector_assign(GrB_Vector w, const GrB_Vector mask, const
     if (!idx.empty()) {
         DevBuf<uint64_t> didx;
         GB_TRY(upload_indices(idx, didx, &w->err));
-        vec_scatter_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres, region); GB_LAUNCHED();
+        vec_scatter_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dv.val, u->dv.pres, utc, tval, tpres, region); GB_LAUNCHED();
     }
-    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, region, std::move(tval), std::move(tpres));
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, utc, false, region);
 }
 
 extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp accum, const GrB_Vector u, const GrB_Index *I, GrB_Index ni,
@@ -452,12 +449,12 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
         const size_t n = (size_t)w->n, sz = (size_t)tc_size(u->type->code);
         DevBuf<void> tval; DevBuf<uint8_t> tpres;
         GB_TRY(tval.alloc(n * sz + 16, &w->err));
-        CU_TRY(cudaMemcpyAsync(tval, (const uint8_t *)u->dval + (size_t)I[0] * sz, n * sz, cudaMemcpyDeviceToDevice, G.stream), &w->err);
-        if (u->dpres) {
+        CU_TRY(cudaMemcpyAsync(tval, (const uint8_t *)u->dv.val + (size_t)I[0] * sz, n * sz, cudaMemcpyDeviceToDevice, G.stream), &w->err);
+        if (u->dv.pres) {
             GB_TRY(tpres.alloc(n, &w->err));
-            CU_TRY(cudaMemcpyAsync(tpres, u->dpres + I[0], n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
+            CU_TRY(cudaMemcpyAsync(tpres, u->dv.pres + I[0], n, cudaMemcpyDeviceToDevice, G.stream), &w->err);
         }
-        return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, u->type->code, false, nullptr, std::move(tval), std::move(tpres));
+        return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, u->type->code, false, nullptr);
     }
     bool all; std::vector<uint64_t> idx;
     GB_TRY(index_list(I, ni, u->n, &all, idx, &w->err, fn));
@@ -468,7 +465,7 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
     const int utc = u->type->code;
     if (all) {
         if (w == u && !mask && !accum) return GrB_SUCCESS;
-        return vector_write(w, mask, accum, desc_flags(desc), u->dval, u->dpres, utc, false, nullptr);
+        return vector_write(w, mask, accum, desc_flags(desc), DenseForm::borrow(u->dv.val, u->dv.pres), utc, false, nullptr);
     }
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     const size_t n = (size_t)w->n;
@@ -477,9 +474,9 @@ extern "C" GrB_Info GrB_Vector_extract(GrB_Vector w, const GrB_Vector mask, cons
     if (!idx.empty()) {
         DevBuf<uint64_t> didx;
         GB_TRY(upload_indices(idx, didx, &w->err));
-        vec_gather_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dval, u->dpres, utc, tval, tpres); GB_LAUNCHED();
+        vec_gather_u_kernel<<<grid_for((int64_t)idx.size()), 256, 0, G.stream>>>(didx, (int64_t)idx.size(), u->dv.val, u->dv.pres, utc, tval, tpres); GB_LAUNCHED();
     }
-    return vector_write(w, mask, accum, desc_flags(desc), tval, tpres, utc, false, nullptr, std::move(tval), std::move(tpres));
+    return vector_write(w, mask, accum, desc_flags(desc), DenseForm{std::move(tval), std::move(tpres)}, utc, false, nullptr);
 }
 
 // ------------------------------------------------------------------ reduce to a scalar
@@ -541,7 +538,7 @@ static GrB_Info vec_reduce(void *c, int ctc, const GrB_BinaryOp accum, const GrB
     GB_TRY(vector_ensure_device(u));
     const int mtc = op->ztype->code;
     Sc r; bool rh = false;
-    GB_TRY(dev_reduce_values(u->dval, u->dpres, u->type->code, (int64_t)u->n, op->opcode, mtc, &r, &rh, &u->err));
+    GB_TRY(dev_reduce_values(u->dv.val, u->dv.pres, u->type->code, (int64_t)u->n, op->opcode, mtc, &r, &rh, &u->err));
     const Sc acc = rh ? r : sc_monoid_identity(op->opcode, mtc);
     Sc out = sc_cast(acc, mtc, ctc);
     if (accum) {

@@ -213,6 +213,7 @@ def test_vector_ops():
     _sweep(mk, lambda u, v: u.eadd(v, INT64.PLUS), _vec_model(pa | pb, np.where(pa & pb, a + b, np.where(pa, a, b))))
     _sweep(mk, lambda u, v: u.apply(INT64.AINV), _vec_model(pa, -a))
     _sweep(mk, lambda u, v: u.extract(idx.tolist()), _vec_model(pa[idx], a[idx]))
+    _sweep(mk, lambda u, v: v.dup(), _vec_model(pb, b))                   # v is device-only: the copy is made on the device
 
     def reduced(ref):
         assert int(ref[0]) == int(a[pa].sum())
@@ -304,6 +305,103 @@ def test_matrix_ops():
         return A.select(">", 4, out=C, mask=M, accum=INT64.MAX)
     _sweep(lambda: (_mat_lists(S, INT64), _mat(Cs, INT64), Matrix.from_csr(Ms.indptr, Ms.indices, mval, *Ms.shape, BOOL)),
            select_accum, _same_csr(sp.csr_matrix(Dsel)))
+
+
+@pytest.mark.parametrize("where", [0, 1])
+@pytest.mark.parametrize("pres", ["added", "dropped"])
+def test_set_dense_into_device_vector(pres, where):
+    """B200_Vector_set_dense into a vector that has a device form of its own: the values are written into its buffer, and a
+    presence buffer is allocated (added) or dropped."""
+    rng = np.random.default_rng(10)
+    n = 3000
+    x0, x = rng.integers(1, 9, n).astype(np.int64), rng.integers(1, 9, n).astype(np.int64)
+    p = rng.random(n) < 0.5
+    old_p, new_p = (None, p) if pres == "added" else (p, None)
+    src = [x, None if new_p is None else new_p.astype(np.uint8)]
+    if where == 1:
+        import torch
+        src = [None if s is None else torch.from_numpy(s).cuda() for s in src]
+        torch.cuda.synchronize()
+        addr = lambda s: s.data_ptr()
+    else:
+        addr = lambda s: s.ctypes.data
+
+    def call(v):
+        gb.base._check(lib.B200_Vector_set_dense(v._vector[0], ffi.cast("void*", addr(src[0])),
+                                                 ffi.NULL if src[1] is None else ffi.cast("uint8_t*", addr(src[1])), where))
+        return v
+    _sweep(lambda: (Vector.from_numpy(x0, old_p),), call, _vec_model(np.ones(n, bool) if new_p is None else new_p, x))
+
+
+@pytest.mark.parametrize("c_form", ["dense", "csr"])
+def test_spmm_dense_write_under_accum(c_form):
+    """mxm on the SpMM route into a non-empty C under an accumulator and no mask: the write-back borrows C's dense form, or
+    the dense image of a CSR C, and C adopts the result as its dense form.  MAX leaves a repeated call's result as it is."""
+    rng = np.random.default_rng(11)
+    S = _rand_csr(rng, 400, 300, 0.02, np.float32)
+    x = rng.integers(1, 5, (300, 8)).astype(np.float32)
+    c = rng.integers(1, 60, (400, 8)).astype(np.float32)
+    nonempty = np.diff(S.indptr) > 0
+    want = np.where(nonempty[:, None], np.maximum(c, S.astype(np.float64) @ x.astype(np.float64)), c)
+    make_c = (lambda: Matrix.from_numpy(c)) if c_form == "dense" else (lambda: _mat(sp.csr_matrix(c), FP32))
+
+    def call(A, X, C):
+        A.mxm(X, semiring=FP32.PLUS_TIMES, out=C, accum=FP32.MAX)
+        kernels = ffi.string(lib.B200_debug_last_kernel()).decode()
+        assert "spmm" in kernels and "write=dense" in kernels, kernels
+        return C
+    _sweep(lambda: (_mat(S, FP32), Matrix.from_numpy(x), make_c()), call, _same_csr(sp.csr_matrix(want)))
+
+
+def test_positional_mxv_inner_in_place():
+    """Positional mxv in its inner form with w = u: the product runs on a stack vector that borrows the iota of k and a copy
+    of u's presence, and T is formed in u's own buffers."""
+    rng = np.random.default_rng(12)
+    n = 500
+    S = _rand_csr(rng, n, n, 0.01, np.float32)
+    pu = rng.random(n) < 0.5
+    u0 = rng.integers(1, 9, n).astype(np.int64)
+
+    def call(A, u):
+        w = u.dup()
+        A.mxv(w, semiring=INT64.MIN_SECONDI, out=w)
+        kernels = ffi.string(lib.B200_debug_last_kernel()).decode()
+        assert "positional=inner" in kernels and "mxv=in-place" in kernels, kernels
+        return w
+
+    def check(ref):
+        I, X = ref
+        ks = [S.indices[S.indptr[i]:S.indptr[i + 1]] for i in range(n)]
+        ks = [k[pu[k]] for k in ks]                      # w(i) = min k over A(i, k) and u(k) both present
+        rows = [i for i in range(n) if len(ks[i])]
+        assert np.array_equal(I, rows) and np.array_equal(X, [ks[i].min() for i in rows])
+    _sweep(lambda: (_mat(S, FP32), Vector.from_numpy(u0, pu)), call, check)
+
+
+@pytest.mark.parametrize("use", ["output", "set_dense"])
+def test_comm_view_hand_overs(use):
+    """A world-1 communicator's result view as the output of an operation (under an accumulator: the view's region is read,
+    then the view owns the result) and as the target of B200_Vector_set_dense (the view gets buffers of its own).  Freeing
+    the communicator frees what the view came to own, and nothing else."""
+    from pygraphblas_b200.distributed import Comm
+    rng = np.random.default_rng(13)
+    n = 1000
+    a, b = rng.integers(1, 9, n).astype(np.int64), rng.integers(1, 9, n).astype(np.int64)
+    pa, pb = rng.random(n) < 0.6, rng.random(n) < 0.6
+
+    def make():
+        comm = Comm(n, INT64, rank=0, world=1)
+        return comm, comm.allgather(Vector.from_numpy(a, pa), 0), Vector.from_numpy(b, pb)
+
+    if use == "output":
+        call = lambda comm, view, v: v.apply(INT64.AINV, out=view, accum=INT64.MIN)
+        model = _vec_model(pa | pb, np.where(pa & pb, np.minimum(a, -b), np.where(pa, a, -b)))
+    else:
+        def call(comm, view, v):
+            view.set_numpy(b, pb)
+            return view
+        model = _vec_model(pb, b)
+    _sweep(make, call, model)
 
 
 @pytest.mark.parametrize("kind", ["row", "matrix"])

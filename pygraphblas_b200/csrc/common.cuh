@@ -103,7 +103,6 @@ public:
 // run plan (spmv_run.cu, warp-independent kernels): entries cut into warp-sized runs of 256
 struct RunPlan {
     DevBuf<uint32_t> headw;          // [ceil(nnz/32)] bit q = entry q starts a row
-    DevBuf<uint16_t> lane;           // [nruns*32] row starts inside the run before the lane's first entry
     DevBuf<uint32_t> base;           // [nruns+1] row starts before the run (= rank of its first row start)
     DevBuf<int32_t> tail_row;        // [nruns] row still open at the end of the run (its last row start), or -1
     DevBuf<uint32_t> tail_last;      // [nruns] last run that row reaches
@@ -120,7 +119,8 @@ struct RunPlan {
 // hot-column plan (spmv_run.cu): the henc most referenced columns get their rank as id, the others col + henc
 struct HotPlan {
     DevBuf<uint32_t> perm;           // [henc] hot rank -> original column
-    DevBuf<uint32_t> col;            // [nnz] encoded column ids
+    DevBuf<void> col;                // encoded column ids: 3-byte ids packed run by run ([nruns] x 768 bytes), or [nnz] x 4 bytes
+    int id_bytes = 4;                // 3 when every encoded id is below 2^24 - 1 (ncols + henc < 2^24), else 4
     DevBuf<void> ws_uhot;            // [henc + 256] x 8 bytes: u at the hot columns, in the tier layout of the launch (spmv_args.cuh)
     uint32_t henc = 0;               // ids below this are hot ranks
     bool planned = false;            // the plan was attempted (col stays NULL when the gathers are not concentrated)

@@ -136,7 +136,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         if (!pushed) GB_TRY(wide ? pull(paw, c.rowptr.get()) : pull(pa, c.rowptr32.get()));
     }
     const char *kernel_name = "pull";
-    int hot_cluster = 0, hot_ctas = 0; uint32_t hot_t0 = 0, hot_t1 = 0, hot_henc = 0;      // cluster size, grid and tiers of the hot-table launch
+    int hot_cluster = 0, hot_ctas = 0, hot_ids = 0; uint32_t hot_t0 = 0, hot_t1 = 0, hot_henc = 0;      // cluster size, grid, id width, tiers of the hot-table launch
     if (use_pull) {
         if (pushed) kernel_name = "push";
     } else if (c.nnz == 0) {
@@ -150,7 +150,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         GB_TRY(spmv_run_plan(c, err));
         RunArgs ra{};
         const RunPlan &rp = c.run;
-        ra.col = c.col; ra.aval = aval; ra.uval = uval; ra.headw = rp.headw; ra.lane_rank = rp.lane; ra.run_base = rp.base;
+        ra.col = c.col; ra.aval = aval; ra.uval = uval; ra.headw = rp.headw; ra.run_base = rp.base;
         ra.nzrow = rp.nzrow; ra.rowptr = c.rowptr32; ra.nruns = rp.nruns; ra.nnz = c.nnz; ra.tval = tval;
         ra.tail_row = rp.tail_row; ra.tail_last = rp.tail_last; ra.long_run = rp.long_run; ra.nlong = rp.nlong;
         ra.add_op = add; ra.mul_op = kmul; ra.flip = kflip;
@@ -166,7 +166,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         Hot2Args hot{};
         if (hot_kb > 0) {
             // the launch runs the prep kernel first: u at the hot columns, T cleared, T's presence from the plan
-            ra.col = c.hot.col;
+            hot.col = c.hot.col; hot.id_bytes = c.hot.id_bytes;
             hot.u_hot = c.hot.ws_uhot; hot.hperm = c.hot.perm; hot.henc = c.hot.henc; hot.u = uval; hot.vsize = tc_size(xt);
             hot.tval = tval; hot.tval_bytes = (size_t)n * zsz; hot.pres_tmpl = rp.pres_tmpl; hot.tpres = tpres; hot.nrows = c.nrows;
             hot.want_cluster = 1;
@@ -181,7 +181,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         }
         const bool ok = fast_sr ? spmv_run_dispatch(xt, add, kmul, ra, hot_kb > 0 ? &hot : nullptr, (size_t)hot_kb << 10) : spmv_run_generic(xt, zt, ra);
         if (!ok) return gb_fail(GrB_PANIC, err, "mxv: internal dispatch error");
-        if (hot_kb > 0) { hot_cluster = hot.cluster; hot_ctas = hot.ctas; hot_t0 = hot.t0; hot_t1 = hot.t1; hot_henc = hot.henc; }
+        if (hot_kb > 0) { hot_cluster = hot.cluster; hot_ctas = hot.ctas; hot_t0 = hot.t0; hot_t1 = hot.t1; hot_henc = hot.henc; hot_ids = hot.id_bytes * 8; }
     }
     gb_kernel_used(kernel_name);
     if (wide) gb_kernel_used("offsets=64");
@@ -190,6 +190,7 @@ static GrB_Info mxv_core(GrB_Vector w, const GrB_Vector mask, const GrB_BinaryOp
         gb_kernel_used(("hot-cluster=" + std::to_string(hot_cluster)).c_str());
         gb_kernel_used(("hot-ctas=" + std::to_string(hot_ctas)).c_str());
         gb_kernel_used(("hot-tiers=" + std::to_string(hot_t0) + "," + std::to_string(hot_t1) + "," + std::to_string(hot_henc)).c_str());
+        gb_kernel_used(("ids=" + std::to_string(hot_ids)).c_str());
         if (burble.on) { hot_note = std::string(kernel_name) + " cluster " + std::to_string(hot_cluster) + ", T0 " + std::to_string(hot_t0); kernel_name = hot_note.c_str(); }
     }
     if (burble.on && wide) { hot_note = std::string(kernel_name) + ", 64-bit offsets"; kernel_name = hot_note.c_str(); }

@@ -5,7 +5,7 @@
 static constexpr int RUN = 256;
 struct RunArgs {
     const uint32_t *col; const void *aval; const void *uval;
-    const uint32_t *headw; const uint16_t *lane_rank; const uint32_t *run_base; const uint32_t *nzrow; const uint32_t *rowptr;
+    const uint32_t *headw; const uint32_t *run_base; const uint32_t *nzrow; const uint32_t *rowptr;
     const int32_t *tail_row; const uint32_t *tail_last;       // structural: which row is open at a run's end, how far it reaches
     int64_t nruns; int64_t nnz;
     void *tval;
@@ -25,7 +25,12 @@ constexpr int FIX_BATCH = 8;
 // table tiers, runs the prep kernel and the hot-table kernel, and fills in the layout and the cluster size it used.
 // u_hot layout: [T0 ranks, replicated in every CTA | slice 0 | ... | slice C-1 (S entries each) | ranks T0+T1 .. henc-1]
 // hot rank T0 + k (k < T1) lives in slice k mod C at index k / C, in the shared memory of the cluster's CTA k mod C.
+// Encoded column ids of 3 bytes (HotPlan::id_bytes = 3) are stored run by run, HOT_IDS3_RUN bytes per run: the 256 low
+// 16-bit halves, then the 256 high bytes; the last run is padded with the id henc.
+constexpr int HOT_IDS3_RUN = RUN * 3;
 struct Hot2Args {
+    const void *col;          // the plan's encoded column ids, id_bytes (3: packed by run, 4: one word per entry) each
+    int id_bytes;
     void *u_hot;              // the plan's u_hot buffer (written by the prep kernel)
     const uint32_t *hperm;    // [henc] column of each hot rank
     const void *u; int vsize; // u and its value size (prep kernel)

@@ -17,17 +17,15 @@ __global__ void plan_rows_kernel(const OT *rowptr, const int64_t *rank, int64_t 
         if (rowptr[r + 1] > rs) { nzrow[rank[r]] = (uint32_t)r; atomicOr(&headw[rs >> 5], 1u << (rs & 31)); }
     }
 }
-__global__ void plan_runs_kernel(const uint32_t *headw, int64_t nruns, int64_t nwords, uint16_t *lane_rank, int64_t *run_cnt) {
+// row starts per run (a lane's rank inside its run is counted by the run kernels themselves: spmv_run_gather)
+__global__ void plan_runs_kernel(const uint32_t *headw, int64_t nruns, int64_t nwords, int64_t *run_cnt) {
     const int lane = threadIdx.x & 31;
     const int64_t run = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (run >= nruns) return;
     const int64_t w = run * 8 + (lane >> 2);
-    const uint32_t hw = w < nwords ? headw[w] : 0u;
-    const int pc = __popc((hw >> ((lane & 3) * 8)) & 0xffu);
-    int inc = pc;
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    lane_rank[run * 32 + lane] = (uint16_t)(inc - pc);
-    if (lane == 31) run_cnt[run] = inc;
+    const uint32_t hw = (w < nwords && (lane & 3) == 0) ? headw[w] : 0u;
+    const int cnt = (int)__reduce_add_sync(0xffffffffu, (unsigned)__popc(hw));
+    if (lane == 0) run_cnt[run] = cnt;
 }
 __global__ void plan_base_kernel(const int64_t *scan, int64_t nruns, uint32_t *run_base) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k <= nruns; k += (int64_t)gridDim.x * blockDim.x) run_base[k] = (uint32_t)scan[k];
@@ -65,7 +63,6 @@ template <typename OT> static GrB_Info spmv_run_plan_t(Csr &c, const OT *rowptr,
     GB_TRY(cnt.alloc((size_t)p.nruns + 1, err));
     GB_TRY(p.pres_tmpl.alloc((size_t)c.nrows, err));
     GB_TRY(p.headw.alloc((size_t)nwords + 8, err));
-    GB_TRY(p.lane.alloc((size_t)p.nruns * 32, err));
     GB_TRY(p.base.alloc((size_t)p.nruns + 1, err));
     GB_TRY(p.tail_row.alloc((size_t)p.nruns, err));
     GB_TRY(p.tail_last.alloc((size_t)p.nruns, err));
@@ -80,7 +77,7 @@ template <typename OT> static GrB_Info spmv_run_plan_t(Csr &c, const OT *rowptr,
     GB_TRY(p.nzrow.alloc((size_t)nz, err));
     plan_rows_kernel<OT><<<grid_for(c.nrows), 256, 0, G.stream>>>(rowptr, flag, c.nrows, p.nzrow, p.headw); GB_LAUNCHED();
     CU_TRY(cudaMemsetAsync(cnt + p.nruns, 0, 8, G.stream), err);
-    plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, p.lane, cnt); GB_LAUNCHED();
+    plan_runs_kernel<<<(unsigned)ceil_div(p.nruns * 32, 256), 256, 0, G.stream>>>(p.headw, p.nruns, nwords, cnt); GB_LAUNCHED();
     GB_TRY(dev_exclusive_scan(cnt, p.nruns + 1, err));
     plan_base_kernel<<<grid_for(p.nruns + 1), 256, 0, G.stream>>>(cnt, p.nruns, p.base); GB_LAUNCHED();
     plan_tails_kernel<OT><<<grid_for(p.nruns), 256, 0, G.stream>>>(p.base, p.nzrow, rowptr, p.nruns, p.tail_row, p.tail_last, cnt); GB_LAUNCHED();
@@ -141,6 +138,17 @@ __global__ void hot_encode_kernel(const uint32_t *col, const uint32_t *inv, int6
         out[k] = r < henc ? r : c + henc;
     }
 }
+// the same ids in 3 bytes, packed run by run (spmv_args.cuh, HOT_IDS3_RUN): the slots of the last run past nnz hold henc
+__global__ void hot_encode3_kernel(const uint32_t *col, const uint32_t *inv, int64_t nnz, int64_t nslots, uint32_t henc, uint8_t *out) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nslots; k += (int64_t)gridDim.x * blockDim.x) {
+        uint32_t id = henc;
+        if (k < nnz) { const uint32_t c = col[k], r = inv[c]; id = r < henc ? r : c + henc; }
+        uint8_t *run = out + (k / RUN) * HOT_IDS3_RUN;
+        const int j = (int)(k % RUN);
+        reinterpret_cast<uint16_t *>(run)[j] = (uint16_t)id;
+        run[RUN * 2 + j] = (uint8_t)(id >> 16);
+    }
+}
 
 GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
     if (c.hot.planned) return GrB_SUCCESS;
@@ -169,11 +177,19 @@ GrB_Info spmv_hot_plan(Csr &c, std::string *err) {
     p.planned = true;
     if (h[0] >= 16) {
         p.henc = (uint32_t)h[2];
+        // 3-byte ids when the largest, ncols - 1 + henc, stays below 2^24 - 1: the kernel's stage guard relies on no id being
+        // all ones (spmv_run_hot2_kernel)
+        p.id_bytes = n + (int64_t)p.henc < ((int64_t)1 << 24) ? 3 : 4;
+        const int64_t nruns = ceil_div(c.nnz, RUN);
         GB_TRY(p.perm.alloc((size_t)p.henc, err));
-        GB_TRY(p.col.alloc((size_t)c.nnz, err));
+        GB_TRY(p.col.alloc(p.id_bytes == 3 ? (size_t)nruns * HOT_IDS3_RUN : (size_t)c.nnz * 4 + 16, err));
         GB_TRY(p.ws_uhot.alloc(((size_t)p.henc + 256) * 8 + 16, err));      // + the unused tail of the last slices (< 16 per CTA)
         CU_TRY(cudaMemcpyAsync(p.perm, perm, (size_t)p.henc * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-        hot_encode_kernel<<<grid_for(c.nnz, 256, 32), 256, 0, G.stream>>>(c.col, inv, c.nnz, p.henc, p.col); GB_LAUNCHED();
+        if (p.id_bytes == 3)
+            hot_encode3_kernel<<<grid_for(nruns * RUN, 256, 32), 256, 0, G.stream>>>(c.col, inv, c.nnz, nruns * RUN, p.henc, (uint8_t *)p.col);
+        else
+            hot_encode_kernel<<<grid_for(c.nnz, 256, 32), 256, 0, G.stream>>>(c.col, inv, c.nnz, p.henc, (uint32_t *)p.col);
+        GB_LAUNCHED();
     }
     CU_TRY(cudaGetLastError(), err);
     c.hot = std::move(p);

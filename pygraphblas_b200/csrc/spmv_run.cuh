@@ -11,7 +11,7 @@
 // The entries are cut into runs of 256 (one warp, 8 consecutive entries per lane).  A cached plan gives
 // every lane where its rows start, so that no lane has to find them out at call time:
 //   run_headw   one bit per entry: "this entry starts a row"
-//   run_base    number of row starts before the run;  run_lane: row starts inside the run before the lane
+//   run_base    number of row starts before the run (a lane adds those of the lanes before it: a warp scan of the bit counts)
 //   nzrow       ids of the non-empty rows (row start rank -> row id);  pres_tmpl: the output's presence
 // so a warp needs no shared memory and no barrier: stream 8 entries, gather, fold between the row-start
 // bits (rows inside a lane are final), one segmented suffix scan over the 32 lanes, and the two partial
@@ -34,7 +34,12 @@ __device__ __forceinline__ void spmv_run_gather(const RunArgs &p, const int64_t 
     const XT *uval = static_cast<const XT *>(p.uval);
     const uint32_t hw = nvalid > 0 ? __ldg(p.headw + (q >> 5)) : 0u;
     L.hb = (hw >> ((lane & 3) * 8)) & 0xffu;                               // this lane's 8 row-start bits
-    L.rank = __ldg(p.run_base + run) + __ldg(p.lane_rank + run * 32 + lane);   // row starts before this lane's first entry
+    // row starts before this lane's first entry: the run's, then the lanes' before it (exclusive scan of the bit counts)
+    const uint32_t pc = __popc(L.hb);
+    uint32_t inc = pc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+    L.rank = __ldg(p.run_base + run) + (inc - pc);
     L.nvalid = nvalid;
     if (SPARSE) {
         // u has holes: a product exists only where u(col) does; the values are fetched only for those
@@ -166,7 +171,9 @@ __global__ void __launch_bounds__(256) spmv_run_kernel(const RunArgs p) {
 //     stage before the next copy is issued).  A warp is its own producer and consumer: no CTA barrier after
 //     the table is in.
 // Column ids are ENCODED by the cached plan: id < henc -> rank among the hottest columns; id >= henc -> original column
-// + henc, gathered from u itself.  u needs no permutation.
+// + henc, gathered from u itself.  u needs no permutation.  When every id fits 24 bits (ncols + henc < 2^24) the plan stores
+// them in 3 bytes, packed run by run (HOT_IDS3_RUN), and a run's ids take 768 instead of 1024 bytes of stream and stage;
+// the kernel holds both bodies (the id width is a template parameter of spmv_run_hot2_body) and runs the one of the plan.
 // The kernel runs as thread-block clusters of C CTAs (C = 1: plain CTAs), and the hot ranks fall in tiers:
 //   id < T0        the replicated tier, in every CTA's own table: LDS;
 //   id < T0 + T1   the distributed tier: rank T0 + k sits in the table of the cluster's CTA k mod C (index k / C), read
@@ -211,13 +218,16 @@ template <typename XT> __device__ __forceinline__ XT ld_dsmem(uint32_t saddr, ui
     else { uint16_t v; asm("ld.shared::cluster.u8 %0, [%1];" : "=h"(v) : "r"(a)); return (XT)(uint8_t)v; }
 }
 
-template <typename XT> __host__ __device__ constexpr int hot2_stage_bytes(bool need_a) { return RUN * 4 + (need_a ? RUN * (int)sizeof(XT) : 0); }
+// a warp's stage: the ids of one run (id_bytes 3 or 4 each), then its values when the multiply reads them
+template <typename XT> __host__ __device__ constexpr int hot2_stage_bytes(bool need_a, int id_bytes) {
+    return RUN * id_bytes + (need_a ? RUN * (int)sizeof(XT) : 0);
+}
 constexpr int HOT2_WARPS = 32;
 
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const RunArgs p, const Hot2Args h) {
+template <typename XT, typename ZT, int ADD, int MUL, int IDB>
+__device__ __forceinline__ void spmv_run_hot2_body(const RunArgs &p, const Hot2Args &h) {
     constexpr bool NEED_A = mul_reads_x(MUL);
-    constexpr int STAGE = hot2_stage_bytes<XT>(NEED_A);
+    constexpr int STAGE = hot2_stage_bytes<XT>(NEED_A, IDB);
     extern __shared__ __align__(128) unsigned char smem_raw[];
     // layout: [warp stages][mbarriers][hot table]
     unsigned char *s_stage = smem_raw;
@@ -233,11 +243,12 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         const int64_t q = r * RUN;
         const int64_t left = p.nnz - q;
         const uint32_t cnt = (uint32_t)(left < RUN ? left : RUN);
-        const uint32_t cb = (cnt * 4u + 15u) & ~15u;                                      // arrays are padded by >= 16 bytes
+        // 3-byte ids: every run, the last one too, is HOT_IDS3_RUN bytes; 4-byte ids: the arrays are padded by >= 16 bytes
+        const uint32_t cb = IDB == 3 ? (uint32_t)HOT_IDS3_RUN : (cnt * 4u + 15u) & ~15u;
         const uint32_t ab = NEED_A ? ((cnt * (uint32_t)sizeof(XT) + 15u) & ~15u) : 0u;
         mbar_expect_tx(bar, cb + ab);
-        tma_bulk_g2s(stage, p.col + q, cb, bar);
-        if (NEED_A) tma_bulk_g2s(stage + RUN * 4, static_cast<const XT *>(p.aval) + q, ab, bar);
+        tma_bulk_g2s(stage, static_cast<const unsigned char *>(h.col) + r * (RUN * IDB), cb, bar);
+        if (NEED_A) tma_bulk_g2s(stage + RUN * IDB, static_cast<const XT *>(p.aval) + q, ab, bar);
     };
 
     const uint32_t t0 = h.t0, t1 = h.t1, slice = h.slice, henc = h.henc;
@@ -282,7 +293,7 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
         const int nvalid = (int)min((int64_t)8, max((int64_t)0, p.nnz - q));
         uint32_t c[8];
         if (NEED_A) {
-            const XT *sa = reinterpret_cast<const XT *>(stage + RUN * 4) + lane * 8;
+            const XT *sa = reinterpret_cast<const XT *>(stage + RUN * IDB) + lane * 8;
             if constexpr (sizeof(XT) == 4) {
                 const uint4 a0 = reinterpret_cast<const uint4 *>(sa)[0], a1 = reinterpret_cast<const uint4 *>(sa)[1];
                 const uint32_t w[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -293,16 +304,32 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
                 for (int j = 0; j < 8; ++j) L.a[j] = sa[j];
             }
         }
-        const uint4 *sc = reinterpret_cast<const uint4 *>(stage) + lane * 2;
-        const uint4 c0 = sc[0], c1 = sc[1];
-        c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
         // WAR guard of the stage.  The bulk copy of the next run writes this stage through the async proxy; nothing orders it
         // after generic-proxy loads that were only ISSUED (a __syncwarp does not wait for their data), and under load a
         // shared-memory load can sit in the LSU queue longer than an L2-hit bulk copy takes -- a lane then folds words of the
         // NEXT run into this run's rows (seen as one wrong hub-row sum in ~1 % of the launches of the overlapped e2e loop).  A vote
-        // that READS the first and last loaded word of every lane cannot issue before the warp's loads have written their
-        // registers; its predicate is never true (encoded ids stay below 2^32 - 1: spmv_hot_plan), so the copy is always issued.
-        uint32_t guard = c[0] & c[7];
+        // that READS words of every id load and the first and last value word of every lane cannot issue before the warp's
+        // loads have written their registers; its predicate is never true, so the copy is always issued.
+        uint32_t guard;
+        if constexpr (IDB == 3) {
+            // the lane's 8 low halves (16 bytes) and 8 high bytes (8 bytes); id j = low half j | high byte j << 16
+            const uint4 lo = reinterpret_cast<const uint4 *>(stage)[lane];
+            const uint2 hi = reinterpret_cast<const uint2 *>(stage + RUN * 2)[lane];
+            const uint32_t h01 = __byte_perm(hi.x, 0u, 0x4140), h23 = __byte_perm(hi.x, 0u, 0x4342);   // high bytes j, j+1 -> bits 0, 16
+            const uint32_t h45 = __byte_perm(hi.y, 0u, 0x4140), h67 = __byte_perm(hi.y, 0u, 0x4342);
+            c[0] = __byte_perm(lo.x, h01, 0x5410); c[1] = __byte_perm(lo.x, h01, 0x7632);
+            c[2] = __byte_perm(lo.y, h23, 0x5410); c[3] = __byte_perm(lo.y, h23, 0x7632);
+            c[4] = __byte_perm(lo.z, h45, 0x5410); c[5] = __byte_perm(lo.z, h45, 0x7632);
+            c[6] = __byte_perm(lo.w, h67, 0x5410); c[7] = __byte_perm(lo.w, h67, 0x7632);
+            // all ones in lo.x and hi.x would make id 0 of the lane 2^24 - 1, which no id reaches (spmv_hot_plan); the raw
+            // words, not the decoded ids, whose top byte the compiler knows to be zero
+            guard = lo.x & lo.w & hi.x & hi.y;
+        } else {
+            const uint4 *sc = reinterpret_cast<const uint4 *>(stage) + lane * 2;
+            const uint4 c0 = sc[0], c1 = sc[1];
+            c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
+            guard = c[0] & c[7];                                            // encoded ids stay below 2^32 - 1: spmv_hot_plan
+        }
         if (NEED_A) {                                                       // the value loads take part too (first and last word of the lane)
             uint32_t w0, w7;
             if constexpr (sizeof(XT) >= 4) { memcpy(&w0, &L.a[0], 4); memcpy(&w7, &L.a[7], 4); }
@@ -319,6 +346,13 @@ __global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const
     };
     for (; run < p.nruns; run += stride) { fetch(run, cur); spmv_run_fold<XT, ZT, ADD, MUL, false>(p, run, lane, cur); }
     cluster_sync_all();                       // no peer reads this CTA's table any more
+}
+
+// one kernel per semiring; the plan's id width picks the body (uniform over the grid)
+template <typename XT, typename ZT, int ADD, int MUL>
+__global__ void __launch_bounds__(HOT2_WARPS * 32, 1) spmv_run_hot2_kernel(const RunArgs p, const Hot2Args h) {
+    if (h.id_bytes == 3) spmv_run_hot2_body<XT, ZT, ADD, MUL, 3>(p, h);
+    else spmv_run_hot2_body<XT, ZT, ADD, MUL, 4>(p, h);
 }
 
 // rows that continue past their run: tail partial (+) head partials of the following runs.  Every run after `run` up to
@@ -390,10 +424,10 @@ __global__ void __launch_bounds__(256) spmv_run_fixup_kernel(const RunArgs p) {
 static inline unsigned fixup_ctas(const RunArgs &a) { return (unsigned)((a.nlong + 7) / 8 + ceil_div(a.nruns, 256)); }
 
 // shared memory the hot-table kernel can use for its table, after the warp stages and barriers
-template <typename XT> static inline uint32_t hot2_table_entries(bool need_a, uint32_t henc, size_t limit_bytes) {
+template <typename XT> static inline uint32_t hot2_table_entries(bool need_a, int id_bytes, uint32_t henc, size_t limit_bytes) {
     static int max_optin = 0;                   // one device per process: ask once
     if (!max_optin) cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, G.device);
-    const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(need_a) + (HOT2_WARPS + 1) * 8 + 8;
+    const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(need_a, id_bytes) + (HOT2_WARPS + 1) * 8 + 8;
     size_t avail = (size_t)max_optin > fixed + 256 ? (size_t)max_optin - fixed - 256 : 0;
     avail = std::min(avail, limit_bytes);
     return (uint32_t)std::min<size_t>(henc, avail / sizeof(XT)) & ~15u;
@@ -433,8 +467,8 @@ template <typename XT, typename ZT, int ADD, int MUL>
 static void hot2_launch(const RunArgs &a, Hot2Args &h, size_t table_limit) {
     constexpr bool NEED_A = mul_reads_x(MUL);
     auto kernel = spmv_run_hot2_kernel<XT, ZT, ADD, MUL>;
-    const uint32_t cap = hot2_table_entries<XT>(NEED_A, h.henc, table_limit);
-    const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(NEED_A) + (HOT2_WARPS + 1) * 8 + 8;
+    const uint32_t cap = hot2_table_entries<XT>(NEED_A, h.id_bytes, h.henc, table_limit);
+    const size_t fixed = (size_t)HOT2_WARPS * hot2_stage_bytes<XT>(NEED_A, h.id_bytes) + (HOT2_WARPS + 1) * 8 + 8;
     const size_t smem_max = fixed + (size_t)cap * sizeof(XT);
     // the dynamic shared-memory limit of a kernel is raised once per size (a driver call per launch is host time the
     // multi-GPU step cannot hide: its kernels take tens of microseconds)

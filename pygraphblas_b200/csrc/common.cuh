@@ -209,13 +209,16 @@ struct GBGlobal {
     int burble = 0;
     cudaEvent_t burble_e0 = nullptr, burble_e1 = nullptr;
     std::string last_kernel;      // kernel paths of the last GrB_mxv / GrB_vxm / GrB_mxm, separated by ';' (B200_debug_last_kernel)
-    int64_t debug_wide = 0;       // B200_debug_wide: > 0 puts every mxv / vxm / transpose and the SpMM, dense-left and SDDMM
-                                  // routes of mxm on the wide route; transposes and SDDMM masks go in chunks of this many entries
+    int64_t debug_wide = 0;       // B200_debug_wide: > 0 puts every mxv / vxm / transpose, the SpMM, dense-left and SDDMM routes
+                                  // of mxm and its masked CSR x CSR methods (not complemented) on the wide route; transposes and
+                                  // SDDMM masks go in chunks of this many entries, masked products in row panels of at most this
+                                  // many entries of A and of M (a longer row makes a panel of its own)
     std::recursive_mutex mu;
 };
 extern GBGlobal G;
 static inline void gb_kernel_used(const char *k) { if (!G.last_kernel.empty()) G.last_kernel += ';'; G.last_kernel += k; }
-// the wide route of mxv / vxm and of the dense-operand mxm (DESIGN.md sections 3.1 and 3.6): 64-bit entry offsets, for a CSR
+// the wide route of mxv / vxm, of the dense-operand mxm and of the masked CSR x CSR mxm (DESIGN.md sections 3.1, 3.2 and 3.6):
+// 64-bit entry offsets, for a CSR
 // without rowptr32 (nnz >= 2^32), and for every CSR while B200_debug_wide is on
 static inline bool csr_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide > 0; }
 // entries per chunk of the wide route's chunked passes (the transpose, the mask of SDDMM): 2^27, or B200_debug_wide's chunk,
@@ -269,7 +272,7 @@ struct GbBurble {
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
 enum WsSlot : int { WS_WORDS = 0, WS_FOUND, WS_FLOPS, WS_TOTAL, WS_CS, WS_CM, WS_CL, WS_C1, WS_SROW, WS_SIDX, WS_SCNT, WS_MROW, WS_MIDX, WS_MCNT,
                     WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW,
-                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_COUNT };
+                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_PANEL_A, WS_PANEL_M, WS_COUNT };
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh = nullptr);
 template <typename T> static inline GrB_Info ws_array(int slot, T **p, size_t count, std::string *err, bool *fresh = nullptr) {
     return ws_get(slot, (void **)p, count * sizeof(T) + 16, err, fresh);

@@ -100,9 +100,11 @@ template <typename ZT> __device__ __forceinline__ void atomic_combine(typename S
 // the low bits would only permute the low bits of c and cluster structured column ids
 __device__ __forceinline__ uint32_t hash_col(uint32_t c, int shift) { return (c * 2654435761u) >> shift; }
 
-struct GemmArgs {
+// BT: the type of B's row offsets (uint32_t: rowptr32; int64_t: rowptr, the wide route of the masked methods).  A's and M's
+// offsets stay 32-bit: the wide route hands the kernels row panels of A and M with offsets rebased to the panel.
+template <typename BT> struct GemmArgsT {
     const uint32_t *a_ptr, *a_col; const void *a_val;
-    const uint32_t *b_ptr, *b_col; const void *b_val;
+    const BT *b_ptr; const uint32_t *b_col; const void *b_val;
     const uint32_t *m_ptr, *m_col; const void *m_val; int m_tc; int m_struct;   // mask (masked kernels)
     int64_t nrows, ncols;
     const int32_t *rows; int64_t nbin;          // rows of this bin
@@ -115,9 +117,11 @@ struct GemmArgs {
     // dense accumulator workspace (one slice per CTA)
     uint32_t *spa_bits; void *spa_val; int64_t spa_words; unsigned int *queue;
 };
+typedef GemmArgsT<uint32_t> GemmArgs;
 
 // ------------------------------------------------------------------ flop count + binning
-__global__ void flops_kernel(const uint32_t *a_ptr, const uint32_t *a_col, const uint32_t *b_ptr, int64_t nrows,
+template <typename BT>
+__global__ void flops_kernel(const uint32_t *a_ptr, const uint32_t *a_col, const BT *b_ptr, int64_t nrows,
                              int64_t *flops, unsigned long long *total) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -618,37 +622,37 @@ template <typename W> __global__ void fill_words_kernel(W *a, W v, int64_t n) {
 // The warp handles 32 A entries at a time: each lane fetches one (k, B row range) up front, the ranges are broadcast by
 // shuffle and the lanes stride the B row -- the dependent-load chain per A entry is paid once per 32 entries.
 // Heavier rows are cut into chunks and go to the streaming kernel (spgemm_stream.cuh).
-struct MaskedArgs {
-    GemmArgs g;
+template <typename BT> struct MaskedArgsT {
+    GemmArgsT<BT> g;
     void *t_words;     // nnz(M) accumulator words
 };
 
-template <typename XT, typename ZT, typename Hit>
-__device__ __forceinline__ void stream_b_rows(const GemmArgs &p, uint32_t pa0, uint32_t pa1, int lane, Hit &&hit) {
+template <typename XT, typename ZT, typename BT, typename Hit>
+__device__ __forceinline__ void stream_b_rows(const GemmArgsT<BT> &p, uint32_t pa0, uint32_t pa1, int lane, Hit &&hit) {
     const XT *aval = static_cast<const XT *>(p.a_val);
     for (uint32_t base = pa0; base < pa1; base += 32) {
         const uint32_t pa = base + lane;
         const bool valid = pa < pa1;
         const uint32_t k = valid ? __ldg(p.a_col + pa) : 0u;
-        const uint32_t bs = valid ? __ldg(p.b_ptr + k) : 0u, be = valid ? __ldg(p.b_ptr + k + 1) : 0u;
+        const BT bs = valid ? __ldg(p.b_ptr + k) : (BT)0, be = valid ? __ldg(p.b_ptr + k + 1) : (BT)0;
         XT av = (XT)1;
         if (p.need_a && valid) av = gload<XT>(aval + pa);
         const int cnt = min(32u, pa1 - base);
         for (int l = 0; l < cnt; ++l) {
-            const uint32_t s = __shfl_sync(0xffffffffu, bs, l), e = __shfl_sync(0xffffffffu, be, l);
+            const BT s = __shfl_sync(0xffffffffu, bs, l), e = __shfl_sync(0xffffffffu, be, l);
             XT a;
             if constexpr (sizeof(XT) == 8) { long long t = __shfl_sync(0xffffffffu, reinterpret_cast<long long &>(av), l); a = reinterpret_cast<XT &>(t); }
             else if constexpr (sizeof(XT) == 4) { int t = __shfl_sync(0xffffffffu, reinterpret_cast<int &>(av), l); a = reinterpret_cast<XT &>(t); }
             else { int t = __shfl_sync(0xffffffffu, (int)av, l); a = (XT)t; }
-            for (uint32_t pb = s + lane; pb < e; pb += 32) hit(__ldg(p.b_col + pb), a, pb);
+            for (BT pb = s + lane; pb < e; pb += 32) hit(__ldg(p.b_col + pb), a, pb);
         }
     }
 }
 
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgs ma) {
+template <typename XT, typename ZT, int ADD, int MUL, typename BT>
+__global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgsT<BT> ma) {
     typedef typename SlotWord<ZT>::W W;
-    const GemmArgs &p = ma.g;
+    const GemmArgsT<BT> &p = ma.g;
     extern __shared__ unsigned char smem_raw[];
     const int add = ADD >= 0 ? ADD : p.add_op;
     const int mul = MUL >= 0 ? MUL : p.mul_op;
@@ -683,7 +687,7 @@ __global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgs ma) {
     }
     __syncwarp();
     const XT *bval = static_cast<const XT *>(p.b_val);
-    auto hit = [&](uint32_t j, XT av, uint32_t pb) {
+    auto hit = [&](uint32_t j, XT av, BT pb) {
         uint32_t s = hash_col(j, hshift);
         while (true) {
             const uint32_t kk = keys[s];
@@ -698,7 +702,7 @@ __global__ void __launch_bounds__(256) masked_hash_kernel(const MaskedArgs ma) {
             s = (s + 1) & tmask;
         }
     };
-    stream_b_rows<XT, ZT>(p, p.a_ptr[row], p.a_ptr[row + 1], lane, hit);
+    stream_b_rows<XT, ZT, BT>(p, p.a_ptr[row], p.a_ptr[row + 1], lane, hit);
     __syncwarp();
     W *tw = static_cast<W *>(ma.t_words);
     for (int q = lane; q < mlen; q += 32) { tw[ms + q] = vals[q]; p.t_found[ms + q] = found[q]; }
@@ -750,8 +754,8 @@ __global__ void row_len_kernel(const uint32_t *ptr, int64_t n, int64_t *out) {
 
 // ------------------------------------------------------------------ masked dot:  T(i,j) = A(i,:) . B(j,:) for (i,j) in M
 // One warp per mask row; lanes take mask entries; sorted-merge intersection of the two rows.
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(256) masked_dot_kernel(const GemmArgs p) {
+template <typename XT, typename ZT, int ADD, int MUL, typename BT>
+__global__ void __launch_bounds__(256) masked_dot_kernel(const GemmArgsT<BT> p) {
     const int add = ADD >= 0 ? ADD : p.add_op;
     const int mul = MUL >= 0 ? MUL : p.mul_op;
     const XT *aval = static_cast<const XT *>(p.a_val), *bval = static_cast<const XT *>(p.b_val);
@@ -768,7 +772,7 @@ __global__ void __launch_bounds__(256) masked_dot_kernel(const GemmArgs p) {
             ZT acc = ident; uint8_t has = 0;
             if (on) {
                 const uint32_t j = p.m_col[q];
-                uint32_t x = as, y = p.b_ptr[j]; const uint32_t ye = p.b_ptr[j + 1];
+                uint32_t x = as; BT y = p.b_ptr[j]; const BT ye = p.b_ptr[j + 1];
                 while (x < ae && y < ye) {
                     const uint32_t cx = __ldg(p.a_col + x), cy = __ldg(p.b_col + y);
                     if (cx == cy) {
@@ -1047,7 +1051,7 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
         DevBuf<int64_t> flops; DevBuf<unsigned long long> total;
         GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
         CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
-        flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
+        flops_kernel<uint32_t><<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
         GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
         int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
         G.last_flops = (uint64_t)total_flops;
@@ -1157,36 +1161,46 @@ struct PhaseTrace {
     }
 };
 
-static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt,
-                              int add, int mul, bool need_a, bool need_b, const Csr &M, int mtc, bool m_struct,
-                              bool dot, Csr &T, std::string *err) {
-    const int64_t nrows = A.nrows, ncols = dot ? B.nrows : B.ncols;
-    T = Csr(); T.nrows = nrows; T.ncols = ncols;
+// One row panel of a masked product: nrows rows of A and M, with 32-bit offsets relative to the panel's first entries (the
+// narrow route: the whole matrices, their rowptr32)
+struct MaskedPanel {
+    const uint32_t *a_ptr, *a_col; const void *a_val;
+    const uint32_t *m_ptr, *m_col; const void *m_val;
+    int64_t nrows, mnnz;
+};
+// the methods a masked call ran: reported once each, in the same order, however many panels ran them
+struct MaskedUse { bool dot = false, warp = false, cls[3] = {false, false, false}, exact[3] = {false, false, false}; };
+
+// The masked methods on one panel: the accumulator word and the found flag of each of its mask entries, in the workspace
+// (*tval, *tfound; 1- and 2-byte types are narrowed into `typed`).  BT: the type of B's row offsets.
+template <typename BT>
+static GrB_Info masked_panel(const MaskedPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
+                             bool need_a, bool need_b, int mtc, bool m_struct, bool dot, int64_t ncols, PhaseTrace &trace,
+                             MaskedUse &use, void **tval, uint8_t **tfound, DevBuf<void> &typed, std::string *err) {
+    const int64_t nrows = P.nrows;
     const size_t zsz = (size_t)tc_size(zt), wsize = zsz == 8 ? 8 : 4;
-    MaskedArgs ma{};
-    GemmArgs &g = ma.g;
-    g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
-    g.m_ptr = M.rowptr32; g.m_col = M.col; g.m_val = M.val; g.m_tc = mtc; g.m_struct = m_struct;
+    MaskedArgsT<BT> ma{};
+    GemmArgsT<BT> &g = ma.g;
+    g.a_ptr = P.a_ptr; g.a_col = P.a_col; g.a_val = P.a_val; g.b_ptr = b_ptr; g.b_col = B.col; g.b_val = bval;
+    g.m_ptr = P.m_ptr; g.m_col = P.m_col; g.m_val = P.m_val; g.m_tc = mtc; g.m_struct = m_struct;
     g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
-    PhaseTrace trace;
-    DevBuf<void> typed;                                        // 1- and 2-byte types: the accumulator words narrowed
     void *words = nullptr; uint8_t *found = nullptr;          // per mask entry: accumulator word, "has a value"
-    GB_TRY(ws_get(WS_WORDS, &words, (size_t)M.nnz * wsize + 16, err));
-    GB_TRY(ws_get(WS_FOUND, (void **)&found, (size_t)M.nnz + 16, err));
+    GB_TRY(ws_get(WS_WORDS, &words, (size_t)P.mnnz * wsize + 16, err));
+    GB_TRY(ws_get(WS_FOUND, (void **)&found, (size_t)P.mnnz + 16, err));
     g.c_val = words; g.t_found = found; ma.t_words = words;
-    G.last_flops = 0;
-    if (M.nnz > 0 && dot) {
+    *tval = words; *tfound = found;
+    if (P.mnnz > 0 && dot) {
         // the dot kernel writes typed values directly
-#define K_DOT(XT, ZT, A_, M_) masked_dot_kernel<XT, ZT, A_, M_><<<grid_for(nrows * 32), 256, 0, G.stream>>>(g)
-        GB_FOR_SEMIRING(xt, zt, add, mul, K_DOT, err); GB_LAUNCHED(); gb_kernel_used("dot");
-    } else if (M.nnz > 0) {
+#define K_DOT(XT, ZT, A_, M_) masked_dot_kernel<XT, ZT, A_, M_, BT><<<grid_for(nrows * 32), 256, 0, G.stream>>>(g)
+        GB_FOR_SEMIRING(xt, zt, add, mul, K_DOT, err); GB_LAUNCHED(); use.dot = true;
+    } else if (P.mnnz > 0) {
         int64_t *flops = nullptr; unsigned long long *total = nullptr;
         GB_TRY(ws_array(WS_FLOPS, &flops, (size_t)nrows, err)); GB_TRY(ws_array(WS_TOTAL, &total, 1, err));
         CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
-        flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
+        flops_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(P.a_ptr, P.a_col, b_ptr, nrows, flops, total); GB_LAUNCHED();
         // accumulators start at accum_init, flags at 0
-        CU_TRY(cudaMemsetAsync(found, 0, (size_t)M.nnz, G.stream), err);
-#define K_IDENT(XT, ZT, A_, M_) fill_accum_init<ZT>(words, M.nnz, (A_) >= 0 ? (A_) : add)
+        CU_TRY(cudaMemsetAsync(found, 0, (size_t)P.mnnz, G.stream), err);
+#define K_IDENT(XT, ZT, A_, M_) fill_accum_init<ZT>(words, P.mnnz, (A_) >= 0 ? (A_) : add)
         GB_FOR_SEMIRING(xt, zt, add, mul, K_IDENT, err); GB_LAUNCHED();
         // classify rows and cut heavy ones into flop-bounded chunks
         int64_t *cs = nullptr, *cm = nullptr, *cl = nullptr, *c1 = nullptr;
@@ -1195,7 +1209,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
         CU_TRY(cudaMemsetAsync(cs + nrows, 0, 8, G.stream), err);
         CU_TRY(cudaMemsetAsync(cm + nrows, 0, 8, G.stream), err); CU_TRY(cudaMemsetAsync(cl + nrows, 0, 8, G.stream), err);
         CU_TRY(cudaMemsetAsync(c1 + nrows, 0, 8, G.stream), err);
-        chunk_count_kernel<<<grid_for(nrows), 256, 0, G.stream>>>(flops, M.rowptr32, nrows, CHUNK_FLOPS, WARP_FLOPS, SMALL_TABLE / 2,
+        chunk_count_kernel<<<grid_for(nrows), 256, 0, G.stream>>>(flops, P.m_ptr, nrows, CHUNK_FLOPS, WARP_FLOPS, SMALL_TABLE / 2,
                                                                   MIDSMALL_TABLE / 2, MEDIUM_TABLE / 2, cs, cm, cl, c1); GB_LAUNCHED();
         GB_TRY(dev_exclusive_scan(cs, nrows + 1, err));
         GB_TRY(dev_exclusive_scan(cm, nrows + 1, err)); GB_TRY(dev_exclusive_scan(cl, nrows + 1, err)); GB_TRY(dev_exclusive_scan(c1, nrows + 1, err));
@@ -1203,7 +1217,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
         GB_TRY(read_i64(cs + nrows, &n_small, err));
         GB_TRY(read_i64(cm + nrows, &n_medium, err)); GB_TRY(read_i64(cl + nrows, &n_long, err)); GB_TRY(read_i64(c1 + nrows, &n_warp, err));
         GB_TRY(read_i64((const int64_t *)total, &tf, err));
-        G.last_flops = (uint64_t)tf;
+        G.last_flops += (uint64_t)tf;
         int32_t *s_row = nullptr, *m_row = nullptr, *l_row = nullptr, *w_rows = nullptr;
         uint32_t *s_idx = nullptr, *s_cnt = nullptr, *m_idx = nullptr, *m_cnt = nullptr, *l_idx = nullptr, *l_cnt = nullptr;
         GB_TRY(ws_array(WS_SROW, &s_row, (size_t)n_small, err)); GB_TRY(ws_array(WS_SIDX, &s_idx, (size_t)n_small, err)); GB_TRY(ws_array(WS_SCNT, &s_cnt, (size_t)n_small, err));
@@ -1215,8 +1229,8 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
         if (n_warp) {
             g.rows = w_rows; g.nbin = n_warp; g.table = SMALL_TABLE;
             const size_t sm = masked_smem(SMALL_TABLE, 8, wsize);
-#define K_MSMALL(XT, ZT, A_, M_) masked_hash_kernel<XT, ZT, A_, M_><<<(unsigned)ceil_div(n_warp, 8), 256, sm, G.stream>>>(ma)
-            GB_FOR_SEMIRING(xt, zt, add, mul, K_MSMALL, err); GB_LAUNCHED(); gb_kernel_used("masked-warp");
+#define K_MSMALL(XT, ZT, A_, M_) masked_hash_kernel<XT, ZT, A_, M_, BT><<<(unsigned)ceil_div(n_warp, 8), 256, sm, G.stream>>>(ma)
+            GB_FOR_SEMIRING(xt, zt, add, mul, K_MSMALL, err); GB_LAUNCHED(); use.warp = true;
         }
         // chunked classes: the streaming kernel (spgemm_stream.cuh), persistent CTAs over blocks of consecutive chunks
         {
@@ -1228,7 +1242,7 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
             // exact bitmap a stray id there would read shared memory out of range: those positions must hold valid ids (0).
             if (B.nnz % 4 && (n_small || n_medium || n_long))
                 CU_TRY(cudaMemsetAsync(B.col.get() + B.nnz, 0, (size_t)(4 - B.nnz % 4) * sizeof(uint32_t), G.stream), err);
-            StreamArgs sa{}; sa.g = g; sa.t_words = words;
+            StreamArgsT<BT> sa{}; sa.g = g; sa.t_words = words;
             struct Cls { int64_t n; const int32_t *row; const uint32_t *idx, *cnt; int nt, bm_log2, vals_cap, grab; };
             const Cls cls[3] = {{n_small, s_row, s_idx, s_cnt, 256, 14, MIDSMALL_TABLE / 2, 8},
                                 {n_medium, m_row, m_idx, m_cnt, 256, 16, MEDIUM_TABLE / 2, 4},
@@ -1251,50 +1265,188 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
                 }
 #define K_MSTREAM(XT, ZT, A_, M_) do { \
                 const int nt = big ? 1024 : 256; \
-                const size_t sm = sm_var + stream_fixed_smem<XT>(nt); \
-                auto kern = masked_stream_kernel<XT, ZT, A_, M_>; \
+                const size_t sm = sm_var + stream_fixed_smem<XT, BT>(nt); \
+                auto kern = masked_stream_kernel<XT, ZT, A_, M_, BT>; \
                 cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm); \
                 int ctas = ctas_big; \
                 if (!big) { int per_sm = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, sm); \
                             ctas = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(sa.nchunks, sa.grab), (int64_t)G.num_sms * std::max(per_sm, 1))); } \
                 kern<<<ctas, nt, sm, G.stream>>>(sa); } while (0)
                 GB_FOR_SEMIRING(xt, zt, add, mul, K_MSTREAM, err); GB_LAUNCHED();
-                gb_kernel_used(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
-                gb_kernel_used(sa.exact ? "filter=exact" : "filter=bloom");
+                use.cls[k] = true; use.exact[k] = sa.exact != 0;
                 trace.mark(k == 0 ? "stream S" : (k == 1 ? "stream M" : "stream L"));
             }
         }
         if (zsz < 4) {      // narrow 32-bit accumulator words to the 1- or 2-byte type, in a second buffer
-            GB_TRY(typed.alloc((size_t)M.nnz * zsz + 16, err));
-            narrow_words_kernel<<<grid_for(M.nnz), 256, 0, G.stream>>>((const uint32_t *)words, (uint8_t *)typed, (int)zsz, M.nnz); GB_LAUNCHED();
-            words = typed;
+            GB_TRY(typed.alloc((size_t)P.mnnz * zsz + 16, err));
+            narrow_words_kernel<<<grid_for(P.mnnz), 256, 0, G.stream>>>((const uint32_t *)words, (uint8_t *)typed, (int)zsz, P.mnnz); GB_LAUNCHED();
+            *tval = typed;
         }
     }
-    GB_TRY(masked_compact(M, found, words, zsz, T, err));
-    typed.reset();
+    return GrB_SUCCESS;
+}
+
+template <typename OT>
+static GrB_Info masked_compact_t(int64_t nrows, int64_t ncols, int64_t mnnz, const OT *m_ptr, const uint32_t *m_col, const uint8_t *found,
+                                 const void *tval, size_t vsize, Csr &T, std::string *err);
+
+// ------------------------------------------------------------------ the wide route of the masked methods
+// Rows of T<M> = A (+).(x) B depend on the same rows of A and M only, so the wide route walks A and M in row panels of at most
+// `bound` entries of each (a longer row is a panel of its own: every row has fewer than 2^31 entries), with their offsets rebased
+// to 32 bits: the kernels keep 32-bit positions in A and M, and the per-mask-entry scratch and the per-row arrays are those of one
+// panel.  B's rows are gathered by A's column ids and cannot be cut: the kernels read B's 64-bit offsets when B is wide.  Each
+// panel is compacted on its own; T is formed from the panels' row counts and entries.
+static constexpr int64_t WIDE_PANEL = (int64_t)1 << 30;
+static constexpr int64_t WIDE_PANEL_ROWS = (int64_t)1 << 26;       // and at most this many rows: the per-row arrays (40 B a row)
+
+// the panel that starts at row r0: out = {r1, A's and M's first entries, M's end}, r1 the last row r <= r0 + max_rows with at most
+// `bound` entries of A and of M in rows [r0, r), and at least r0 + 1
+__global__ void panel_end_kernel(const int64_t *a_ptr, const int64_t *m_ptr, int64_t r0, int64_t nrows, int64_t bound, int64_t max_rows,
+                                 int64_t *out) {
+    const int64_t a0 = a_ptr[r0], m0 = m_ptr[r0];
+    int64_t lo = r0 + 1, hi = min(nrows, r0 + max_rows);
+    while (lo < hi) {
+        const int64_t mid = lo + (hi - lo + 1) / 2;
+        if (a_ptr[mid] - a0 <= bound && m_ptr[mid] - m0 <= bound) lo = mid; else hi = mid - 1;
+    }
+    out[0] = lo; out[1] = a0; out[2] = m0; out[3] = m_ptr[lo];
+}
+// out[r] = ptr[r0 + r] - ptr[r0], r = 0 .. n: the 32-bit offsets of a panel of n rows
+__global__ void panel_rowptr_kernel(const int64_t *ptr, int64_t r0, int64_t n, uint32_t *out) {
+    const int64_t base = ptr[r0];
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= n; r += (int64_t)gridDim.x * blockDim.x) out[r] = (uint32_t)(ptr[r0 + r] - base);
+}
+
+template <typename BT>
+static GrB_Info spgemm_masked_wide(const Csr &A, const Csr &B, const BT *b_ptr, const void *aval, const void *bval, int xt, int zt,
+                                   int add, int mul, bool need_a, bool need_b, const Csr &M, int mtc, bool m_struct, bool dot,
+                                   PhaseTrace &trace, MaskedUse &use, Csr &T, std::string *err) {
+    const int64_t nrows = A.nrows, ncols = dot ? B.nrows : B.ncols;
+    const size_t zsz = (size_t)tc_size(zt), asz = need_a ? (size_t)tc_size(xt) : 0, msz = M.val.get() ? (size_t)tc_size(mtc) : 0;
+    const int64_t bound = std::min(G.debug_wide > 0 ? wide_chunk() : WIDE_PANEL, WIDE_PANEL);
+    std::vector<Csr> parts;
+    DevBuf<int64_t> ends;
+    GB_TRY(ends.alloc(4, err));
+    // the panel that starts at row r0, compacted into `part`; *r1 = its end
+    auto panel = [&](int64_t r0, int64_t *r1, Csr &part) -> GrB_Info {
+        panel_end_kernel<<<1, 1, 0, G.stream>>>(A.rowptr, M.rowptr, r0, nrows, bound, WIDE_PANEL_ROWS, ends); GB_LAUNCHED();
+        int64_t h[4];
+        CU_TRY(cudaMemcpyAsync(h, ends, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
+        CU_TRY(cudaStreamSynchronize(G.stream), err);
+        *r1 = h[0];
+        const int64_t a0 = h[1], m0 = h[2], m1 = h[3];
+        const int64_t pn = *r1 - r0;
+        uint32_t *ap = nullptr, *mp = nullptr;
+        GB_TRY(ws_array(WS_PANEL_A, &ap, (size_t)pn + 1, err)); GB_TRY(ws_array(WS_PANEL_M, &mp, (size_t)pn + 1, err));
+        panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(A.rowptr, r0, pn, ap); GB_LAUNCHED();
+        panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(M.rowptr, r0, pn, mp); GB_LAUNCHED();
+        const MaskedPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr,
+                            mp, M.col + m0, msz ? static_cast<const uint8_t *>(M.val.get()) + m0 * msz : nullptr, pn, m1 - m0};
+        void *tval = nullptr; uint8_t *found = nullptr;
+        DevBuf<void> typed;
+        GB_TRY(masked_panel<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, mtc, m_struct, dot, ncols, trace, use,
+                                &tval, &found, typed, err));
+        return masked_compact_t<uint32_t>(pn, ncols, P.mnnz, mp, P.m_col, found, tval, zsz, part, err);
+    };
+    int64_t r1 = 0;
+    if (nrows > 0) {
+        parts.emplace_back();
+        GB_TRY(panel(0, &r1, parts[0]));
+        if (r1 == nrows) {                      // one panel: it is T
+            T = std::move(parts[0]);
+            G.last_nnz_out = (uint64_t)T.nnz;
+            return GrB_SUCCESS;
+        }
+    }
+    GB_TRY(csr_from_row_counts(nrows, ncols, zsz, T, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr + nrows, 0, 8, G.stream), err);
+            for (int64_t r0 = 0, q = 0; r0 < nrows; r0 = r1, ++q) {
+                if (q > 0) { parts.emplace_back(); GB_TRY(panel(r0, &r1, parts.back())); }
+                else r1 = parts[0].nrows;
+                row_len_kernel<<<grid_for(r1 - r0), 256, 0, G.stream>>>(parts.back().rowptr32, r1 - r0, rowptr + r0); GB_LAUNCHED();
+            }
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            int64_t at = 0;
+            for (Csr &part : parts) {
+                if (part.nnz) {
+                    CU_TRY(cudaMemcpyAsync(t.col.get() + at, part.col, (size_t)part.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
+                    CU_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(t.val.get()) + at * zsz, part.val, (size_t)part.nnz * zsz,
+                                           cudaMemcpyDeviceToDevice, G.stream), err);
+                }
+                at += part.nnz;
+                part = Csr();
+            }
+            return GrB_SUCCESS;
+        }));
+    G.last_nnz_out = (uint64_t)T.nnz;
+    return GrB_SUCCESS;
+}
+
+static void masked_report(const MaskedUse &u, bool wide) {
+    bool first = true;
+    auto entry = [&](const char *k) { gb_kernel_used(k); if (first && wide) gb_kernel_used("offsets=64"); first = false; };
+    if (u.dot) entry("dot");
+    if (u.warp) entry("masked-warp");
+    for (int k = 0; k < 3; ++k) {
+        if (!u.cls[k]) continue;
+        entry(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
+        gb_kernel_used(u.exact[k] ? "filter=exact" : "filter=bloom");
+    }
+}
+
+// The narrow route runs the masked methods once on the whole of A and M; the wide route (csr_wide: an operand of 2^32 or more
+// entries, or B200_debug_wide) on row panels, with B's 64-bit offsets when B is wide.
+static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt,
+                              int add, int mul, bool need_a, bool need_b, const Csr &M, int mtc, bool m_struct,
+                              bool dot, Csr &T, std::string *err) {
+    const int64_t nrows = A.nrows, ncols = dot ? B.nrows : B.ncols;
+    T = Csr(); T.nrows = nrows; T.ncols = ncols;
+    const size_t zsz = (size_t)tc_size(zt);
+    PhaseTrace trace;
+    MaskedUse use;
+    G.last_flops = 0;
+    const bool wide = csr_wide(A) || csr_wide(B) || csr_wide(M);
+    if (!wide) {
+        DevBuf<void> typed;
+        void *words = nullptr; uint8_t *found = nullptr;
+        const MaskedPanel P{A.rowptr32, A.col, aval, M.rowptr32, M.col, M.val, nrows, M.nnz};
+        GB_TRY(masked_panel<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, mtc, m_struct, dot, ncols, trace,
+                                      use, &words, &found, typed, err));
+        GB_TRY(masked_compact(M, found, words, zsz, T, err));
+    } else if (csr_wide(B)) {
+        GB_TRY(spgemm_masked_wide<int64_t>(A, B, B.rowptr.get(), aval, bval, xt, zt, add, mul, need_a, need_b, M, mtc, m_struct, dot,
+                                           trace, use, T, err));
+    } else {
+        GB_TRY(spgemm_masked_wide<uint32_t>(A, B, B.rowptr32.get(), aval, bval, xt, zt, add, mul, need_a, need_b, M, mtc, m_struct, dot,
+                                            trace, use, T, err));
+    }
+    masked_report(use, wide);
     trace.mark("compaction");
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
 
 template <typename OT>
-static GrB_Info masked_compact_t(const Csr &M, const OT *m_ptr, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
-    const int64_t nrows = M.nrows;
-    return csr_from_row_counts(nrows, M.ncols, vsize, T, err,
+static GrB_Info masked_compact_t(int64_t nrows, int64_t ncols, int64_t mnnz, const OT *m_ptr, const uint32_t *m_col, const uint8_t *found,
+                                 const void *tval, size_t vsize, Csr &T, std::string *err) {
+    return csr_from_row_counts(nrows, ncols, vsize, T, err,
         [&](int64_t *rowptr) {
             CU_TRY(cudaMemsetAsync(rowptr, 0, ((size_t)nrows + 1) * 8, G.stream), err);
-            if (M.nnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, found, nrows, rowptr); GB_LAUNCHED(); }
+            if (mnnz > 0) { row_found_count_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, found, nrows, rowptr); GB_LAUNCHED(); }
             return GrB_SUCCESS;
         },
         [&](Csr &t) {
-            row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, M.col, found, (const uint8_t *)tval, (int)vsize,
+            row_found_fill_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(m_ptr, m_col, found, (const uint8_t *)tval, (int)vsize,
                                                                               nrows, t.rowptr, t.col, (uint8_t *)t.val); GB_LAUNCHED();
             return GrB_SUCCESS;
         });
 }
 GrB_Info masked_compact(const Csr &M, const uint8_t *found, const void *tval, size_t vsize, Csr &T, std::string *err) {
-    GB_TRY(csr_wide(M) ? masked_compact_t<int64_t>(M, M.rowptr.get(), found, tval, vsize, T, err)
-                       : masked_compact_t<uint32_t>(M, M.rowptr32.get(), found, tval, vsize, T, err));
+    GB_TRY(csr_wide(M) ? masked_compact_t<int64_t>(M.nrows, M.ncols, M.nnz, M.rowptr.get(), M.col, found, tval, vsize, T, err)
+                       : masked_compact_t<uint32_t>(M.nrows, M.ncols, M.nnz, M.rowptr32.get(), M.col, found, tval, vsize, T, err));
     G.last_nnz_out = (uint64_t)T.nnz;
     return GrB_SUCCESS;
 }
@@ -1383,7 +1535,8 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
     if (Mask) GB_TRY(matrix_ensure_device(Mask));
     const Csr &a = *pa;
     const Csr &b = (f.tran1 && !dot) ? B->devT : B->dev;
-    if (!a.rowptr32 || !b.rowptr32 || (Mask && !Mask->dev.rowptr32))
+    // the masked methods have a wide route (spgemm_masked); the unmasked and complemented-mask bins have 32-bit offsets only
+    if (!use_mask && (!a.rowptr32 || !b.rowptr32 || (Mask && !Mask->dev.rowptr32)))
         return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
 
     DevBuf<void> a_cast, b_cast;

@@ -19,8 +19,8 @@
 // (scale 20: 63 MB of column ids), which is what the coalesced 128-bit loads are for.
 #pragma once
 
-struct StreamArgs {
-    GemmArgs g;
+template <typename BT> struct StreamArgsT {
+    GemmArgsT<BT> g;
     const int32_t *chunk_row; const uint32_t *chunk_idx; const uint32_t *chunk_cnt; int64_t nchunks;
     void *t_words;                  // nnz(M) accumulator words (pre-set to accum_init)
     unsigned int *queue;            // next block of chunks
@@ -40,18 +40,21 @@ __host__ __device__ inline size_t stream_var_smem(int bm_log2, int table, int va
     const size_t head = ((((size_t)1 << bm_log2) / 8 + (size_t)table * 6 + 7) & ~(size_t)7) + (size_t)vals_cap * (wsize + 1);
     return (head + 15) & ~(size_t)15;
 }
-template <typename XT> __host__ __device__ inline size_t stream_fixed_smem(int nt) {
+// BT: B's row offsets.  A B row start per batch entry is a BT; a queue entry's B position is absolute for uint32_t offsets and
+// relative to the row start of its A entry for int64_t ones (a row has fewer than 2^31 entries), so the queue stays 10 bytes.
+template <typename XT, typename BT> __host__ __device__ inline size_t stream_fixed_smem(int nt) {
     // per-batch A entry arrays + survivor queues (column, B position, batch index of the A entry) + long-row list (entry, first trip)
-    return (size_t)nt * (4 + 4 + sizeof(XT)) + (size_t)(nt / 32) * STREAM_QCAP * (8 + 2) + (size_t)nt * (2 + 4) + 64;
+    return (size_t)nt * (sizeof(BT) + 4 + sizeof(XT)) + (size_t)(nt / 32) * STREAM_QCAP * (8 + 2) + (size_t)nt * (2 + 4) + 64;
 }
 
 // One code path, one call site each for the streaming loop and for the survivor drain: the kernel must stay small -- its first
 // version inlined the resolve / atomic code at every push (11 k SASS instructions, 176 KB) and lost 2x to instruction fetch.
-template <typename XT, typename ZT, int ADD, int MUL>
-__global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs sa) {
+template <typename XT, typename ZT, int ADD, int MUL, typename BT>
+__global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgsT<BT> sa) {
     typedef typename SlotWord<ZT>::W W;
+    constexpr bool WIDE = sizeof(BT) == 8;
     const int NT = blockDim.x, NW = NT >> 5;
-    const GemmArgs &p = sa.g;
+    const GemmArgsT<BT> &p = sa.g;
     const int add = ADD >= 0 ? ADD : p.add_op;
     const int mul = MUL >= 0 ? MUL : p.mul_op;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -67,8 +70,8 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
     const int hshift = sa.table ? __clz(sa.table) + 1 : 0;
     int32_t *gslot = sa.spa_slot ? sa.spa_slot + (size_t)blockIdx.x * p.ncols : nullptr;
     XT *s_av = reinterpret_cast<XT *>(rest);
-    uint32_t *s_bs = reinterpret_cast<uint32_t *>(rest + (size_t)NT * sizeof(XT));
-    uint32_t *s_len = s_bs + NT;
+    BT *s_bs = reinterpret_cast<BT *>(rest + (size_t)NT * sizeof(XT));
+    uint32_t *s_len = reinterpret_cast<uint32_t *>(s_bs + NT);
     uint32_t *s_ltrip = s_len + NT;                              // long rows: trips before this row (exclusive running sum)
     uint2 *s_q = reinterpret_cast<uint2 *>(s_ltrip + NT);
     uint16_t *s_qe = reinterpret_cast<uint16_t *>(s_q + NW * STREAM_QCAP);
@@ -144,10 +147,10 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
             for (uint32_t base = c0; base < c1; base += NT) {
                 // the batch's A entries: B row range and A value, one per thread
                 const uint32_t pa = base + tid;
-                uint32_t bs = 0, len = 0; XT av = (XT)1;
+                BT bs = 0; uint32_t len = 0; XT av = (XT)1;
                 if (pa < c1) {
                     const uint32_t k = __ldg(p.a_col + pa);
-                    bs = __ldg(p.b_ptr + k); len = __ldg(p.b_ptr + k + 1) - bs;
+                    bs = __ldg(p.b_ptr + k); len = (uint32_t)(__ldg(p.b_ptr + k + 1) - bs);
                     if (p.need_a) av = gload<XT>(aval + pa);
                 }
                 if (tid == 0) { s_nlong = 0; s_ltrips = 0; }
@@ -162,7 +165,7 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
                 const int nlong = (int)s_nlong;
                 if (tid == 0) {                                   // trips of the long rows, in list order (few rows: serial)
                     uint32_t run = 0;
-                    for (int x = 0; x < nlong; ++x) { const int e = s_long[x]; s_ltrip[x] = run; run += (((s_bs[e] & 3u) + s_len[e]) + item_len - 1u) >> sa.blk_log2; }
+                    for (int x = 0; x < nlong; ++x) { const int e = s_long[x]; s_ltrip[x] = run; run += ((((uint32_t)s_bs[e] & 3u) + s_len[e]) + item_len - 1u) >> sa.blk_log2; }
                     s_ltrips = run;
                 }
                 __syncthreads();
@@ -172,7 +175,7 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
                 int lx = 0;                                        // cursor into the long-row list (items come in increasing order)
                 for (uint32_t item = warp; ; item += NW) {
                     const bool flush = item >= nitems;            // one last pass per warp: nothing to stream, the queue is emptied
-                    int ent = 0; uint32_t s = 0, e = 0;
+                    int ent = 0; BT s = 0, e = 0;
                     if (!flush) {
                         if (item < (uint32_t)nent) {
                             ent = (int)item;
@@ -182,18 +185,18 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
                             const uint32_t t = item - (uint32_t)nent;
                             while (lx + 1 < nlong && s_ltrip[lx + 1] <= t) ++lx;
                             ent = s_long[lx];
-                            const uint32_t b0 = s_bs[ent], p0 = b0 & ~3u, k = t - s_ltrip[lx];
-                            s = max(b0, p0 + k * item_len); e = min(b0 + s_len[ent], p0 + (k + 1u) * item_len);
+                            const BT b0 = s_bs[ent], p0 = b0 & ~(BT)3; const uint32_t k = t - s_ltrip[lx];
+                            s = max(b0, p0 + (BT)(k * item_len)); e = min(b0 + s_len[ent], p0 + (BT)((k + 1u) * item_len));
                         }
                     }
                     // ---- stream positions [s, e): trips of 128 (four consecutive ids per lane, one 128-bit load); the next trip's load is
                     //      issued before this trip is tested.  Trip counts are warp-uniform: every lane takes part in the ballots.
-                    uint32_t tb = s & ~3u;
-                    uint32_t pb = tb + (uint32_t)lane * 4u;
+                    BT tb = s & ~(BT)3;
+                    BT pb = tb + (uint32_t)lane * 4u;
                     uint4 c = make_uint4(0u, 0u, 0u, 0u);
                     if (pb < e) c = __ldg(reinterpret_cast<const uint4 *>(p.b_col + pb));      // past e: inside B's allocation, valid ids (spgemm_masked)
                     for (; tb < e || (flush && qn > 0); tb += 128u) {
-                        const uint32_t pbn = pb + 128u;
+                        const BT pbn = pb + 128u;
                         uint4 cn = make_uint4(0u, 0u, 0u, 0u);
                         if (pbn < e) cn = __ldg(reinterpret_cast<const uint4 *>(p.b_col + pbn));
                         const uint32_t jj[4] = {c.x, c.y, c.z, c.w};
@@ -203,7 +206,12 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
 #pragma unroll
                         for (uint32_t i = 0; i < 4; ++i) {
                             const uint32_t ball = __ballot_sync(0xffffffffu, h[i]);
-                            if (h[i]) { const int o = qn + __popc(ball & lt_mask); myq[o] = make_uint2(jj[i], pb + i); myqe[o] = (uint16_t)ent; }
+                            if (h[i]) {
+                                const int o = qn + __popc(ball & lt_mask);
+                                if constexpr (WIDE) myq[o] = make_uint2(jj[i], (uint32_t)(pb + i - s_bs[ent]));
+                                else myq[o] = make_uint2(jj[i], pb + i);
+                                myqe[o] = (uint16_t)ent;
+                            }
                             qn += __popc(ball);
                         }
                         c = cn; pb = pbn;
@@ -225,7 +233,9 @@ __global__ void __launch_bounds__(1024, 1) masked_stream_kernel(const StreamArgs
                                     }
                                 } else { const int32_t q = gslot[j]; if (q >= 0) lo = (uint32_t)q; }      // one L2 access per survivor
                                 if (lo != 0xffffffffu && (p.m_struct || sc_cast(sc_load(p.m_tc, p.m_val, lo), p.m_tc, TC_BOOL).u != 0)) {
-                                    const XT bv = p.need_b ? gload<XT>(bval + qe.y) : (XT)1;
+                                    BT qb = qe.y;
+                                    if constexpr (WIDE) qb += s_bs[myqe[qn - count + lane]];
+                                    const XT bv = p.need_b ? gload<XT>(bval + qb) : (XT)1;
                                     const ZT prod = MulApply<XT, ZT>::f(mul, s_av[myqe[qn - count + lane]], bv);
                                     if (local) { atomic_combine<ZT>(&vals[lo - ms], prod, add); found[lo - ms] = 1; }
                                     else { atomic_combine<ZT>(&tw[lo], prod, add); p.t_found[lo] = 1; }

@@ -6,6 +6,7 @@ import os
 import zlib
 
 import numpy as np
+import scipy.sparse as sp
 
 import pygraphblas_b200 as gb
 from pygraphblas_b200 import ffi, lib
@@ -76,6 +77,85 @@ def spmv_specialised(add, mul, typ):
     if typ in ("FP32", "FP64", "INT32", "INT64", "UINT32", "UINT64"):
         return (add == "PLUS" and mul in ("TIMES", "SECOND", "FIRST", "PAIR")) or (add == "MIN" and mul in ("PLUS", "FIRST", "SECOND"))
     return False
+
+
+# ------------------------------------------------------------------ the hot-table SpMV, restated (spmv_run.cu / spmv_run.cuh)
+HOT_EXT = 1 << 17
+HOT_T = ("BOOL", "INT32", "INT64", "UINT32", "UINT64", "FP32", "FP64")      # the types of the specialised semirings
+VSIZE = {"BOOL": 1, "INT32": 4, "UINT32": 4, "FP32": 4, "INT64": 8, "UINT64": 8, "FP64": 8}
+
+
+def kernel_mul(mul, vxm):
+    """The multiply the run kernels see: x = the matrix entry, y = u's (FIRST and SECOND swap in vxm form)."""
+    return {"FIRST": "SECOND", "SECOND": "FIRST"}.get(mul, mul) if vxm else mul
+
+
+def hot_reads_u(mul, vxm):
+    """The multiply reads u: only then is there a gather for the hot table to serve (else the plain run kernel)."""
+    return kernel_mul(mul, vxm) not in ("FIRST", "PAIR")
+
+
+def hot_reads_a(mul, vxm):
+    """The multiply reads A's values: the warp stage holds them beside the ids (mul_reads_x)."""
+    return kernel_mul(mul, vxm) not in ("SECOND", "PAIR")
+
+
+def hot_henc(S, vxm=False):
+    """henc of spmv_hot_plan: the referenced columns of the CSR the kernel pulls along (A for mxv, A' for vxm), at most HOT_EXT."""
+    deg = np.diff(S.indptr) if vxm else np.bincount(S.indices, minlength=S.shape[1])
+    return min(int(np.count_nonzero(deg)), HOT_EXT)
+
+
+def hot_id_bits(S, vxm=False):
+    """The id width spmv_hot_plan picks: 3 bytes when ncols + henc < 2^24 (ncols of the pulled CSR), else 4."""
+    ncols = S.shape[0] if vxm else S.shape[1]
+    return 24 if ncols + hot_henc(S, vxm) < (1 << 24) else 32
+
+
+def hot_table_cap(typ, reads_a, id_bits, henc, limit_bytes, max_optin):
+    """Restates hot2_table_entries: the table entries left after the warp stages and barriers, at most limit_bytes."""
+    idb = id_bits // 8
+    stage = 256 * idb + (256 * VSIZE[typ] if reads_a else 0)
+    fixed = 32 * stage + 33 * 8 + 8
+    avail = min(max(max_optin - fixed - 256, 0), limit_bytes)
+    return min(henc, avail // VSIZE[typ]) & ~15
+
+
+def hot_tiers(henc, cap, C, t0kb, vsize):
+    """Restates hot2_tiers: (C, T0, T1, slice)."""
+    if C == 1 or henc - cap < 16:
+        return 1, cap, 0, 0
+    t0 = min(((t0kb << 10) // vsize) & ~15, cap)
+    need = henc - t0
+    sl = min(cap - t0, (-(-need // C) + 15) & ~15)
+    if sl == 0:
+        return 1, cap, 0, 0
+    return C, t0, min(need, sl * C), sl
+
+
+def max_optin():
+    """The device's opt-in shared memory per block (what hot2_table_entries asks the driver for)."""
+    import torch
+    return int(torch.cuda.get_device_properties(0).shared_memory_per_block_optin)
+
+
+def expected_hot_launch(S, vxm, typ, mul, hot_kb, C, t0kb, smem_optin):
+    """(C, T0, T1, henc) and the id width of a hot-table call on the CSR S (A; the kernel pulls along A' in vxm form)."""
+    henc, bits = hot_henc(S, vxm), hot_id_bits(S, vxm)
+    cap = hot_table_cap(typ, hot_reads_a(mul, vxm), bits, henc, hot_kb << 10, smem_optin)
+    c, t0, t1, _ = hot_tiers(henc, cap, C, t0kb, VSIZE[typ])
+    return (c, t0, t1, henc), bits
+
+
+def hot_tokens():
+    """(kernel entries, {key: value}) of the last call's seam reading."""
+    ks = last_kernel().split(";")
+    return entries(ks), dict(k.split("=", 1) for k in ks if "=" in k)
+
+
+def hot_launch_of(tok):
+    """(C, T0, T1, henc) and the id width the library reports for a hot-table call."""
+    return (int(tok["hot-cluster"]),) + tuple(int(x) for x in tok["hot-tiers"].split(",")), int(tok["ids"])
 
 
 # ------------------------------------------------------------------ the kernel-path seam
@@ -196,6 +276,40 @@ def o_csr(typ, S, vals):
     m.J = S.indices.astype(np.uint64)
     m.X = np.ascontiguousarray(vals)
     return m
+
+
+def oracle_spmv(typ, sr, S, vals, uv, vxm):
+    """The oracle's mxv (A = S) or vxm (u' S) with dense u, on the entries of u that S references only: the referenced
+    indices are renumbered in order (the oracle's fold order is kept), so a u of 2^24 entries costs what S does."""
+    if vxm:
+        keep = np.flatnonzero(np.diff(S.indptr))
+        T = sp.csr_matrix((np.ones(S.nnz, np.int8), S.indices, np.r_[0, np.cumsum(np.diff(S.indptr)[keep])]), shape=(len(keep), S.shape[1]))
+        uo = orc.SpVec(typ, len(keep), np.arange(len(keep)), uv[keep])
+        return orc.vxm(orc.SpVec(typ, S.shape[1]), None, None, sr, uo, o_csr(typ, T, vals), "")
+    keep, inv = np.unique(S.indices, return_inverse=True)
+    T = sp.csr_matrix((np.ones(S.nnz, np.int8), inv.astype(np.int64), S.indptr), shape=(S.shape[0], len(keep)))
+    uo = orc.SpVec(typ, len(keep), np.arange(len(keep)), uv[keep])
+    return orc.mxv(orc.SpVec(typ, S.shape[0]), None, None, sr, o_csr(typ, T, vals), uo, "")
+
+
+def uniform_pattern(ncols, deg, cols=None):
+    """Every referenced column (cols, default all ncols) referenced exactly deg times: the stable degree sort then ranks the
+    j-th referenced column as j, so every hot rank (and so both sides of every tier boundary) is gathered.  Square when
+    every column is referenced, else one row per referenced column."""
+    cols = np.arange(ncols, dtype=np.int64) if cols is None else np.asarray(cols, np.int64)
+    nrows = ncols if len(cols) == ncols else len(cols)
+    j = np.repeat(cols, deg)
+    t = np.tile(np.arange(deg, dtype=np.int64), len(cols))
+    r = (np.repeat(np.arange(len(cols), dtype=np.int64), deg) * 7 + t * 4099) % nrows
+    S = sp.csr_matrix((np.ones(len(j), np.int8), (r, j)), shape=(nrows, ncols))
+    S.sort_indices()
+    assert S.nnz == len(cols) * deg
+    return S
+
+
+def spread_columns(ncols, low, nspread):
+    """The columns 0 .. low-1 and nspread columns spread evenly over the rest, the last column included."""
+    return np.concatenate([np.arange(low), np.linspace(low, ncols - 1, nspread).astype(np.int64)])
 
 
 # ------------------------------------------------------------------ coverage ledgers

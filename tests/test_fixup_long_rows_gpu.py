@@ -3,7 +3,9 @@ reaches at most FIX_LONG = 8 runs further is folded by one thread, a longer one 
 matrix holds rows whose open span sits just below, at and above that boundary, rows that need one, two and three trips of
 the warp, rows that end exactly at a run's end, and a long last row that ends inside a partial last run.  Every route that
 runs the fix-up (hot-table kernel at every cluster size, plain run kernel, sparse u) must give the oracle's values (the value
-pools make every fold exact in any order) and identical bytes on every call."""
+pools make every fold exact in any order) and identical bytes on every call.  The matrix is built twice: on 2^18 columns the
+hot-table kernel streams 3-byte ids, on 2^24 + 4096 columns 4-byte ids, whose bulk copy of the partial last run is rounded
+up to 16 bytes rather than taking a whole padded run."""
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -11,11 +13,11 @@ import scipy.sparse as sp
 from pygraphblas_b200 import Matrix, Vector
 from oracle import oracle as orc
 import util
-from kernel_check import compare, entries, last_kernel, o_csr, semiring, seed_of, tunables, values, fp_pool_for
+from kernel_check import compare, entries, hot_id_bits, last_kernel, o_csr, semiring, seed_of, tunables, values, fp_pool_for
 
 RUN = 256
 FIX_LONG = 8
-NCOLS = 1 << 18
+NCOLS = {"ids24": 1 << 18, "ids32": (1 << 24) + 4096}
 # open spans (runs past the run the row starts in) of the rows placed at an offset of 100 inside a run; "end" rows end on
 # the last entry of a run
 SPANS = [1, 7, 8, 9, 31, 32, 33, 255, 256, 257, 600]
@@ -23,7 +25,7 @@ END_SPANS = [5, 20]
 LAST_SPAN = 12
 
 
-def build_pattern():
+def build_pattern(ncols):
     """(S, spans): a CSR pattern of >= 2^20 entries (the hot-table kernel's minimum) and the open span of every long row."""
     rng = np.random.default_rng(11)
     lens, spans = [], []
@@ -66,8 +68,8 @@ def build_pattern():
     indices = np.empty(int(indptr[-1]), np.int64)
     for r in np.flatnonzero(row_len):
         L = int(row_len[r])
-        indices[indptr[r]:indptr[r + 1]] = np.sort(rng.choice(NCOLS, L, replace=False))
-    S = sp.csr_matrix((np.ones(len(indices), np.int8), indices, indptr), shape=(nrows, NCOLS))
+        indices[indptr[r]:indptr[r + 1]] = np.sort(rng.choice(ncols, L, replace=False))
+    S = sp.csr_matrix((np.ones(len(indices), np.int8), indices, indptr), shape=(nrows, ncols))
     return S, spans
 
 
@@ -80,9 +82,10 @@ def open_spans(S):
     return (ends[last] - 1) // RUN - run_of[last]
 
 
-@pytest.fixture(scope="module")
-def pattern():
-    S, spans = build_pattern()
+@pytest.fixture(scope="module", params=list(NCOLS))
+def pattern(request):
+    S, spans = build_pattern(NCOLS[request.param])
+    assert hot_id_bits(S) == int(request.param[3:])          # the width the plan picks (ncols + henc against 2^24)
     got = open_spans(S)
     # every designed span is an open span of the plan, on both sides of the boundary, and one needs three warp trips
     assert set(spans) <= set(got.tolist())
@@ -96,7 +99,10 @@ SRS = [("PLUS", "TIMES", "FP32"), ("PLUS", "TIMES", "FP64"), ("MIN", "PLUS", "FP
 
 def call(A, u, sr):
     w = A.mxv(u, semiring=semiring(*sr))
-    ent = entries(last_kernel().split(";"))
+    ks = last_kernel().split(";")
+    ent = entries(ks)
+    if ent[0].startswith("run+hot"):
+        ent = [f"{ent[0]} {k}" for k in ks if k.startswith("ids=")]
     x, p = w.to_numpy()
     return ent[0], (np.ascontiguousarray(x).tobytes(), np.ascontiguousarray(p).tobytes()), w.to_arrays()
 
@@ -118,7 +124,8 @@ def test_long_open_rows(pattern, sr):
     u = Vector.from_numpy(uv, typ=util.g_type(typ))
     ref = orc.mxv(orc.SpVec(typ, nrows), None, None, sr, Ao, orc.SpVec(typ, ncols, np.arange(ncols), uv), "")
     base = None
-    settings = [("run+hot-table (TMA-staged)", {"B200GRB_SPMV_HOT": 128, "B200GRB_SPMV_CLUSTER": C, "B200GRB_SPMV_HOT_REPL": t0})
+    hot = f"run+hot-table (TMA-staged) ids={hot_id_bits(S)}"
+    settings = [(hot, {"B200GRB_SPMV_HOT": 128, "B200GRB_SPMV_CLUSTER": C, "B200GRB_SPMV_HOT_REPL": t0})
                 for C, t0 in ((1, 0), (2, 32), (4, 0), (8, 96), (16, 32))]
     settings += [("run", {"B200GRB_SPMV_HOT": 0})]
     for route, env in settings:

@@ -6,7 +6,8 @@ B200GRB_SPMV_HOT_REPL request (entries, multiple of 16, at most cap), the rest o
 distributed tier T1, and the hot ranks past T0 + T1 up to henc are read from u_hot in L2.  Plain CTAs are launched when
 one table holds every hot rank or T0 takes the whole table.  Every call asserts the cluster size and the tiers the
 library reports (`hot-cluster=`, `hot-tiers=T0,T1,henc`) against this restatement; an H100 co-schedules every C <= 16.
-The SASS checks need no GPU."""
+Each call also asserts the id width (`ids=24` / `ids=32`, spmv_hot_plan: 4-byte ids once ncols + henc reaches 2^24), and
+every cluster size is reached at both widths.  The SASS checks need no GPU."""
 import os
 import re
 import shutil
@@ -18,37 +19,17 @@ import scipy.sparse as sp
 
 from pygraphblas_b200 import Matrix, Vector
 from pygraphblas_b200.generators import rmat_csr
-from oracle import oracle as orc
 import util
-from kernel_check import compare, entries, last_kernel, o_csr, semiring, seed_of, tunables, values, fp_pool_for
+from kernel_check import (HOT_EXT, compare, expected_hot_launch, hot_launch_of, hot_tokens, max_optin, oracle_spmv, semiring, seed_of,
+                          spread_columns, tunables, uniform_pattern, values, fp_pool_for)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "pygraphblas_b200", "libb200grb.so")
-HOT_EXT = 1 << 17
 CLUSTERS = (1, 2, 4, 8, 16)
 HOT_SRS = [("PLUS", "TIMES"), ("MIN", "PLUS"), ("PLUS", "SECOND")]
 SRS = [sr + (t,) for t in ("FP32", "FP64", "INT32", "UINT64") for sr in HOT_SRS] + [("LOR", "LAND", "BOOL")]
-VSIZE = {"FP32": 4, "FP64": 8, "INT32": 4, "UINT64": 8, "BOOL": 1}
 ROUTES = {"run+hot-table (TMA-staged)"}
-REACHED_C, SIDES = set(), set()
-
-
-def tokens():
-    ks = last_kernel().split(";")
-    return entries(ks), dict(k.split("=", 1) for k in ks if "=" in k)
-
-
-def uniform_pattern(ncols, deg):
-    """Every column referenced exactly deg times: the stable degree sort then ranks column j as j, so every hot rank
-    (and so both sides of every tier boundary) is gathered."""
-    nrows = ncols
-    j = np.repeat(np.arange(ncols, dtype=np.int64), deg)
-    t = np.tile(np.arange(deg, dtype=np.int64), ncols)
-    r = (j * 7 + t * 4099) % nrows
-    S = sp.csr_matrix((np.ones(len(j), np.int8), (r, j)), shape=(nrows, ncols))
-    S.sort_indices()
-    assert S.nnz == ncols * deg
-    return S
+REACHED_C, SIDES = set(), set()         # REACHED_C: (C, id width) of every launch
 
 
 def rmat_pattern(scale):
@@ -56,39 +37,19 @@ def rmat_pattern(scale):
     return sp.csr_matrix((np.ones(len(indices), np.int8), indices, indptr), shape=(n, n))
 
 
-def tiers(henc, cap, C, t0kb, vsize):
-    """Restates hot2_tiers: (C, T0, T1, slice)."""
-    if C == 1 or henc - cap < 16:
-        return 1, cap, 0, 0
-    t0 = min(((t0kb << 10) // vsize) & ~15, cap)
-    need = henc - t0
-    sl = min(cap - t0, (-(-need // C) + 15) & ~15)
-    if sl == 0:
-        return 1, cap, 0, 0
-    return C, t0, min(need, sl * C), sl
-
-
-def expected_tiers(S, vxm, typ, hot_kb, C, t0kb):
-    """(C, T0, T1, henc) of a call: henc from the column degrees of the CSR the kernel pulls along (A' for vxm), cap from
-    the table limit (128 KB or B200GRB_SPMV_HOT; the shared memory left after the stages exceeds 128 KB for these types)."""
-    deg = np.diff(S.indptr) if vxm else np.bincount(S.indices, minlength=S.shape[1])
-    henc = min(int(np.count_nonzero(deg)), HOT_EXT)
-    cap = min(henc, (hot_kb << 10) // VSIZE[typ]) & ~15
-    c, t0, t1, _ = tiers(henc, cap, C, t0kb, VSIZE[typ])
-    return c, t0, t1, henc
-
-
 def run_all(S, label, settings, srs=SRS, forms=("mxv", "vxm"), hot_kb=128):
     """For each semiring and form: the C = 1 result, then each (C, T0 KB) of settings must give the same bytes; every
-    result is compared with the oracle, and the launch the library reports with the restated tiers.  Returns the set
-    of (C, T0, T1, henc) launched."""
+    result is compared with the oracle, and the launch the library reports (tiers and id width) with the restatement
+    (kernel_check.expected_hot_launch: the table is capped by hot_kb and by the shared memory left after the stages).
+    Returns the set of (C, T0, T1, henc) launched."""
     nrows, ncols = S.shape
+    smem = max_optin()
     errors, launched = [], set()
     for sr0 in srs:
         typ = sr0[2]
         pool = fp_pool_for(sr0[0], sr0[1]) if typ in util.FP_T else "edge"
         av = values(seed_of(label, typ), typ, S.nnz, pool, 0)
-        A, Ao = Matrix.from_csr(S.indptr, S.indices, av, nrows, ncols, util.g_type(typ)), o_csr(typ, S, av)
+        A = Matrix.from_csr(S.indptr, S.indices, av, nrows, ncols, util.g_type(typ))
         for form in forms:
             vxm = form == "vxm"
             # SECOND reads u in mxv form; in vxm form FIRST does (the other one gathers nothing and takes the plain run kernel)
@@ -96,20 +57,19 @@ def run_all(S, label, settings, srs=SRS, forms=("mxv", "vxm"), hot_kb=128):
             n_in = nrows if vxm else ncols
             uv = values(seed_of(label, sr, form), typ, n_in, pool, 1)
             u = Vector.from_numpy(uv, typ=util.g_type(typ))
-            uo = orc.SpVec(typ, n_in, np.arange(n_in), uv)
-            ref = orc.vxm(orc.SpVec(typ, nrows if not vxm else ncols), None, None, sr, uo, Ao, "") if vxm else \
-                orc.mxv(orc.SpVec(typ, nrows), None, None, sr, Ao, uo, "")
+            ref = oracle_spmv(typ, sr, S, av, uv, vxm)
             base = None
             for C, t0kb in [(1, 0)] + list(settings):
                 with tunables(B200GRB_SPMV_CLUSTER=C, B200GRB_SPMV_HOT_REPL=t0kb):
                     w = u.vxm(A, semiring=semiring(*sr)) if vxm else A.mxv(u, semiring=semiring(*sr))
-                    ent, tok = tokens()
+                    ent, tok = hot_tokens()
                 assert ent[0] in ROUTES, (label, sr, form, C, ent)
-                got_t = (int(tok["hot-cluster"]),) + tuple(int(x) for x in tok["hot-tiers"].split(","))
-                want_t = expected_tiers(S, vxm, typ, hot_kb, C, t0kb)
+                got_t, got_bits = hot_launch_of(tok)
+                want_t, want_bits = expected_hot_launch(S, vxm, typ, sr[1], hot_kb, C, t0kb, smem)
                 assert got_t == want_t, (label, sr, form, C, t0kb, got_t, want_t)
+                assert got_bits == want_bits, (label, sr, form, C, t0kb, tok, want_bits)
                 launched.add(got_t)
-                REACHED_C.add(got_t[0])
+                REACHED_C.add((got_t[0], got_bits))
                 x, p = w.to_numpy()
                 got = (np.ascontiguousarray(x).tobytes(), np.ascontiguousarray(p).tobytes())
                 if base is None:
@@ -125,9 +85,12 @@ def run_all(S, label, settings, srs=SRS, forms=("mxv", "vxm"), hot_kb=128):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("pattern", ["rmat18", "even"])
+@pytest.mark.parametrize("pattern", ["rmat18", "even", "even-ids32"])
 def test_cluster_sizes_are_bit_identical(pattern):
-    S = rmat_pattern(18) if pattern == "rmat18" else uniform_pattern((1 << 17) + 4096, 8)
+    # even-ids32: the columns of "even" with the cold ones spread up to the last of 2^24 + 4096, so mxv pulls along a CSR
+    # whose ids take 4 bytes (vxm along A', of 2^17 + 4096 columns: 3 bytes)
+    S = {"rmat18": lambda: rmat_pattern(18), "even": lambda: uniform_pattern((1 << 17) + 4096, 8),
+         "even-ids32": lambda: uniform_pattern(WIDE, 8, spread_columns(WIDE, HOT_EXT, 4096))}[pattern]()
     settings = [(C, t0) for C in CLUSTERS[1:] for t0 in (0, 32, 96)]
     with tunables(B200GRB_SPMV_HOT=128):
         launched = run_all(S, pattern, settings, srs=SRS[:-1])
@@ -152,29 +115,33 @@ def test_plain_ctas_when_nothing_is_spread(case):
     SIDES.add(f"plain-{case}")
 
 
-# (ncols, per-column degree, C, T0 KB): FP32 tables of 128 KB (cap = 32768 entries)
+# (ncols, per-column degree, C, T0 KB, referenced columns or None for all): FP32 tables of 128 KB (cap = 32768 entries).
+# The -ids32 cases reference the same number of columns, spread up to the last of 2^24 + 4096 (4-byte ids)
+WIDE = (1 << 24) + 4096
 TIER_CASES = {
-    "c8-rest-and-u": ((1 << 17) + 4096, 8, 8, 96),        # T0 + T1 < henc = 2^17 < ncols: every tier and u
-    "c4-no-repl": ((1 << 17) + 4096, 8, 4, 0),            # T0 = 0: the table is all slices
-    "c16-short": ((1 << 16) + 40, 16, 16, 0),             # fewer hot columns than C * cap: partly filled slices
-    "c2-short-repl": ((1 << 16) + 40, 16, 2, 64),
+    "c8-rest-and-u": ((1 << 17) + 4096, 8, 8, 96, None),        # T0 + T1 < henc = 2^17 < ncols: every tier and u
+    "c4-no-repl": ((1 << 17) + 4096, 8, 4, 0, None),            # T0 = 0: the table is all slices
+    "c16-short": ((1 << 16) + 40, 16, 16, 0, None),             # fewer hot columns than C * cap: partly filled slices
+    "c2-short-repl": ((1 << 16) + 40, 16, 2, 64, None),
+    "c8-rest-and-u-ids32": (WIDE, 8, 8, 96, (HOT_EXT, 4096)),   # ranks 0 .. 2^17 - 1 on the lowest columns, 4096 cold ones
+    "c16-short-ids32": (WIDE, 16, 16, 0, (0, (1 << 16) + 40)),  # every referenced column hot, spread over all of u
 }
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", list(TIER_CASES))
 def test_tier_boundaries(case):
-    ncols, deg, C, t0kb = TIER_CASES[case]
-    S = uniform_pattern(ncols, deg)
+    ncols, deg, C, t0kb, spread = TIER_CASES[case]
+    S = uniform_pattern(ncols, deg, None if spread is None else spread_columns(ncols, *spread))
     srs = [("PLUS", "TIMES", "FP32"), ("MIN", "PLUS", "FP32")]
     with tunables(B200GRB_SPMV_HOT=128):
         launched = run_all(S, case, [(C, t0kb)], srs=srs, forms=("mxv",))
-    # the tiers the library reported for the cluster launch (rank j = column j: every rank is gathered, so each boundary
-    # inside the hot ranks has a gathered rank on both of its sides)
+    # the tiers the library reported for the cluster launch (rank j = the j-th referenced column: every rank is gathered, so
+    # each boundary inside the hot ranks has a gathered rank on both of its sides)
     (c, t0, t1, henc), = [t for t in launched if t[0] > 1]
     assert c == C
     for b in (t0, t0 + t1, henc):
-        if 0 < b < ncols:
+        if 0 < b < S.nnz // deg:
             SIDES.add(f"{case}-{b - 1}|{b}")
     if t0 + t1 < henc:
         SIDES.add(f"{case}-rest")
@@ -184,10 +151,10 @@ def test_tier_boundaries(case):
 
 def test_every_cluster_size_and_tier_was_reached(request):
     mine = [it for it in request.session.items if it.module is request.module and it is not request.node and "gpu" in it.keywords]
-    gpu_count = 2 + 3 + len(TIER_CASES)
+    gpu_count = 3 + 3 + len(TIER_CASES)
     if len(mine) < gpu_count or not REACHED_C:
         pytest.skip("the GPU cases of the module did not all run")
-    assert REACHED_C >= set(CLUSTERS), sorted(REACHED_C)
+    assert REACHED_C >= {(c, bits) for c in CLUSTERS for bits in (24, 32)}, sorted(REACHED_C)
     assert {s for s in SIDES if s.endswith("-rest")} and {s for s in SIDES if s.endswith("-partial-slices")}, SIDES
     assert all(any(s.startswith(c + "-") for s in SIDES) for c in TIER_CASES), SIDES
     assert len({s for s in SIDES if s.startswith("plain-")}) == 3, SIDES

@@ -1,32 +1,44 @@
-"""The hot-table SpMV kernel on 3-byte column ids (spmv_run.cuh, spmv_hot_plan): the plan stores the encoded ids in 3 bytes,
-packed run by run, when every id fits (ncols + henc < 2^24), and in 4 bytes otherwise.  The library reports the width it
-launched (`ids=24` / `ids=32` beside `hot-tiers=`); every result must match the oracle and be bit-identical to the plain run
-kernel (B200GRB_SPMV_HOT=0), which shares the runs, the fold and the fix-up and reads every value of u from u itself.
+"""The hot-table SpMV kernel on 3-byte and 4-byte column ids (spmv_run.cuh, spmv_hot_plan): the plan stores the encoded ids in
+3 bytes, packed run by run, when every id fits (ncols + henc < 2^24), and in 4 bytes otherwise.  The library reports the width
+it launched (`ids=24` / `ids=32` beside `hot-tiers=`); every result must match the oracle and be bit-identical to the plain
+run kernel (B200GRB_SPMV_HOT=0), which shares the runs, the fold and the fix-up and reads every value of u from u itself.
+
+Every specialised semiring runs on every type it is specialised for, in both forms: mxv pulls along A, vxm along A'
+(here A is the transposed pattern, so A' is the same skewed pattern).  The width is restated from the CSR the kernel pulls
+along; a multiply that ignores u gathers nothing and takes the plain run kernel.
 
 The matrices are skewed (most entries on a few thousand columns, so the default route takes the hot-table kernel), reference
 at least 2^17 columns (henc = 2^17) including the last one (the largest id, ncols - 1 + henc), have a number of entries that
 is not a multiple of 256 (the last run is padded) and a hub row that spans hundreds of runs (the fix-up's long-row path)."""
+import functools
+
 import numpy as np
 import pytest
 import scipy.sparse as sp
 
 from pygraphblas_b200 import Matrix, Vector
-from oracle import oracle as orc
 import util
-from kernel_check import compare, entries, last_kernel, o_csr, semiring, seed_of, tunables, values, fp_pool_for
+from kernel_check import (HOT_EXT, HOT_T, compare, expected_hot_launch, fp_pool_for, hot_launch_of, hot_reads_u, hot_tokens,
+                          max_optin, oracle_spmv, seed_of, semiring, spmv_specialised, tunables, values)
 
-HOT_EXT = 1 << 17
 RUN = 256
 HOT_ROUTE = "run+hot-table (TMA-staged)"
-SRS = [("PLUS", "TIMES", "FP32"), ("PLUS", "TIMES", "FP64"), ("PLUS", "TIMES", "INT64"), ("LOR", "LAND", "BOOL")]
 HUB = 60_000
+DEFAULT_C, DEFAULT_T0_KB, DEFAULT_HOT_KB = 2, 32, 128          # the library's defaults (common.cuh, spmv.cu)
+PAIRS = [("PLUS", m) for m in ("TIMES", "SECOND", "FIRST", "PAIR")] + [("MIN", m) for m in ("PLUS", "FIRST", "SECOND")] + \
+        [("LOR", m) for m in ("LAND", "PAIR", "SECOND", "FIRST")] + [("ANY", "PAIR")]
+SRS = [(a, m, t) for t in HOT_T for a, m in PAIRS if spmv_specialised(a, m, t)]
+FORMS = ("mxv", "vxm")
 
-# ncols of each case: the 3-byte ids of a graph of ~1 M columns, and ncols + henc one below and at 2^24
+# ncols of each case: the 3-byte ids of a graph of ~1 M columns, ncols + henc one below and at 2^24, and 4-byte ids well past it
 CASES = {
     "skewed": (1 << 20) + 4099,
     "below-2^24": (1 << 24) - HOT_EXT - 1,
     "at-2^24": (1 << 24) - HOT_EXT,
+    "well-above": (1 << 24) + (1 << 20) + 4099,
 }
+# (case, add, mul, typ, form, "ids=24" / "ids=32" / "run") of every call made
+REACHED = set()
 
 
 def skewed_pattern(ncols, seed):
@@ -48,41 +60,85 @@ def skewed_pattern(ncols, seed):
     return S
 
 
+@functools.lru_cache(maxsize=1)
+def operands(case):
+    """The pattern of mxv (A = S) and of vxm (A = S', so that the kernel pulls along A' = S): {form: CSR of A}."""
+    S = skewed_pattern(CASES[case], seed_of("packed-ids", case, bits=32))
+    St = S.T.tocsr()
+    St.sort_indices()
+    return {"mxv": S, "vxm": St}
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", list(CASES))
 def test_packed_ids_match_oracle_and_plain_run_kernel(case):
-    ncols = CASES[case]
-    S = skewed_pattern(ncols, seed_of("packed-ids", case, bits=32))
-    nrows = S.shape[0]
-    want_ids = "24" if ncols + HOT_EXT < (1 << 24) else "32"
+    pats = operands(case)
+    smem = max_optin()
     errors = []
-    for sr in SRS:
-        typ = sr[2]
-        pool = fp_pool_for(sr[0], sr[1]) if typ in util.FP_T else "edge"
-        av = values(seed_of(case, typ, "a"), typ, S.nnz, pool, 0)
-        uv = values(seed_of(case, typ, "u"), typ, ncols, pool, 1)
-        A = Matrix.from_csr(S.indptr, S.indices, av, nrows, ncols, util.g_type(typ))
-        u = Vector.from_numpy(uv, typ=util.g_type(typ))
-        label = f"{case} {'_'.join(sr)}"
+    for form in FORMS:
+        vxm = form == "vxm"
+        S = pats[form]
+        nrows, ncols = S.shape
+        n_in = nrows if vxm else ncols
+        mats, vecs = {}, {}
+        for sr in SRS:
+            add, mul, typ = sr
+            pool = fp_pool_for(add, mul) if typ in util.FP_T else "edge"
+            if (typ, pool) not in mats:
+                av = values(seed_of(case, typ, pool, form, "a"), typ, S.nnz, pool, 0)
+                uv = values(seed_of(case, typ, pool, form, "u"), typ, n_in, pool, 1)
+                mats = {(typ, pool): (Matrix.from_csr(S.indptr, S.indices, av, nrows, ncols, util.g_type(typ)), av)}
+                vecs = {(typ, pool): (Vector.from_numpy(uv, typ=util.g_type(typ)), uv)}
+            (A, av), (u, uv) = mats[(typ, pool)], vecs[(typ, pool)]
+            s = semiring(*sr)
+            label = f"{case} {form} {'_'.join(sr)}"
 
-        w = A.mxv(u, semiring=semiring(*sr))
-        ks = last_kernel().split(";")
-        tok = dict(k.split("=", 1) for k in ks if "=" in k)
-        assert entries(ks)[0] == HOT_ROUTE, (label, ks)
-        assert tok.get("ids") == want_ids, (label, ks)
-        assert int(tok["hot-tiers"].split(",")[2]) == HOT_EXT, (label, ks)
-        x, p = w.to_numpy()
-        hot_bytes = (np.ascontiguousarray(x).tobytes(), np.ascontiguousarray(p).tobytes())
-        ref = orc.mxv(orc.SpVec(typ, nrows), None, None, sr, o_csr(typ, S, av), orc.SpVec(typ, ncols, np.arange(ncols), uv), "")
-        e = compare(*w.to_arrays(), ref.I, ref.X, typ, sr[0], label)
-        if e:
-            errors.append(e)
+            w = u.vxm(A, semiring=s) if vxm else A.mxv(u, semiring=s)
+            ent, tok = hot_tokens()
+            if hot_reads_u(mul, vxm):
+                want_launch, want_bits = expected_hot_launch(S, vxm, typ, mul, DEFAULT_HOT_KB, DEFAULT_C, DEFAULT_T0_KB, smem)
+                assert ent[0] == HOT_ROUTE, (label, ent)
+                got_launch, got_bits = hot_launch_of(tok)
+                assert got_bits == want_bits, (label, tok, want_bits)
+                assert got_launch == want_launch and want_launch[3] == HOT_EXT, (label, got_launch, want_launch)
+                REACHED.add((case, add, mul, typ, form, f"ids={got_bits}"))
+            else:                                  # the multiply ignores u: nothing to gather, the plain run kernel
+                assert ent[0] == "run" and "ids" not in tok, (label, ent, tok)
+                REACHED.add((case, add, mul, typ, form, "run"))
+            x, p = w.to_numpy()
+            hot_bytes = (np.ascontiguousarray(x).tobytes(), np.ascontiguousarray(p).tobytes())
+            ref = oracle_spmv(typ, sr, S, av, uv, vxm)
+            e = compare(*w.to_arrays(), ref.I, ref.X, typ, add, label)
+            if e:
+                errors.append(e)
 
-        with tunables(B200GRB_SPMV_HOT=0):
-            w0 = A.mxv(u, semiring=semiring(*sr))
-            ks0 = last_kernel().split(";")
-        assert entries(ks0)[0] == "run" and not any(k.startswith("ids=") for k in ks0), (label, ks0)
-        x0, p0 = w0.to_numpy()
-        if (np.ascontiguousarray(x0).tobytes(), np.ascontiguousarray(p0).tobytes()) != hot_bytes:
-            errors.append(f"{label}: the hot-table kernel's bytes differ from the plain run kernel's")
-    assert not errors, "\n".join(errors)
+            with tunables(B200GRB_SPMV_HOT=0):
+                w0 = u.vxm(A, semiring=s) if vxm else A.mxv(u, semiring=s)
+                ent0, tok0 = hot_tokens()
+            assert ent0[0] == "run" and "ids" not in tok0, (label, ent0, tok0)
+            x0, p0 = w0.to_numpy()
+            if (np.ascontiguousarray(x0).tobytes(), np.ascontiguousarray(p0).tobytes()) != hot_bytes:
+                errors.append(f"{label}: the hot-table kernel's bytes differ from the plain run kernel's")
+    assert not errors, "\n".join(errors[:40])
+
+
+def expected_reach():
+    """Every (case, semiring, type, form) with the width its CSR gives, or "run" where the multiply ignores u."""
+    out = set()
+    for case, ncols in CASES.items():
+        bits = 24 if ncols + HOT_EXT < (1 << 24) else 32       # every case references >= 2^17 columns: henc = 2^17
+        for add, mul, typ in SRS:
+            for form in FORMS:
+                out.add((case, add, mul, typ, form, f"ids={bits}" if hot_reads_u(mul, form == "vxm") else "run"))
+    return out
+
+
+def test_every_semiring_type_form_and_width_was_reached(request):
+    mine = [it for it in request.session.items if it.module is request.module and it is not request.node and "gpu" in it.keywords]
+    if len(mine) < len(CASES) or not REACHED:
+        pytest.skip("the GPU cases of the module did not all run")
+    want = expected_reach()
+    assert REACHED == want, (sorted(want - REACHED)[:20], sorted(REACHED - want)[:20])
+    # both widths, each at every type and in both forms
+    for bits in ("ids=24", "ids=32"):
+        assert {(t, f) for _, _, _, t, f, b in REACHED if b == bits} == {(t, f) for t in HOT_T for f in FORMS}, bits

@@ -28,7 +28,7 @@ from pygraphblas_b200 import Matrix, Vector, descriptor
 from pygraphblas_b200.generators import rmat_csr
 from oracle import oracle as orc
 import util
-from kernel_check import (compare, entries, fp_pool_for as _fp_pool_for, last_kernel, o_csr, products_by_entry, record_kernels,
+from kernel_check import (compare, entries, fp_pool_for as _fp_pool_for, last_kernel, o_csr, oracle_spmv, products_by_entry, record_kernels,
                           seed_of, semiring, spmv_specialised, tunables, values, vec_products as _vec_products)
 
 pytestmark = pytest.mark.gpu
@@ -93,7 +93,10 @@ SPMV = {
     "tile-8": dict(shape="small", env={}, kernel="run", only=None),          # a matrix smaller than 8 runs
     "run": dict(shape="run", env={}, kernel="run", only=None),
     "run-sparse-u": dict(shape="run", env={}, kernel="run (sparse u)", only=None, sparse_u=True),
-    "hot": dict(shape="rmat", env={"B200GRB_SPMV_HOT": 128}, kernel="run+hot-table (TMA-staged)", only=spmv_specialised),
+    "hot": dict(shape="rmat", env={"B200GRB_SPMV_HOT": 128}, kernel="run+hot-table (TMA-staged)", only=spmv_specialised, ids="24"),
+    # the same on 4-byte ids: a square matrix of more than 2^24 columns, so mxv and vxm both pull along such a CSR
+    "hot-ids32": dict(shape="skewed-wide", env={"B200GRB_SPMV_HOT": 128}, kernel="run+hot-table (TMA-staged)", only=spmv_specialised,
+                      ids="32"),
     "pull": dict(shape="pull", env={}, kernel="pull", only=lambda a, m, t: a in ("LOR", "LAND", "ANY"), mask=True),
     "push": dict(shape="pull", env={"B200GRB_FORCE_PUSH": 1}, kernel="push", only=lambda a, m, t: a in ("LOR", "LAND", "ANY"),
                  mask=True, sparse_u=True),
@@ -101,8 +104,26 @@ SPMV = {
 HOT_T = ["BOOL", "INT32", "UINT64", "FP32", "FP64"]
 
 
+@functools.lru_cache(maxsize=1)
+def skewed_wide():
+    """2^24 + 4099 rows and columns, ~1.2 M entries: columns concentrated on the lowest 2^17 (the hot ranks) plus cold ones
+    up to the last column (ids up to ncols - 1 + henc), rows spread over all of them (A' references more than 2^17 columns
+    too); the number of entries is not a multiple of 256 (the last run is partial)."""
+    n = (1 << 24) + 4099
+    rng = np.random.default_rng(15)
+    cols = np.concatenate([rng.integers(0, n, 400_000), ((1 << 17) * rng.random(800_000) ** 3).astype(np.int64), [n - 1]])
+    rows = np.concatenate([rng.integers(0, n, len(cols) - 1), [n - 1]])
+    S = sp.csr_matrix((np.ones(len(cols), np.int32), (rows, cols)), shape=(n, n))
+    S.sort_indices()
+    S = sp.csr_matrix((np.ones(S.nnz, bool), S.indices, S.indptr), shape=S.shape)
+    assert S.nnz >= (1 << 20) and S.nnz % 256
+    return S
+
+
 @functools.lru_cache(maxsize=None)
 def spmv_pattern(shape):
+    if shape == "skewed-wide":
+        return skewed_wide()
     if shape == "small":
         return pattern(11, 300, 400, 6)                       # 1800 entries: the run kernel on a small matrix
     if shape == "run":
@@ -120,7 +141,7 @@ def spmv_pattern(shape):
 
 def _spmv_expect(path, cfg, typ, add, mul, vxm):
     k = cfg["kernel"]
-    if path == "hot" and mul == ("SECOND" if vxm else "FIRST"):
+    if path.startswith("hot") and mul == ("SECOND" if vxm else "FIRST"):
         return "run"                                           # the multiply ignores u: no gathers for the hot table to serve
     return k
 
@@ -159,9 +180,14 @@ def run_spmv_path(path, typ):
                     want_k = _spmv_expect(path, cfg, typ, sr[0], sr[1], vxm)
                     form = "vxm" if vxm else "mxv"
                     assert entries(ks) == [want_k], (path, sr, form, ks)
+                    if want_k.startswith("run+hot"):
+                        assert f"ids={cfg['ids']}" in ks, (path, sr, form, ks)
                     gI, gX = w.to_arrays()
-                    ref = (orc.vxm(orc.SpVec(w.type.name, n_out), mo, None, sr, uo, Ao, "S" if mo else "") if vxm else
-                           orc.mxv(orc.SpVec(w.type.name, n_out), mo, None, sr, Ao, uo, "S" if mo else ""))
+                    if path == "hot-ids32":          # dense u of 2^24 entries, no mask: the oracle on the referenced entries of u
+                        ref = oracle_spmv(typ, sr, S, av, uv, vxm)
+                    else:
+                        ref = (orc.vxm(orc.SpVec(w.type.name, n_out), mo, None, sr, uo, Ao, "S" if mo else "") if vxm else
+                               orc.mxv(orc.SpVec(w.type.name, n_out), mo, None, sr, Ao, uo, "S" if mo else ""))
                     cands = _vec_products(uv, upres, S, av, sr[1], vxm) if sr[0] == "ANY" else None
                     e = compare(gI, gX, ref.I, ref.X, typ, sr[0], f"{form} {'_'.join(sr)}", cands)
                     if e:
@@ -179,10 +205,10 @@ def test_spmv_edges(path, typ):
 
 
 @pytest.mark.parametrize("typ", HOT_T)
-@pytest.mark.parametrize("path", ["hot"])
+@pytest.mark.parametrize("path", ["hot", "hot-ids32"])
 def test_spmv_hot_table_edges(path, typ):
-    """R-MAT scale 17: edge values land at hot and cold columns of u and inside hub rows that span many runs, whose
-    partials the fix-up kernel folds."""
+    """R-MAT scale 17 (3-byte ids): edge values land at hot and cold columns of u and inside hub rows that span many runs,
+    whose partials the fix-up kernel folds.  hot-ids32: the same on the 4-byte body."""
     run_spmv_path(path, typ)
 
 
@@ -378,7 +404,7 @@ def _general_values(rng, typ, n, scale):
     return x.astype(dt)
 
 
-BOUND_SPMV = ["tile-8", "run", "run-sparse-u", "hot"]
+BOUND_SPMV = ["tile-8", "run", "run-sparse-u", "hot", "hot-ids32"]
 
 
 @pytest.mark.parametrize("scale", ["normal", "subnormal"])
@@ -400,6 +426,8 @@ def test_fp_sums_within_error_bound(path, typ, scale):
             w = A.mxv(u, semiring=s)
             ks = _kernels()
         assert entries(ks) == [_spmv_expect(path, cfg, typ, "PLUS", "TIMES", False)], ks
+        if "ids" in cfg:
+            assert f"ids={cfg['ids']}" in ks, ks
         gI, gX = w.to_arrays()
         Ar = np.repeat(np.arange(nrows), np.diff(S.indptr))
         keep = upres[S.indices]
@@ -434,13 +462,13 @@ def test_fp_sums_within_error_bound(path, typ, scale):
 
 
 # ------------------------------------------------------------------ every path of the table was reached
-ALL_PATHS = {"run", "run (sparse u)", "run+hot-table (TMA-staged)", "pull",
+ALL_PATHS = {"run", "run (sparse u)", "run+hot-table (TMA-staged)", "ids=24", "ids=32", "pull",
              "push", "esc-small", "esc-medium", "spa", "masked-warp", "stream-S", "stream-M", "stream-L", "dot"}
 
 
 SPMV_CASES = ["tile-8", "run", "run-sparse-u", "pull", "push"]
 MIXED_PATHS = ["tile-8", "run", "esc-small", "spa", "masked-warp", "stream-L", "dot"]
-FULL_COUNT = (len(SPMV_CASES) * len(ALL_T) + len(HOT_T) + len(GEMM) * len(ALL_T) + len(MIXED_PATHS) * len(MIXED)
+FULL_COUNT = (len(SPMV_CASES) * len(ALL_T) + 2 * len(HOT_T) + len(GEMM) * len(ALL_T) + len(MIXED_PATHS) * len(MIXED)
               + (len(BOUND_SPMV) + len(GEMM)) * len(FP_T) * 2)
 
 

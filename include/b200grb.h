@@ -237,14 +237,23 @@ int64_t B200_debug_live_allocs(void);
 /* wide-route test seam: chunk > 0 puts every GrB_mxv / GrB_vxm, every transpose and the SpMM, dense-left and SDDMM routes of
  * GrB_mxm on the code that serves matrices with 2^32 or more entries (64-bit entry offsets; transposes and SDDMM masks cut into
  * chunks of `chunk` entries), whatever the matrix's size; 0 switches it off.  The 32-bit row offsets stay built for the other
- * operations */
+ * operations.  The unmasked and complemented-mask CSR x CSR products of GrB_mxm stay on their 32-bit kernels under it */
 void B200_debug_wide(int64_t chunk);
+/* wide-route test seam of the unmasked and complemented-mask CSR x CSR products of GrB_mxm: chunk > 0 puts every such product on
+ * the code that serves operands with 2^32 or more entries (row panels of A and of the mask's blocking entries with 32-bit
+ * offsets, B's 64-bit offsets), whatever the operands' size, with panels of at most `chunk` entries of A and of the mask.
+ * result_limit > 0 stands for 2^32 in that route's size rule (a product whose result would have that many entries or more
+ * is refused with GrB_INVALID_VALUE), and spa_budget > 0 for the 2^32 bytes the dense accumulators of one panel may take
+ * (0: the defaults).  chunk = 0 switches all three off */
+void B200_debug_wide_gemm(int64_t chunk, int64_t result_limit, int64_t spa_budget);
 /* kernel-path test seam: the paths the last GrB_mxv / GrB_vxm / GrB_mxm took, separated by ';' ("run",
  * "run (sparse u)", "run+hot-table (TMA-staged)", "pull", "push", "esc-small", "esc-medium", "spa", "spa-split", "masked-warp", "stream-L",
  * "dot", ...); recorded whether the burble is on or not, valid until the next such call.  Host-decided variants follow
  * their entry as "key=value" tokens: "filter=exact" or "filter=bloom" after each "stream-S" / "stream-M" / "stream-L"
  * (the mask-row membership filter is an exact bitmap or a one-hash Bloom filter), and "mxv=in-place" after an mxv / vxm
- * entry when the product was formed straight in w's buffers */
+ * entry when the product was formed straight in w's buffers.  "offsets=64" follows the first entry of a call that ran on the
+ * wide route (64-bit offsets).  An unmasked or complemented-mask product lists "esc-small", "esc-medium", "spa" and "spa-split"
+ * once each, in that order, however many row panels ran them, with "offsets=64" after the first on the wide route */
 const char *B200_debug_last_kernel(void);
 /* per-matrix SpGEMM/SpMV work figures of the most recent GrB_mxm (flops = number of
  * multiplies, nnz_out = nvals of the product T as the kernels formed it, before the accumulator and the write-back:

@@ -213,6 +213,10 @@ struct GBGlobal {
                                   // of mxm and its masked CSR x CSR methods (not complemented) on the wide route; transposes and
                                   // SDDMM masks go in chunks of this many entries, masked products in row panels of at most this
                                   // many entries of A and of M (a longer row makes a panel of its own)
+    // B200_debug_wide_gemm: chunk > 0 puts every unmasked and complemented-mask CSR x CSR mxm on the wide route, in row panels of
+    // at most this many entries of A and of M'; limit > 0 stands for 2^32 in that route's size rule, spa_budget > 0 for
+    // WIDE_SPA_BUDGET (spgemm.cu)
+    int64_t debug_wide_gemm = 0, debug_gemm_limit = 0, debug_spa_budget = 0;
     std::recursive_mutex mu;
 };
 extern GBGlobal G;
@@ -838,18 +842,25 @@ static inline GrB_Info source_csr(GrB_Matrix A, bool tran, Csr **out) {
 // T = a fresh nrows x ncols CSR formed row by row.  count(rowptr) enqueues the work that leaves all nrows + 1 slots defined:
 // the entry count of row r in slot r, 0 in slot nrows.  The slots are scanned into row offsets, T.nnz is read back, and T gets
 // col and, when vsize > 0, val (vsize bytes per entry, plus the 16-byte tail of every value array).  fill(T) writes them and
-// runs only when T has entries.  Both return GrB_Info.  rowptr32 is built last.
-template <typename Count, typename Fill>
-static GrB_Info csr_from_row_counts(int64_t nrows, int64_t ncols, size_t vsize, Csr &T, std::string *err, Count &&count, Fill &&fill) {
+// runs only when T has entries.  Both return GrB_Info.  rowptr32 is built last.  check(nnz), when given, sees T's entry count
+// before col and val are allocated, and its failure is the call's.
+template <typename Count, typename Fill, typename Check>
+static GrB_Info csr_from_row_counts(int64_t nrows, int64_t ncols, size_t vsize, Csr &T, std::string *err, Count &&count, Fill &&fill,
+                                    Check &&check) {
     T = Csr(); T.nrows = nrows; T.ncols = ncols;
     GB_TRY(T.rowptr.alloc((size_t)nrows + 1, err));
     GB_TRY(count(T.rowptr.get()));
     GB_TRY(dev_exclusive_scan(T.rowptr, nrows + 1, err));
     GB_TRY(read_i64(T.rowptr + nrows, &T.nnz, err));
+    GB_TRY(check(T.nnz));
     GB_TRY(T.col.alloc((size_t)T.nnz, err));
     if (vsize) GB_TRY(T.val.alloc((size_t)T.nnz * vsize + 16, err));
     if (T.nnz > 0) GB_TRY(fill(T));
     return dev_build_rowptr32(T, err);
+}
+template <typename Count, typename Fill>
+static GrB_Info csr_from_row_counts(int64_t nrows, int64_t ncols, size_t vsize, Csr &T, std::string *err, Count &&count, Fill &&fill) {
+    return csr_from_row_counts(nrows, ncols, vsize, T, err, count, fill, [](int64_t) { return GrB_SUCCESS; });
 }
 // T = src's pattern in fresh arrays, with a value array of vsize bytes per entry holding src's values when with_values
 // (device_ops.cu).  rowptr32 is left to the caller, to be built once the values are in place.

@@ -167,6 +167,11 @@ static int64_t g_fail_alloc = 0, g_live_allocs = 0;
 extern "C" void B200_debug_fail_alloc(int64_t k) { g_fail_alloc = k > 0 ? k : 0; }
 extern "C" int64_t B200_debug_live_allocs(void) { return g_live_allocs; }
 extern "C" void B200_debug_wide(int64_t chunk) { G.debug_wide = chunk > 0 ? chunk : 0; }
+extern "C" void B200_debug_wide_gemm(int64_t chunk, int64_t result_limit, int64_t spa_budget) {
+    G.debug_wide_gemm = chunk > 0 ? chunk : 0;
+    G.debug_gemm_limit = chunk > 0 && result_limit > 0 ? result_limit : 0;
+    G.debug_spa_budget = chunk > 0 && spa_budget > 0 ? spa_budget : 0;
+}
 extern "C" const char *B200_debug_last_kernel(void) { return G.last_kernel.c_str(); }
 
 GrB_Info dmalloc(void **p, size_t bytes, std::string *err) {

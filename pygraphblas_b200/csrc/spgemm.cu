@@ -189,8 +189,8 @@ __device__ __forceinline__ bool mask_blocks(const uint32_t *m_col, uint32_t ms, 
 // ------------------------------------------------------------------ unmasked, symbolic pass: shared-memory hash
 // One row per group (a warp, or the whole CTA): count its distinct columns (COMP: those not blocked by M', tested once per
 // distinct column, when it first enters the table).
-template <bool WARP, bool COMP = false>
-__global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
+template <bool WARP, bool COMP, typename BT>
+__global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgsT<BT> p) {
     extern __shared__ unsigned char smem_raw[];
     const int gsize = WARP ? 32 : blockDim.x;
     const int gid = WARP ? (threadIdx.x >> 5) : 0;
@@ -214,7 +214,7 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
         if (WARP) {       // lane per A entry, each lane walks its B row
             for (uint32_t pa = as + tid; pa < ae; pa += 32) {
                 const uint32_t k = p.a_col[pa];
-                for (uint32_t pb = p.b_ptr[k]; pb < p.b_ptr[k + 1]; ++pb) {
+                for (BT pb = p.b_ptr[k]; pb < p.b_ptr[k + 1]; ++pb) {
                     const uint32_t j = __ldg(p.b_col + pb);
                     uint32_t s = hash_col(j, hshift);
                     while (true) {
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(256) hash_symbolic_kernel(const GemmArgs p) {
             const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
             for (uint32_t pa = as + warp; pa < ae; pa += nwarps) {
                 const uint32_t k = p.a_col[pa];
-                for (uint32_t pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
+                for (BT pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
                     const uint32_t j = __ldg(p.b_col + pb);
                     uint32_t s = hash_col(j, hshift);
                     while (true) {
@@ -281,9 +281,11 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int *s_warp, int *tot
 static constexpr int ESC_SMALL = 128, ESC_MEDIUM = 2048;
 static constexpr size_t ESC_SMEM_SMALL = (size_t)8 * ESC_SMALL * 16;                       // 8 warps x (keys 8 B + value words 8 B)
 static constexpr size_t ESC_SMEM_MEDIUM = (size_t)ESC_MEDIUM * 16 + 3 * 256 * 4 + 256 * 8;   // + offsets, starts, lengths, A values of a chunk
+// the medium bin with B's 64-bit offsets: the B row starts of a chunk take 8 bytes each
+template <typename BT> static constexpr size_t esc_smem_medium() { return ESC_SMEM_MEDIUM + 256 * (sizeof(BT) - 4); }
 
-template <typename XT, typename ZT, int ADD, int MUL, bool WARP, bool COMP = false>
-__global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
+template <typename XT, typename ZT, int ADD, int MUL, bool WARP, bool COMP, typename BT>
+__global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgsT<BT> p) {
     typedef typename SlotWord<ZT>::W W;
     constexpr int CAP = WARP ? ESC_SMALL : ESC_MEDIUM;
     extern __shared__ unsigned char smem_raw[];
@@ -306,10 +308,10 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
     if constexpr (WARP) {
         for (uint32_t pa0 = as; pa0 < ae; pa0 += 32) {          // a lane per A entry, each lane walks its B row
             const uint32_t pa = pa0 + lane;
-            uint32_t bs = 0, len = 0; XT av = (XT)1;
+            BT bs = 0; uint32_t len = 0; XT av = (XT)1;
             if (pa < ae) {
                 const uint32_t k = p.a_col[pa];
-                bs = p.b_ptr[k]; len = p.b_ptr[k + 1] - bs;
+                bs = p.b_ptr[k]; len = (uint32_t)(p.b_ptr[k + 1] - bs);
                 if (p.need_a) av = gload<XT>(aval + pa);
             }
             int inc = (int)len;
@@ -328,14 +330,15 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
         }
     } else {
         uint32_t *s_off = reinterpret_cast<uint32_t *>(smem_raw + (size_t)CAP * 16);
-        uint32_t *s_bs = s_off + 256, *s_len = s_bs + 256;
+        BT *s_bs = reinterpret_cast<BT *>(s_off + 256);
+        uint32_t *s_len = reinterpret_cast<uint32_t *>(s_bs + 256);
         XT *s_av = reinterpret_cast<XT *>(s_len + 256);
         for (uint32_t pa0 = as; pa0 < ae; pa0 += 256) {         // a thread per A entry of the chunk, then a warp per entry, lanes along its B row
             const uint32_t pa = pa0 + threadIdx.x;
-            uint32_t bs = 0, len = 0; XT av = (XT)1;
+            BT bs = 0; uint32_t len = 0; XT av = (XT)1;
             if (pa < ae) {
                 const uint32_t k = p.a_col[pa];
-                bs = p.b_ptr[k]; len = p.b_ptr[k + 1] - bs;
+                bs = p.b_ptr[k]; len = (uint32_t)(p.b_ptr[k + 1] - bs);
                 if (p.need_a) av = gload<XT>(aval + pa);
             }
             int total = 0;
@@ -344,7 +347,8 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
             __syncthreads();
             const int nent = (int)min(256u, ae - pa0);
             for (int e = warp; e < nent; e += nwarps) {
-                const uint32_t o = s_off[e], b0 = s_bs[e], l = s_len[e];
+                const uint32_t o = s_off[e], l = s_len[e];
+                const BT b0 = s_bs[e];
                 const XT a = s_av[e];
                 for (uint32_t t = lane; t < l; t += 32) {
                     const uint32_t pos = o + t;
@@ -402,8 +406,8 @@ __global__ void __launch_bounds__(256) esc_numeric_kernel(const GemmArgs p) {
 
 // COMP: each CTA owns a second bitmap, the slice gridDim.x slices further on in spa_bits.  M'(row,:) is set into it when the
 // row starts and a product tests it before its atomics, so a blocked column costs no atomic; the sweep clears it.
-template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC, bool COMP = false>
-__global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
+template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC, bool COMP, typename BT>
+__global__ void __launch_bounds__(512) spa_kernel(const GemmArgsT<BT> p) {
     typedef typename SlotWord<ZT>::W W;
     __shared__ int s_warp[33];
     __shared__ unsigned int s_next;
@@ -434,7 +438,7 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
             const uint32_t k = p.a_col[pa];
             XT av = (XT)1;
             if (NUMERIC && p.need_a) av = gload<XT>(aval + pa);
-            for (uint32_t pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
+            for (BT pb = p.b_ptr[k] + lane; pb < p.b_ptr[k + 1]; pb += 32) {
                 const uint32_t j = __ldg(p.b_col + pb);
                 const uint32_t bit = 1u << (j & 31);
                 if (COMP && (mbits[j >> 5] & bit)) continue;
@@ -483,8 +487,9 @@ __global__ void __launch_bounds__(512) spa_kernel(const GemmArgs p) {
 // processed in groups; each row of a group (its slot) owns a dense accumulator, a presence bitmap and a bitmap of M'(row,:) in
 // HBM.  A(row,:) is cut into chunks of about CHUNK_FLOPS products (equal runs of A entries) that persistent CTAs take from a
 // queue.  The sweeps split each row into ranges of SPLIT_RANGE_WORDS bitmap words, one CTA per (range, slot).
-struct SplitArgs {
-    const uint32_t *a_col; const void *a_val; const uint32_t *b_ptr, *b_col; const void *b_val;
+// BT: the type of B's row offsets, as in GemmArgsT; A's positions in the chunk list are relative to the row panel
+template <typename BT> struct SplitArgsT {
+    const uint32_t *a_col; const void *a_val; const BT *b_ptr; const uint32_t *b_col; const void *b_val;
     const uint32_t *m_ptr, *m_col;
     const int32_t *rows;                 // the rows of the group, by slot
     const uint32_t *chunks;              // per chunk: slot, first A entry, end A entry
@@ -498,7 +503,7 @@ struct SplitArgs {
 static constexpr int64_t SPLIT_RANGE_WORDS = 2048;
 
 // M'(row,:) into the mask bitmap of every slot (blockIdx.y = slot)
-__global__ void split_mask_kernel(const SplitArgs s) {
+template <typename BT> __global__ void split_mask_kernel(const SplitArgsT<BT> s) {
     const int64_t row = s.rows[blockIdx.y];
     uint32_t *mb = s.mbit + (size_t)blockIdx.y * s.words;
     for (uint32_t q = s.m_ptr[row] + blockIdx.x * blockDim.x + threadIdx.x; q < s.m_ptr[row + 1]; q += gridDim.x * blockDim.x) {
@@ -507,8 +512,8 @@ __global__ void split_mask_kernel(const SplitArgs s) {
     }
 }
 
-template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC>
-__global__ void __launch_bounds__(512) split_chunk_kernel(const SplitArgs s) {
+template <typename XT, typename ZT, int ADD, int MUL, bool NUMERIC, typename BT>
+__global__ void __launch_bounds__(512) split_chunk_kernel(const SplitArgsT<BT> s) {
     typedef typename SlotWord<ZT>::W W;
     __shared__ unsigned int s_next;
     const int add = ADD >= 0 ? ADD : s.add_op;
@@ -529,7 +534,7 @@ __global__ void __launch_bounds__(512) split_chunk_kernel(const SplitArgs s) {
             const uint32_t k = s.a_col[pa];
             XT av = (XT)1;
             if (NUMERIC && s.need_a) av = gload<XT>(aval + pa);
-            for (uint32_t pb = s.b_ptr[k] + lane; pb < s.b_ptr[k + 1]; pb += 32) {
+            for (BT pb = s.b_ptr[k] + lane; pb < s.b_ptr[k + 1]; pb += 32) {
                 const uint32_t j = __ldg(s.b_col + pb);
                 const uint32_t bit = 1u << (j & 31);
                 if (mb[j >> 5] & bit) continue;
@@ -544,8 +549,8 @@ __global__ void __launch_bounds__(512) split_chunk_kernel(const SplitArgs s) {
 }
 
 // popcount of one (range, slot): symbolic (CLEAR) adds it to c_cnt[row] and clears both bitmaps of the range; numeric stores it
-template <bool CLEAR>
-__global__ void __launch_bounds__(256) split_count_kernel(const SplitArgs s) {
+template <bool CLEAR, typename BT>
+__global__ void __launch_bounds__(256) split_count_kernel(const SplitArgsT<BT> s) {
     __shared__ int s_warp[33];
     const int64_t slot = blockIdx.y, r = blockIdx.x;
     const int64_t w0 = r * SPLIT_RANGE_WORDS, w1 = min(w0 + SPLIT_RANGE_WORDS, s.words);
@@ -566,8 +571,8 @@ __global__ void __launch_bounds__(256) split_count_kernel(const SplitArgs s) {
 
 // ordered sweep of one (range, slot): the entries go out sorted at c_ptr[row] + (their range's offset within the row), the
 // accumulator words are reset to ident and both bitmaps cleared
-template <typename ZT>
-__global__ void __launch_bounds__(256) split_fill_kernel(const SplitArgs s, typename SlotWord<ZT>::W ident) {
+template <typename ZT, typename BT>
+__global__ void __launch_bounds__(256) split_fill_kernel(const SplitArgsT<BT> s, typename SlotWord<ZT>::W ident) {
     typedef typename SlotWord<ZT>::W W;
     __shared__ int s_warp[33];
     const int64_t slot = blockIdx.y, r = blockIdx.x;
@@ -942,14 +947,15 @@ struct SplitPlan {
     DevBuf<unsigned int> queue;
 };
 
-static GrB_Info split_prepare(const RowBins &bins, const int64_t *flops, const Csr &A, int64_t ncols, size_t wsize, SplitPlan &sp,
+// a_ptr: the 32-bit offsets of the row panel; the chunks' A positions are relative to it
+static GrB_Info split_prepare(const RowBins &bins, const int64_t *flops, const uint32_t *a_ptr, int64_t ncols, size_t wsize, SplitPlan &sp,
                               std::string *err) {
     const unsigned int n3 = bins.count[3];
     DevBuf<unsigned int> cnt; DevBuf<int64_t> picked;
     GB_TRY(cnt.alloc(2, err));
     CU_TRY(cudaMemsetAsync(cnt, 0, 8, G.stream), err);
     GB_TRY(sp.keep.alloc(n3, err)); GB_TRY(picked.alloc((size_t)4 * n3, err));
-    split_pick_kernel<<<grid_for(n3), 256, 0, G.stream>>>(bins.rows + bins.offset[3], n3, flops, SPLIT_FLOPS, A.rowptr32, sp.keep, picked, cnt);
+    split_pick_kernel<<<grid_for(n3), 256, 0, G.stream>>>(bins.rows + bins.offset[3], n3, flops, SPLIT_FLOPS, a_ptr, sp.keep, picked, cnt);
     GB_LAUNCHED();
     unsigned int h[2];
     GB_TRY(read_counts(cnt, h, 2, err));
@@ -995,21 +1001,22 @@ static GrB_Info split_prepare(const RowBins &bins, const int64_t *flops, const C
 }
 
 // the launches of group g: its mask bitmaps, then the chunk kernel on a fresh queue; returns the group's argument block
-static SplitArgs split_group(const SplitPlan &sp, const SplitArgs &base, int64_t g, int64_t *ng, std::string *err) {
-    SplitArgs s = base;
+template <typename BT>
+static SplitArgsT<BT> split_group(const SplitPlan &sp, const SplitArgsT<BT> &base, int64_t g, int64_t *ng, std::string *err) {
+    SplitArgsT<BT> s = base;
     s.rows = sp.rows + g * sp.group;
     *ng = std::min(sp.group, sp.nsplit - g * sp.group);
     s.chunks = sp.chunks + 3 * sp.chunk_off[g];
     s.nchunks = sp.chunk_off[g + 1] - sp.chunk_off[g];
-    split_mask_kernel<<<dim3((unsigned)std::min<int64_t>(ceil_div(sp.ncols, 256), 128), (unsigned)*ng), 256, 0, G.stream>>>(s);
+    split_mask_kernel<BT><<<dim3((unsigned)std::min<int64_t>(ceil_div(sp.ncols, 256), 128), (unsigned)*ng), 256, 0, G.stream>>>(s);
     GB_LAUNCHED();
     cudaMemsetAsync(s.queue, 0, 4, G.stream);          // errors surface at the caller's cudaGetLastError
     return s;
 }
 static int split_ctas(int64_t nchunks) { return (int)std::max<int64_t>(1, std::min<int64_t>(nchunks, (int64_t)G.num_sms * 2)); }
 
-template <typename XT, typename ZT, int ADD, int MUL>
-static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgs &base, std::string *err) {
+template <typename XT, typename ZT, int ADD, int MUL, typename BT>
+static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgsT<BT> &base, std::string *err) {
     typedef typename SlotWord<ZT>::W W;
     const int add = ADD >= 0 ? ADD : base.add_op;
     fill_words_kernel<W><<<grid_for(sp.group * sp.ncols), 256, 0, G.stream>>>(static_cast<W *>(sp.acc), pack_slot<ZT>(accum_init<ZT>(add)),
@@ -1017,30 +1024,47 @@ static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgs &base, std::s
     GB_LAUNCHED();
     for (int64_t g = 0; g + 1 < (int64_t)sp.chunk_off.size(); ++g) {
         int64_t ng = 0;
-        const SplitArgs s = split_group(sp, base, g, &ng, err);
-        split_chunk_kernel<XT, ZT, ADD, MUL, true><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
-        split_count_kernel<false><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
+        const SplitArgsT<BT> s = split_group<BT>(sp, base, g, &ng, err);
+        split_chunk_kernel<XT, ZT, ADD, MUL, true, BT><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
+        split_count_kernel<false, BT><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
         CU_TRY(cudaMemsetAsync(sp.range_cnt + ng * sp.nrange, 0, 8, G.stream), err);
         GB_TRY(dev_exclusive_scan(sp.range_cnt, ng * sp.nrange + 1, err));
-        split_fill_kernel<ZT><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s, pack_slot<ZT>(accum_init<ZT>(add)));
+        split_fill_kernel<ZT, BT><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s, pack_slot<ZT>(accum_init<ZT>(add)));
         G.launches += 4;
     }
     CU_TRY(cudaGetLastError(), err);
     return GrB_SUCCESS;
 }
 
-// T = A (+).(x) B, unmasked.  A and B values already of the multiply's operand type.  With Mb (the entries of a complemented
-// mask that block, see mask_true_pattern) holding entries, T = (A (+).(x) B)<!Mb>: the same bins, chosen by the unfiltered
-// product counts, run their COMP instantiations, which never form a blocked entry.
-static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt,
-                                int add, int mul, bool need_a, bool need_b, const Csr *Mb, Csr &T, std::string *err) {
-    const int64_t nrows = A.nrows, ncols = B.ncols;
-    const bool comp = Mb && Mb->nnz > 0;
+// One row panel of an unmasked or complemented product: nrows rows of A and of M' (the entries of a complemented mask that
+// block, see mask_true_pattern), with 32-bit offsets relative to the panel's first entries (the narrow route: the whole
+// matrices, their rowptr32).  m_ptr is null when no entry blocks.
+struct UnmaskedPanel {
+    const uint32_t *a_ptr, *a_col; const void *a_val;
+    const uint32_t *m_ptr, *m_col;
+    int64_t nrows;
+};
+// the bins a call ran (esc-small, esc-medium, spa, spa-split): reported once each, in this order, however many panels ran them
+struct UnmaskedUse { bool bin[4] = {false, false, false, false}; };
+// the wide route's size rule, counted over the panels: the entries of T formed so far, refused on reaching `limit`
+struct ResultCount { int64_t limit = 0, total = 0; };
+static const char *const WIDE_RESULT_REFUSAL = "GrB_mxm: results of >= 2^32 entries are not supported with an operand of >= 2^32 entries";
+
+// T = A (+).(x) B on one panel, unmasked.  A and B values already of the multiply's operand type.  With P.m_ptr set,
+// T = (A (+).(x) B)<!M'>: the same bins, chosen by the unfiltered product counts, run their COMP instantiations, which never form
+// a blocked entry.  BT: the type of B's row offsets (b_ptr).  spa_budget > 0 caps the dense-accumulator CTAs at that many bytes
+// of accumulators and bitmaps (the wide route; the narrow one runs 2 per SM).  rc (the wide route, when the size rule counts):
+// the panel is refused, before its entries are allocated, when T would reach rc->limit entries.  G.last_flops grows by the panel's products.
+template <typename BT>
+static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
+                                bool need_a, bool need_b, int64_t spa_budget, UnmaskedUse &use, ResultCount *rc, Csr &T, std::string *err) {
+    const int64_t nrows = P.nrows, ncols = B.ncols;
+    const bool comp = P.m_ptr != nullptr;
     const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
     RowBins bins;
     SplitPlan sp;
-    GemmArgs g{};
-    SplitArgs sa{};
+    GemmArgsT<BT> g{};
+    SplitArgsT<BT> sa{};
     const int32_t *spa_rows = nullptr;
     int64_t spa_n = 0;
     int spa_ctas = 1;
@@ -1051,24 +1075,28 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
         DevBuf<int64_t> flops; DevBuf<unsigned long long> total;
         GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
         CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
-        flops_kernel<uint32_t><<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr32, A.col, B.rowptr32, nrows, flops, total); GB_LAUNCHED();
+        flops_kernel<BT><<<grid_for(nrows * 32), 256, 0, G.stream>>>(P.a_ptr, P.a_col, b_ptr, nrows, flops, total); GB_LAUNCHED();
         GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
         int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
-        G.last_flops = (uint64_t)total_flops;
+        G.last_flops += (uint64_t)total_flops;
         // the dense-accumulator bin: with a complemented mask its rows above SPLIT_FLOPS go to spa-split
-        if (comp && bins.count[3]) GB_TRY(split_prepare(bins, flops, A, ncols, wsize, sp, err));
+        if (comp && bins.count[3]) GB_TRY(split_prepare(bins, flops, P.a_ptr, ncols, wsize, sp, err));
         spa_rows = sp.nsplit ? sp.keep.get() : bins.rows + bins.offset[3];
         spa_n = sp.nsplit ? sp.nkeep : (int64_t)bins.count[3];
         flops.reset(); total.reset();
 
-        g.a_ptr = A.rowptr32; g.a_col = A.col; g.a_val = aval; g.b_ptr = B.rowptr32; g.b_col = B.col; g.b_val = bval;
+        g.a_ptr = P.a_ptr; g.a_col = P.a_col; g.a_val = P.a_val; g.b_ptr = b_ptr; g.b_col = B.col; g.b_val = bval;
         g.nrows = nrows; g.ncols = ncols; g.add_op = add; g.mul_op = mul; g.need_a = need_a; g.need_b = need_b;
         g.c_cnt = cnt;
-        if (comp) { g.m_ptr = Mb->rowptr32; g.m_col = Mb->col; }
-        sa.a_col = A.col; sa.a_val = aval; sa.b_ptr = B.rowptr32; sa.b_col = B.col; sa.b_val = bval; sa.m_ptr = g.m_ptr; sa.m_col = g.m_col;
+        if (comp) { g.m_ptr = P.m_ptr; g.m_col = P.m_col; }
+        sa.a_col = P.a_col; sa.a_val = P.a_val; sa.b_ptr = b_ptr; sa.b_col = B.col; sa.b_val = bval; sa.m_ptr = g.m_ptr; sa.m_col = g.m_col;
         sa.queue = sp.queue; sa.pres = sp.pres; sa.mbit = sp.mbit; sa.acc = sp.acc; sa.words = sp.words; sa.ncols = ncols; sa.nrange = sp.nrange;
         sa.add_op = add; sa.mul_op = mul; sa.need_a = need_a; sa.need_b = need_b; sa.c_cnt = cnt; sa.range_cnt = sp.range_cnt;
         spa_ctas = std::max(1, std::min<int>((int)spa_n, G.num_sms * 2));
+        if (spa_budget > 0 && spa_n) {  // one CTA's accumulator, presence bitmap and (comp) mask bitmap: ncols > 0 here
+            const int64_t per_cta = ncols * (int64_t)wsize + ceil_div(ncols, 32) * 4 * (comp ? 2 : 1);
+            spa_ctas = (int)std::max<int64_t>(1, std::min<int64_t>(spa_budget / per_cta, spa_ctas));
+        }
         if (spa_n) {
             g.spa_words = ceil_div(ncols, 32);
             const size_t words = (size_t)spa_ctas * g.spa_words * (comp ? 2 : 1);     // comp: + the mask bitmaps
@@ -1078,30 +1106,32 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
             GB_TRY(queue.alloc(2, err));
             CU_TRY(cudaMemsetAsync(queue, 0, 8, G.stream), err);
         }
-        // the bins are reported here: a complemented mask may block every product, and then the numeric pass does not run
+        // the bins are recorded here: a complemented mask may block every product, and then the numeric pass does not run
         if (bins.count[1]) {
             g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1]; g.table = SMALL_TABLE;
-            (comp ? hash_symbolic_kernel<true, true> : hash_symbolic_kernel<true>)<<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g);
-            GB_LAUNCHED(); gb_kernel_used("esc-small");
+            (comp ? hash_symbolic_kernel<true, true, BT> : hash_symbolic_kernel<true, false, BT>)
+                <<<(unsigned)ceil_div(g.nbin, 8), 256, 8 * SMALL_TABLE * 4, G.stream>>>(g);
+            GB_LAUNCHED(); use.bin[0] = true;
         }
         if (bins.count[2]) {
             g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2]; g.table = MEDIUM_TABLE;
-            (comp ? hash_symbolic_kernel<false, true> : hash_symbolic_kernel<false>)<<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g);
-            GB_LAUNCHED(); gb_kernel_used("esc-medium");
+            (comp ? hash_symbolic_kernel<false, true, BT> : hash_symbolic_kernel<false, false, BT>)
+                <<<(unsigned)g.nbin, 256, MEDIUM_TABLE * 4, G.stream>>>(g);
+            GB_LAUNCHED(); use.bin[1] = true;
         }
         if (spa_n) {
             g.rows = spa_rows; g.nbin = spa_n; g.queue = queue;
-            (comp ? spa_kernel<bool, bool, -1, -1, false, true> : spa_kernel<bool, bool, -1, -1, false>)<<<spa_ctas, 512, 0, G.stream>>>(g);
-            GB_LAUNCHED(); gb_kernel_used("spa");
+            (comp ? spa_kernel<bool, bool, -1, -1, false, true, BT> : spa_kernel<bool, bool, -1, -1, false, false, BT>)<<<spa_ctas, 512, 0, G.stream>>>(g);
+            GB_LAUNCHED(); use.bin[2] = true;
         }
         for (int64_t k = 0; k + 1 < (int64_t)sp.chunk_off.size(); ++k) {
             int64_t ng = 0;
-            const SplitArgs s = split_group(sp, sa, k, &ng, err);
-            split_chunk_kernel<bool, bool, -1, -1, false><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
-            split_count_kernel<true><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
+            const SplitArgsT<BT> s = split_group<BT>(sp, sa, k, &ng, err);
+            split_chunk_kernel<bool, bool, -1, -1, false, BT><<<split_ctas(s.nchunks), 512, 0, G.stream>>>(s);
+            split_count_kernel<true, BT><<<dim3((unsigned)sp.nrange, (unsigned)ng), 256, 0, G.stream>>>(s);
             G.launches += 2;
         }
-        if (sp.nsplit) gb_kernel_used("spa-split");
+        if (sp.nsplit) use.bin[3] = true;
         return GrB_SUCCESS;
     };
     // ---- numeric (shared-memory bins: expand-sort-compress)
@@ -1109,14 +1139,14 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
         g.c_ptr = t.rowptr; g.c_col = t.col; g.c_val = t.val;
         if (bins.count[1]) {
             g.rows = bins.rows + bins.offset[1]; g.nbin = bins.count[1];
-#define K_ESC_SMALL(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, true, true> : esc_numeric_kernel<XT, ZT, A_, M_, true>) \
+#define K_ESC_SMALL(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, true, true, BT> : esc_numeric_kernel<XT, ZT, A_, M_, true, false, BT>) \
                 <<<(unsigned)ceil_div(g.nbin, 8), 256, ESC_SMEM_SMALL, G.stream>>>(g)
             GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_SMALL, err); GB_LAUNCHED();
         }
         if (bins.count[2]) {
             g.rows = bins.rows + bins.offset[2]; g.nbin = bins.count[2];
-#define K_ESC_MEDIUM(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, false, true> : esc_numeric_kernel<XT, ZT, A_, M_, false>) \
-                <<<(unsigned)g.nbin, 256, ESC_SMEM_MEDIUM, G.stream>>>(g)
+#define K_ESC_MEDIUM(XT, ZT, A_, M_) (comp ? esc_numeric_kernel<XT, ZT, A_, M_, false, true, BT> : esc_numeric_kernel<XT, ZT, A_, M_, false, false, BT>) \
+                <<<(unsigned)g.nbin, 256, esc_smem_medium<BT>(), G.stream>>>(g)
             GB_FOR_SEMIRING(xt, zt, add, mul, K_ESC_MEDIUM, err); GB_LAUNCHED();
         }
         if (spa_n) {
@@ -1126,20 +1156,26 @@ static GrB_Info spgemm_unmasked(const Csr &A, const Csr &B, const void *aval, co
             g.spa_val = spa_val;
 #define K_SPA(XT, ZT, A_, M_) do { \
             fill_accum_init<ZT>(g.spa_val, (int64_t)spa_ctas * ncols, (A_) >= 0 ? (A_) : add); \
-            (comp ? spa_kernel<XT, ZT, A_, M_, true, true> : spa_kernel<XT, ZT, A_, M_, true>)<<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
+            (comp ? spa_kernel<XT, ZT, A_, M_, true, true, BT> : spa_kernel<XT, ZT, A_, M_, true, false, BT>)<<<spa_ctas, 512, 0, G.stream>>>(g); } while (0)
             GB_FOR_SEMIRING(xt, zt, add, mul, K_SPA, err); G.launches += 2;
         }
         if (sp.nsplit) {
             sa.c_ptr = t.rowptr; sa.c_col = t.col; sa.c_val = t.val;
-#define K_SPLIT(XT, ZT, A_, M_) GB_TRY((split_numeric<XT, ZT, A_, M_>(sp, sa, err)))
+#define K_SPLIT(XT, ZT, A_, M_) GB_TRY((split_numeric<XT, ZT, A_, M_, BT>(sp, sa, err)))
             GB_FOR_SEMIRING(xt, zt, add, mul, K_SPLIT, err);
         }
         spa_bits.reset(); queue.reset(); bins.rows.reset();
         return GrB_SUCCESS;
     };
-    GB_TRY(csr_from_row_counts(nrows, ncols, tc_size(zt), T, err, symbolic, numeric));
-    G.last_nnz_out = (uint64_t)T.nnz;
-    return GrB_SUCCESS;
+    // the size rule: checked on the panel's entry count after the scan, before its arrays are allocated
+    auto check = [&](int64_t nnz) {
+        if (rc) {
+            rc->total += nnz;
+            if (rc->total >= rc->limit) return gb_fail(GrB_INVALID_VALUE, err, "%s", WIDE_RESULT_REFUSAL);
+        }
+        return GrB_SUCCESS;
+    };
+    return csr_from_row_counts(nrows, ncols, tc_size(zt), T, err, symbolic, numeric, check);
 }
 
 // T<M> = A (+).(x) B restricted to a non-complemented mask M (pattern of T is a subset of M's).
@@ -1317,6 +1353,34 @@ __global__ void panel_rowptr_kernel(const int64_t *ptr, int64_t r0, int64_t n, u
     for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= n; r += (int64_t)gridDim.x * blockDim.x) out[r] = (uint32_t)(ptr[r0 + r] - base);
 }
 
+// The size rule of the unmasked wide route, in one pass over A's 64-bit offsets: total[0] += the products of every row (U, an upper
+// bound on nnz(T)), total[1] += max(0, nnz of the longest B row named by A(i,:) - nnz(M'(i,:))) (L: that B row lies in T(i,:) but
+// for what M' blocks, so L is a lower bound on nnz(T)).  m_ptr: M''s offsets, null without a complemented mask.  Warp per row.
+template <typename BT>
+__global__ void gemm_bound_kernel(const int64_t *a_ptr, const uint32_t *a_col, const BT *b_ptr, const int64_t *m_ptr, int64_t nrows,
+                                  unsigned long long *total) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    unsigned long long u = 0, l = 0;
+    for (int64_t r = warp; r < nrows; r += nwarps) {
+        int64_t f = 0, longest = 0;
+        for (int64_t p = a_ptr[r] + lane; p < a_ptr[r + 1]; p += 32) {
+            const uint32_t k = a_col[p];
+            const int64_t len = (int64_t)(b_ptr[k + 1] - b_ptr[k]);
+            f += len; longest = max(longest, len);
+        }
+        for (int o = 16; o > 0; o >>= 1) {
+            f += __shfl_xor_sync(0xffffffffu, f, o);
+            longest = max(longest, (int64_t)__shfl_xor_sync(0xffffffffu, longest, o));
+        }
+        if (m_ptr) longest -= m_ptr[r + 1] - m_ptr[r];
+        if (lane == 0) { u += (unsigned long long)f; if (longest > 0) l += (unsigned long long)longest; }
+    }
+    if (lane == 0 && u) atomicAdd(&total[0], u);
+    if (lane == 0 && l) atomicAdd(&total[1], l);
+}
+
 template <typename BT>
 static GrB_Info spgemm_masked_wide(const Csr &A, const Csr &B, const BT *b_ptr, const void *aval, const void *bval, int xt, int zt,
                                    int add, int mul, bool need_a, bool need_b, const Csr &M, int mtc, bool m_struct, bool dot,
@@ -1395,6 +1459,133 @@ static void masked_report(const MaskedUse &u, bool wide) {
         entry(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
         gb_kernel_used(u.exact[k] ? "filter=exact" : "filter=bloom");
     }
+}
+
+// ------------------------------------------------------------------ the wide route of the unmasked and complemented-mask bins
+// The same row panels as the masked route's (of A and M', the entries of a complemented mask that block): each panel runs the
+// whole pipeline (flops, bins, symbolic, scan, numeric) into a CSR of its rows; T is the one panel, or is formed from the panels'
+// row counts and entries.  B is read through its 64-bit offsets when it is wide.  The route forms results of fewer than 2^32
+// entries: T would take 34 GB or more in FP32 (twice that while the panels are joined), which does not fit beside a wide operand
+// on an 80 GB card.  gemm_bound_kernel bounds nnz(T) before any panel runs: L >= the limit is refused at once; U < the limit
+// needs no further check; otherwise the panels' symbolic counts are added up and the call refused as soon as the scan of a
+// panel's counts reaches the limit, before that panel's entries are allocated or formed.  The dense accumulators of a panel are capped at WIDE_SPA_BUDGET bytes (one FP32 accumulator is
+// 1 GB at n = 2^28).
+static constexpr int64_t WIDE_RESULT = (int64_t)1 << 32;
+static constexpr int64_t WIDE_SPA_BUDGET = (int64_t)1 << 32;
+// the route of a CSR x CSR product without a (non-complemented) mask: a CSR without rowptr32, or any CSR under B200_debug_wide_gemm
+static inline bool gemm_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide_gemm > 0; }
+
+template <typename BT>
+static GrB_Info spgemm_unmasked_wide(const Csr &A, const Csr &B, const BT *b_ptr, const void *aval, const void *bval, int xt, int zt,
+                                     int add, int mul, bool need_a, bool need_b, const Csr *Mb, UnmaskedUse &use, Csr &T,
+                                     std::string *err) {
+    const int64_t nrows = A.nrows, ncols = B.ncols;
+    const bool comp = Mb && Mb->nnz > 0;
+    const size_t zsz = (size_t)tc_size(zt), asz = need_a ? (size_t)tc_size(xt) : 0;
+    const bool seam = G.debug_wide_gemm > 0;
+    const int64_t bound = std::min(seam ? G.debug_wide_gemm : WIDE_PANEL, WIDE_PANEL);
+    const int64_t budget = seam && G.debug_spa_budget > 0 ? G.debug_spa_budget : WIDE_SPA_BUDGET;
+    ResultCount rc;
+    rc.limit = seam && G.debug_gemm_limit > 0 ? G.debug_gemm_limit : WIDE_RESULT;
+    const int64_t *m_ptr = comp ? Mb->rowptr.get() : nullptr;
+    bool counting = false;
+    if (nrows > 0) {
+        DevBuf<unsigned long long> tot;
+        GB_TRY(tot.alloc(2, err));
+        CU_TRY(cudaMemsetAsync(tot, 0, 16, G.stream), err);
+        gemm_bound_kernel<BT><<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr, A.col, b_ptr, m_ptr, nrows, tot); GB_LAUNCHED();
+        unsigned long long h[2];
+        CU_TRY(cudaMemcpyAsync(h, tot, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
+        CU_TRY(cudaStreamSynchronize(G.stream), err);
+        if (h[1] >= (unsigned long long)rc.limit) return gb_fail(GrB_INVALID_VALUE, err, "%s", WIDE_RESULT_REFUSAL);
+        counting = h[0] >= (unsigned long long)rc.limit;
+    }
+    std::vector<Csr> parts;
+    DevBuf<int64_t> ends;
+    GB_TRY(ends.alloc(4, err));
+    // the panel that starts at row r0, formed into `part`; *r1 = its end.  Without M', A's offsets stand in for panel_end_kernel's M.
+    auto panel = [&](int64_t r0, int64_t *r1, Csr &part) -> GrB_Info {
+        panel_end_kernel<<<1, 1, 0, G.stream>>>(A.rowptr, comp ? m_ptr : A.rowptr.get(), r0, nrows, bound, WIDE_PANEL_ROWS, ends); GB_LAUNCHED();
+        int64_t h[4];
+        CU_TRY(cudaMemcpyAsync(h, ends, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
+        CU_TRY(cudaStreamSynchronize(G.stream), err);
+        *r1 = h[0];
+        const int64_t a0 = h[1], m0 = h[2], pn = *r1 - r0;
+        uint32_t *ap = nullptr, *mp = nullptr;
+        GB_TRY(ws_array(WS_PANEL_A, &ap, (size_t)pn + 1, err));
+        panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(A.rowptr, r0, pn, ap); GB_LAUNCHED();
+        if (comp) {
+            GB_TRY(ws_array(WS_PANEL_M, &mp, (size_t)pn + 1, err));
+            panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(m_ptr, r0, pn, mp); GB_LAUNCHED();
+        }
+        const UnmaskedPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr,
+                              mp, comp ? Mb->col + m0 : nullptr, pn};
+        return spgemm_unmasked<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, budget, use, counting ? &rc : nullptr, part, err);
+    };
+    int64_t r1 = 0;
+    if (nrows > 0) {
+        parts.emplace_back();
+        GB_TRY(panel(0, &r1, parts[0]));
+        if (r1 == nrows) {                      // one panel: it is T
+            T = std::move(parts[0]);
+            return GrB_SUCCESS;
+        }
+    }
+    return csr_from_row_counts(nrows, ncols, zsz, T, err,
+        [&](int64_t *rowptr) {
+            CU_TRY(cudaMemsetAsync(rowptr + nrows, 0, 8, G.stream), err);
+            for (int64_t r0 = 0, q = 0; r0 < nrows; r0 = r1, ++q) {
+                if (q > 0) { parts.emplace_back(); GB_TRY(panel(r0, &r1, parts.back())); }
+                else r1 = parts[0].nrows;
+                row_len_kernel<<<grid_for(r1 - r0), 256, 0, G.stream>>>(parts.back().rowptr32, r1 - r0, rowptr + r0); GB_LAUNCHED();
+            }
+            return GrB_SUCCESS;
+        },
+        [&](Csr &t) {
+            int64_t at = 0;
+            for (Csr &part : parts) {
+                if (part.nnz) {
+                    CU_TRY(cudaMemcpyAsync(t.col.get() + at, part.col, (size_t)part.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
+                    CU_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(t.val.get()) + at * zsz, part.val, (size_t)part.nnz * zsz,
+                                           cudaMemcpyDeviceToDevice, G.stream), err);
+                }
+                at += part.nnz;
+                part = Csr();
+            }
+            return GrB_SUCCESS;
+        });
+}
+
+static void unmasked_report(const UnmaskedUse &u, bool wide) {
+    static const char *const names[4] = {"esc-small", "esc-medium", "spa", "spa-split"};
+    bool first = true;
+    for (int k = 0; k < 4; ++k) {
+        if (!u.bin[k]) continue;
+        gb_kernel_used(names[k]);
+        if (first && wide) gb_kernel_used("offsets=64");
+        first = false;
+    }
+}
+
+// T = A (+).(x) B, unmasked, or (A (+).(x) B)<!Mb> with Mb the entries of a complemented mask that block.  The narrow route runs
+// the bins once on the whole of A and Mb; the wide route (an operand or the mask of 2^32 or more entries, or B200_debug_wide_gemm)
+// on row panels, with B's 64-bit offsets when B is wide.
+static GrB_Info spgemm_unmasked_call(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt, int add, int mul,
+                                     bool need_a, bool need_b, const Csr *Mb, bool wide, Csr &T, std::string *err) {
+    const bool comp = Mb && Mb->nnz > 0;
+    UnmaskedUse use;
+    G.last_flops = 0;
+    if (!wide) {
+        const UnmaskedPanel P{A.rowptr32, A.col, aval, comp ? Mb->rowptr32.get() : nullptr, comp ? Mb->col.get() : nullptr, A.nrows};
+        GB_TRY(spgemm_unmasked<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, 0, use, nullptr, T, err));
+    } else if (gemm_wide(B)) {
+        GB_TRY(spgemm_unmasked_wide<int64_t>(A, B, B.rowptr.get(), aval, bval, xt, zt, add, mul, need_a, need_b, Mb, use, T, err));
+    } else {
+        GB_TRY(spgemm_unmasked_wide<uint32_t>(A, B, B.rowptr32.get(), aval, bval, xt, zt, add, mul, need_a, need_b, Mb, use, T, err));
+    }
+    G.last_nnz_out = (uint64_t)T.nnz;
+    unmasked_report(use, wide);
+    return GrB_SUCCESS;
 }
 
 // The narrow route runs the masked methods once on the whole of A and M; the wide route (csr_wide: an operand of 2^32 or more
@@ -1522,7 +1713,7 @@ struct MxmPos { int side = 0; int tc = 0; int64_t off = 0; const uint64_t *ids =
 // T = op(A) (+).(x) op(B) under Mask (*masked tells the write-back): a mask that is not complemented selects the masked
 // methods; a complemented one runs the unmasked bins with the filter of the entries that block (DESIGN.md section 3.2)
 static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, int zt, int add, int mul, const GrB_Matrix A, const GrB_Matrix B,
-                            const MxmPos &pos, Csr &T, bool *masked, std::string *err) {
+                            const MxmPos &pos, GbBurble &burble, Csr &T, bool *masked, std::string *err) {
     const bool need_a = mul_reads_x(mul), need_b = mul_reads_y(mul);
     const bool use_mask = Mask && !f.mask_comp;
     *masked = Mask != nullptr;
@@ -1535,9 +1726,12 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
     if (Mask) GB_TRY(matrix_ensure_device(Mask));
     const Csr &a = *pa;
     const Csr &b = (f.tran1 && !dot) ? B->devT : B->dev;
-    // the masked methods have a wide route (spgemm_masked); the unmasked and complemented-mask bins have 32-bit offsets only
-    if (!use_mask && (!a.rowptr32 || !b.rowptr32 || (Mask && !Mask->dev.rowptr32)))
-        return gb_fail(GrB_INVALID_VALUE, err, "GrB_mxm: operands with >= 2^32 entries are not supported");
+    // the unmasked and complemented-mask bins take their wide route when an operand or the mask is wide (spgemm_unmasked_call);
+    // the masked methods choose theirs in spgemm_masked
+    const bool wide = !use_mask && (gemm_wide(a) || gemm_wide(b) || (Mask && gemm_wide(Mask->dev)));
+    if (wide && burble.on)
+        burble.note("spgemm, 64-bit offsets", (double)a.nnz * (4.0 + (need_a ? tc_size(xt) : 0)) + (double)b.nnz * (4.0 + (need_b ? tc_size(xt) : 0)) +
+                                              (double)(a.nrows + b.nrows + 2) * 8);
 
     DevBuf<void> a_cast, b_cast;
     const void *aval = a.val, *bval = b.val;
@@ -1560,7 +1754,7 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
         const Csr *mb = nullptr;
         if (Mask && f.mask_struct) mb = &Mask->dev;
         else if (Mask) { GB_TRY(mask_true_pattern(Mask->dev, Mask->type->code, mtrue, err)); mb = &mtrue; }
-        r = spgemm_unmasked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, T, err);
+        r = spgemm_unmasked_call(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, wide, T, err);
     }
     a_cast.reset(); b_cast.reset();
     return r;
@@ -1600,7 +1794,7 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
     if (A->dn.valid && !B->dn.valid && op_mirror(mul) >= 0 && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))
         return spmm_left_mxm(C, Mask, accum, semiring, A, B, f, burble);                            // dense X on the left
     Csr T; bool masked = false;
-    GB_TRY(mxm_product(Mask, f, xt, zt, add, mul, A, B, MxmPos(), T, &masked, err));
+    GB_TRY(mxm_product(Mask, f, xt, zt, add, mul, A, B, MxmPos(), burble, T, &masked, err));
     return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);
 }
 
@@ -1623,14 +1817,14 @@ GrB_Info positional_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp 
         MxmPos pos; pos.tc = zt; pos.off = p.off; pos.ids = ids_k;
         pos.side = A->dev.nnz <= B->dev.nnz ? 1 : 2;
         const int mul = pos.side == 1 ? OP_FIRST : OP_SECOND;
-        GB_TRY(mxm_product(Mask, f, zt, zt, add, mul, A, B, pos, T, &masked, err));
+        GB_TRY(mxm_product(Mask, f, zt, zt, add, mul, A, B, pos, burble, T, &masked, err));
         gb_kernel_used("positional=inner");
         gb_kernel_used(pos.side == 1 ? "positional-operand=A" : "positional-operand=B");
         return matrix_writeback(C, Mask, accum, f, std::move(T), zt, masked, err);
     }
     // ---- count form: product = i (FIRSTI) or j (SECONDJ), + off
     const bool idem = add == OP_MIN || add == OP_MAX || add == OP_ANY;       // the count is not needed, only the pattern
-    GB_TRY(mxm_product(Mask, f, TC_INT64, TC_INT64, idem ? OP_ANY : OP_PLUS, OP_PAIR, A, B, MxmPos(), T, &masked, err));
+    GB_TRY(mxm_product(Mask, f, TC_INT64, TC_INT64, idem ? OP_ANY : OP_PLUS, OP_PAIR, A, B, MxmPos(), burble, T, &masked, err));
     DevBuf<void> v;
     GB_TRY(v.alloc((size_t)T.nnz * tc_size(zt) + 16, err));
     GB_TRY(pos_csr_values(v, zt, (const int64_t *)T.val.get(), add, T, /*by_col=*/p.second, p.second ? ids_n : ids_m, p.off, err));

@@ -276,7 +276,7 @@ struct GbBurble {
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
 enum WsSlot : int { WS_WORDS = 0, WS_FOUND, WS_FLOPS, WS_TOTAL, WS_CS, WS_CM, WS_CL, WS_C1, WS_SROW, WS_SIDX, WS_SCNT, WS_MROW, WS_MIDX, WS_MCNT,
                     WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW,
-                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_PANEL_A, WS_PANEL_M, WS_COUNT };
+                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_PANEL_A, WS_PANEL_M, WS_GEMM_TREE, WS_COUNT };
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh = nullptr);
 template <typename T> static inline GrB_Info ws_array(int slot, T **p, size_t count, std::string *err, bool *fresh = nullptr) {
     return ws_get(slot, (void **)p, count * sizeof(T) + 16, err, fresh);
@@ -385,6 +385,15 @@ GrB_Info mask_true_pattern(const Csr &M, int mtc, Csr &out, std::string *err);
 // 2^32 entries, already on the device and not complemented: one dot product per entry of the mask (sddmm.cu)
 GrB_Info sddmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
                    const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
+// C<Mask> = accum(C, T) for a dense m x n T, presence bytes optional (tpres NULL: every position present): the vector write-back
+// over the m*n positions with no mask or a dense-form mask, so C keeps or takes a dense form; the CSR write-back under a CSR
+// mask (spmm.cu).  Consumes T.
+GrB_Info spmm_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f, DevBuf<void> &&tval,
+                        DevBuf<uint8_t> &&tpres, int zt, std::string *err);
+// C<Mask> = accum(C, op(A) (+).(x) op(B)) for dense-form A and B without presence bytes, a builtin non-positional semiring, an
+// m x n result of at most 2^31-1 positions, and no sparse non-complemented mask: the tiled semiring GEMM (gemm.cu)
+GrB_Info gemm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const GrB_Semiring s, const GrB_Matrix A,
+                  const GrB_Matrix B, const DescFlags &f, GbBurble &burble);
 
 // ---------------------------------------------------------------- scalar carrier
 // A value of any builtin type held in 64 bits: BOOL/UINT* in .u, INT* in .i, FP* in .d

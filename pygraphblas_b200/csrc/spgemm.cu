@@ -1790,6 +1790,8 @@ extern "C" GrB_Info GrB_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_Binar
         GB_TRY(matrix_ensure_device(Mask));
         return sddmm_mxm(C, Mask, accum, semiring, A, B, f, burble);
     }
+    if (A->dn.valid && B->dn.valid && !A->dn.pres && !B->dn.pres && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))
+        return gemm_mxm(C, Mask, accum, semiring, A, B, f, burble);                                 // two full dense operands
     if (B->dn.valid && !f.tran1) return spmm_mxm(C, Mask, accum, semiring, A, B, f, burble);         // dense X: DESIGN.md section 3.6
     if (A->dn.valid && !B->dn.valid && op_mirror(mul) >= 0 && (bn == 0 || am <= (uint64_t)INT32_MAX / bn))
         return spmm_left_mxm(C, Mask, accum, semiring, A, B, f, burble);                            // dense X on the left

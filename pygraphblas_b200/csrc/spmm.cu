@@ -331,8 +331,8 @@ static GrB_Info spmm_product(const Csr &a, const void *aval, const void *xval, c
 
 // C<Mask> = accum(C, T) for a dense T (m x k).  With no mask or a dense-form mask, C is viewed as a vector of m*k positions and
 // the vector write-back runs on it, so C keeps (or takes) the dense form.  A CSR mask sends T through the CSR write-back.
-static GrB_Info spmm_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f,
-                               DevBuf<void> &&tval, DevBuf<uint8_t> &&tpres, int zt, std::string *err) {
+GrB_Info spmm_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum, const DescFlags &f,
+                        DevBuf<void> &&tval, DevBuf<uint8_t> &&tpres, int zt, std::string *err) {
     const int64_t m = (int64_t)C->nrows, k = (int64_t)C->ncols;
     if (Mask && !Mask->dn.valid) {
         Csr T;

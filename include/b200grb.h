@@ -253,7 +253,9 @@ void B200_debug_wide_gemm(int64_t chunk, int64_t result_limit, int64_t spa_budge
  * (the mask-row membership filter is an exact bitmap or a one-hash Bloom filter), and "mxv=in-place" after an mxv / vxm
  * entry when the product was formed straight in w's buffers.  "offsets=64" follows the first entry of a call that ran on the
  * wide route (64-bit offsets).  An unmasked or complemented-mask product lists "esc-small", "esc-medium", "spa" and "spa-split"
- * once each, in that order, however many row panels ran them, with "offsets=64" after the first on the wide route */
+ * once each, in that order, however many row panels ran them, with "offsets=64" after the first on the wide route; a
+ * complemented-mask product whose rows took the pull route lists "pull" after them, followed by "pull=dot" (GxB_AxB_DOT on
+ * the descriptor) or "pull=auto" (the B200GRB_MXM_PULL rule) */
 const char *B200_debug_last_kernel(void);
 /* per-matrix SpGEMM/SpMV work figures of the most recent GrB_mxm (flops = number of
  * multiplies, nnz_out = nvals of the product T as the kernels formed it, before the accumulator and the write-back:

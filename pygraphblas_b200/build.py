@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200grb.so")
 SOURCES = ["objects.cu", "device_ops.cu", "spmv.cu", "spmv_run.cu", "spmv_run_int.cu", "spmv_run_generic.cu", "spmv_pull.cu",
            "spgemm.cu", "vector_ops.cu", "matrix_ops.cu", "matrix_assign.cu", "dist.cu", "hyper.cu", "compat.cu",
-           "positional.cu", "spmm.cu", "sddmm.cu", "gemm.cu"]
+           "positional.cu", "spmm.cu", "sddmm.cu", "gemm.cu", "spgemm_pull.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", "-O3"] + GENCODE + ["-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "186,177,550"]

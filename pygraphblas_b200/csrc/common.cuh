@@ -259,6 +259,9 @@ struct Tunables {
     int stream_blk_log2 = 7;   // B200GRB_STREAM_BLK   log2 of the block of a long B row one warp takes (masked SpGEMM)
     int mxv_inplace = 1;       // B200GRB_MXV_INPLACE  0: mxv / vxm never form T in w's own buffers; 1: when w has no copy in flight;
                                //                      2: always, the compute stream first joins w's last overlapped copies
+    double mxm_pull = 0.0;     // B200GRB_MXM_PULL     alpha of the per-row pull rule of a complemented-mask mxm (LOR / LAND / ANY);
+                               //                      0: off (only GxB_AxB_DOT pulls).  DESIGN.md section 3.2
+    int64_t mxm_pull_budget = (int64_t)1 << 28;   // B200GRB_MXM_PULL_BUDGET  bytes of bitmaps of one group of pull rows
 };
 const Tunables &tunables();
 
@@ -276,7 +279,8 @@ struct GbBurble {
 // 10-70 ms per call when the pool has to map fresh memory (masked GrB_mxm: 620 MB of column maps) -- these buffers never leave.
 enum WsSlot : int { WS_WORDS = 0, WS_FOUND, WS_FLOPS, WS_TOTAL, WS_CS, WS_CM, WS_CL, WS_C1, WS_SROW, WS_SIDX, WS_SCNT, WS_MROW, WS_MIDX, WS_MCNT,
                     WS_LROW, WS_LIDX, WS_LCNT, WS_WROWS, WS_QUEUES, WS_SPA_SLOT, WS_MASK_ROW,
-                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_PANEL_A, WS_PANEL_M, WS_GEMM_TREE, WS_COUNT };
+                    WS_SPLIT_BUF, WS_SPLIT_ROWS, WS_SPLIT_CHUNKS, WS_SPLIT_RANGES, WS_PANEL_A, WS_PANEL_M, WS_GEMM_TREE,
+                    WS_PULL_ROWS, WS_PULL_BUF, WS_COUNT };
 GrB_Info ws_get(int slot, void **p, size_t bytes, std::string *err, bool *fresh = nullptr);
 template <typename T> static inline GrB_Info ws_array(int slot, T **p, size_t count, std::string *err, bool *fresh = nullptr) {
     return ws_get(slot, (void **)p, count * sizeof(T) + 16, err, fresh);

@@ -44,6 +44,8 @@ static void tunables_load() {
     t.spgemm_trace = getenv("B200GRB_SPGEMM_TRACE") != nullptr;
     t.stream_blk_log2 = std::min(12, std::max(7, geti("B200GRB_STREAM_BLK", 7)));
     t.mxv_inplace = geti("B200GRB_MXV_INPLACE", 1);
+    if (const char *e = getenv("B200GRB_MXM_PULL")) t.mxm_pull = std::max(0.0, atof(e));
+    if (const char *e = getenv("B200GRB_MXM_PULL_BUDGET")) t.mxm_pull_budget = std::max<int64_t>(1, atoll(e));
     g_tun = t; g_tun_loaded = true;
 }
 const Tunables &tunables() { if (!g_tun_loaded) tunables_load(); return g_tun; }

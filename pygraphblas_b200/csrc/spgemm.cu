@@ -20,7 +20,9 @@
 // The general write-back  C<M> = accum(C, T)  (mask value/structure/complement, replace,
 // accumulator, typecasts) is a row-wise three-way merge (matrix_finalize).
 #include "common.cuh"
+#include "spgemm_pull.cuh"
 #include <algorithm>
+#include <functional>
 #include <limits>
 #include <type_traits>
 
@@ -1044,20 +1046,29 @@ struct UnmaskedPanel {
     const uint32_t *m_ptr, *m_col;
     int64_t nrows;
 };
-// the bins a call ran (esc-small, esc-medium, spa, spa-split): reported once each, in this order, however many panels ran them
-struct UnmaskedUse { bool bin[4] = {false, false, false, false}; };
+// the bins a call ran (esc-small, esc-medium, spa, spa-split, pull): reported once each, in this order, however many panels ran them
+struct UnmaskedUse { bool bin[5] = {false, false, false, false, false}; bool pull_dot = false; };
+// The pull route of an eligible call (spgemm_pull.cu): the rule's mode, and op(B)' with its values, formed by `ensure` only
+// once a row pulls.  rows: the rows that pulled.
+struct PullSide {
+    bool dot = false; double alpha = 0.0;
+    std::function<GrB_Info(PullOperands &)> ensure;
+    int64_t rows = 0;
+};
 // the wide route's size rule, counted over the panels: the entries of T formed so far, refused on reaching `limit`
 struct ResultCount { int64_t limit = 0, total = 0; };
 static const char *const WIDE_RESULT_REFUSAL = "GrB_mxm: results of >= 2^32 entries are not supported with an operand of >= 2^32 entries";
 
 // T = A (+).(x) B on one panel, unmasked.  A and B values already of the multiply's operand type.  With P.m_ptr set,
 // T = (A (+).(x) B)<!M'>: the same bins, chosen by the unfiltered product counts, run their COMP instantiations, which never form
-// a blocked entry.  BT: the type of B's row offsets (b_ptr).  spa_budget > 0 caps the dense-accumulator CTAs at that many bytes
-// of accumulators and bitmaps (the wide route; the narrow one runs 2 per SM).  rc (the wide route, when the size rule counts):
+// a blocked entry.  pull (the narrow route of an eligible call, else null): the rows its rule picks leave the bins for the pull
+// route, one more participant of the count - scan - fill.  BT: the type of B's row offsets (b_ptr).  spa_budget > 0 caps the
+// dense-accumulator CTAs at that many bytes of accumulators and bitmaps (the wide route; the narrow one runs 2 per SM).  rc (the wide route, when the size rule counts):
 // the panel is refused, before its entries are allocated, when T would reach rc->limit entries.  G.last_flops grows by the panel's products.
 template <typename BT>
 static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
-                                bool need_a, bool need_b, int64_t spa_budget, UnmaskedUse &use, ResultCount *rc, Csr &T, std::string *err) {
+                                bool need_a, bool need_b, int64_t spa_budget, UnmaskedUse &use, ResultCount *rc, PullSide *pull, Csr &T,
+                                std::string *err) {
     const int64_t nrows = P.nrows, ncols = B.ncols;
     const bool comp = P.m_ptr != nullptr;
     const size_t wsize = tc_size(zt) == 8 ? 8 : 4;
@@ -1069,6 +1080,8 @@ static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *
     int64_t spa_n = 0;
     int spa_ctas = 1;
     DevBuf<unsigned int> queue; DevBuf<uint32_t> spa_bits;
+    PullOperands po{P.a_ptr, P.a_col, P.a_val, P.m_ptr, P.m_col, nullptr, nullptr, nullptr, nrows, ncols, B.nrows, xt, zt, add, mul, need_a, need_b};
+    PullPlan pp;
     // ---- symbolic: the bins count the entries of their rows
     auto symbolic = [&](int64_t *cnt) {
         CU_TRY(cudaMemsetAsync(cnt, 0, ((size_t)nrows + 1) * 8, G.stream), err);
@@ -1076,6 +1089,10 @@ static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *
         GB_TRY(flops.alloc((size_t)nrows, err)); GB_TRY(total.alloc(1, err));
         CU_TRY(cudaMemsetAsync(total, 0, 8, G.stream), err);
         flops_kernel<BT><<<grid_for(nrows * 32), 256, 0, G.stream>>>(P.a_ptr, P.a_col, b_ptr, nrows, flops, total); GB_LAUNCHED();
+        if (pull && (pull->dot || pull->alpha > 0)) {      // the pull rows get no products in the bins' flops
+            GB_TRY(pull_plan(po, flops, pull->dot, pull->alpha, B.nnz, pp, err));
+            if (pp.n) GB_TRY(pull->ensure(po));
+        }
         GB_TRY(make_bins(flops, nrows, BinLimits{SMALL_FLOPS, MEDIUM_FLOPS}, bins, err));
         int64_t total_flops = 0; GB_TRY(read_i64((const int64_t *)total, &total_flops, err));
         G.last_flops += (uint64_t)total_flops;
@@ -1132,6 +1149,10 @@ static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *
             G.launches += 2;
         }
         if (sp.nsplit) use.bin[3] = true;
+        if (pp.n) {
+            GB_TRY(pull_count(po, pp, cnt, err));
+            use.bin[4] = true; use.pull_dot = pull->dot; pull->rows += pp.n;
+        }
         return GrB_SUCCESS;
     };
     // ---- numeric (shared-memory bins: expand-sort-compress)
@@ -1164,6 +1185,7 @@ static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *
 #define K_SPLIT(XT, ZT, A_, M_) GB_TRY((split_numeric<XT, ZT, A_, M_, BT>(sp, sa, err)))
             GB_FOR_SEMIRING(xt, zt, add, mul, K_SPLIT, err);
         }
+        if (pp.n) GB_TRY(pull_fill(po, pp, t.rowptr, t.col, t.val, err));
         spa_bits.reset(); queue.reset(); bins.rows.reset();
         return GrB_SUCCESS;
     };
@@ -1520,7 +1542,8 @@ static GrB_Info spgemm_unmasked_wide(const Csr &A, const Csr &B, const BT *b_ptr
         }
         const UnmaskedPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr,
                               mp, comp ? Mb->col + m0 : nullptr, pn};
-        return spgemm_unmasked<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, budget, use, counting ? &rc : nullptr, part, err);
+        return spgemm_unmasked<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, budget, use, counting ? &rc : nullptr, nullptr, part,
+                                   err);
     };
     int64_t r1 = 0;
     if (nrows > 0) {
@@ -1557,27 +1580,28 @@ static GrB_Info spgemm_unmasked_wide(const Csr &A, const Csr &B, const BT *b_ptr
 }
 
 static void unmasked_report(const UnmaskedUse &u, bool wide) {
-    static const char *const names[4] = {"esc-small", "esc-medium", "spa", "spa-split"};
+    static const char *const names[5] = {"esc-small", "esc-medium", "spa", "spa-split", "pull"};
     bool first = true;
-    for (int k = 0; k < 4; ++k) {
+    for (int k = 0; k < 5; ++k) {
         if (!u.bin[k]) continue;
         gb_kernel_used(names[k]);
         if (first && wide) gb_kernel_used("offsets=64");
         first = false;
     }
+    if (u.bin[4]) gb_kernel_used(u.pull_dot ? "pull=dot" : "pull=auto");
 }
 
 // T = A (+).(x) B, unmasked, or (A (+).(x) B)<!Mb> with Mb the entries of a complemented mask that block.  The narrow route runs
 // the bins once on the whole of A and Mb; the wide route (an operand or the mask of 2^32 or more entries, or B200_debug_wide_gemm)
-// on row panels, with B's 64-bit offsets when B is wide.
+// on row panels, with B's 64-bit offsets when B is wide.  pull: the pull route of an eligible call (narrow only), or null.
 static GrB_Info spgemm_unmasked_call(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt, int add, int mul,
-                                     bool need_a, bool need_b, const Csr *Mb, bool wide, Csr &T, std::string *err) {
+                                     bool need_a, bool need_b, const Csr *Mb, bool wide, PullSide *pull, Csr &T, std::string *err) {
     const bool comp = Mb && Mb->nnz > 0;
     UnmaskedUse use;
     G.last_flops = 0;
     if (!wide) {
         const UnmaskedPanel P{A.rowptr32, A.col, aval, comp ? Mb->rowptr32.get() : nullptr, comp ? Mb->col.get() : nullptr, A.nrows};
-        GB_TRY(spgemm_unmasked<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, 0, use, nullptr, T, err));
+        GB_TRY(spgemm_unmasked<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, 0, use, nullptr, pull, T, err));
     } else if (gemm_wide(B)) {
         GB_TRY(spgemm_unmasked_wide<int64_t>(A, B, B.rowptr.get(), aval, bval, xt, zt, add, mul, need_a, need_b, Mb, use, T, err));
     } else {
@@ -1754,7 +1778,38 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
         const Csr *mb = nullptr;
         if (Mask && f.mask_struct) mb = &Mask->dev;
         else if (Mask) { GB_TRY(mask_true_pattern(Mask->dev, Mask->type->code, mtrue, err)); mb = &mtrue; }
-        r = spgemm_unmasked_call(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, wide, T, err);
+        // a complemented mask and a saturating monoid on the narrow route: GxB_AxB_DOT pulls every row with products, the
+        // default descriptor the rows the B200GRB_MXM_PULL rule picks (DESIGN.md section 3.2)
+        PullSide ps;
+        DevBuf<void> bt_cast;
+        const bool eligible = Mask && !wide && (add == OP_LOR || add == OP_LAND || add == OP_ANY);
+        if (eligible) {
+            ps.dot = f.axb == GxB_AxB_DOT;
+            ps.alpha = f.axb == GxB_DEFAULT ? tunables().mxm_pull : 0.0;
+            // op(B)': B itself under INP1 = TRAN, else B's cached transpose; its values of the multiply's x type, or op(B)'s
+            // row index p (the column in op(B)') for the positional inner form on op(B)
+            ps.ensure = [&](PullOperands &o) -> GrB_Info {
+                if (!f.tran1) GB_TRY(matrix_ensure_transpose(B));
+                const Csr &bt = f.tran1 ? B->dev : B->devT;
+                if (!bt.rowptr32) return gb_fail(GrB_PANIC, err, "GrB_mxm: the pull route needs 32-bit offsets of op(B)'");
+                o.bt_ptr = bt.rowptr32; o.bt_col = bt.col; o.bt_val = bt.val;
+                if (pos.side == 2) {
+                    GB_TRY(bt_cast.alloc((size_t)bt.nnz * tc_size(pos.tc) + 16, err));
+                    GB_TRY(pos_csr_values(bt_cast, pos.tc, nullptr, OP_ANY, bt, /*by_col=*/true, pos.ids, pos.off, err));
+                    o.bt_val = bt_cast;
+                } else if (need_b && B->type->code != xt) {
+                    GB_TRY(dev_cast_values(bt_cast, xt, bt.val, B->type->code, bt.nnz, err));
+                    o.bt_val = bt_cast;
+                }
+                return GrB_SUCCESS;
+            };
+        }
+        r = spgemm_unmasked_call(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, wide, eligible ? &ps : nullptr, T, err);
+        if (r == GrB_SUCCESS && ps.rows && burble.on) {
+            static std::string note;                    // outlives the call's burble line (calls are serialised under GB_LOCK)
+            note = "spgemm pull, " + std::to_string(ps.rows) + " rows" + (ps.dot ? " (GxB_AxB_DOT)" : " (auto)");
+            burble.note(note.c_str(), burble.bytes);
+        }
     }
     a_cast.reset(); b_cast.reset();
     return r;

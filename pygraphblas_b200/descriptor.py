@@ -1,12 +1,13 @@
 """Descriptors.  Mirrors reference: pygraphblas/descriptor.py:10-182: the 27 builtin
 combinations of T0/T1 (transpose input), C (complement mask), S (structural mask),
-R (replace output), usable as arguments, context managers and combinable with `&`."""
+R (replace output), usable as arguments, context managers and combinable with `&`.  GxB_AxB_METHOD set on a
+descriptor (GxB_AxB_DOT: the pull route of a complemented-mask mxm, DESIGN.md section 3.2) is combined the same way."""
 import contextvars
 from .base import lib, ffi, _check, NULL
 
 current_desc = contextvars.ContextVar("current_desc")
 
-_FIELDS = ("GrB_INP0", "GrB_INP1", "GrB_MASK", "GrB_OUTP")
+_FIELDS = ("GrB_INP0", "GrB_INP1", "GrB_MASK", "GrB_OUTP", "GxB_AxB_METHOD")
 
 
 class Descriptor:

@@ -19,7 +19,7 @@ GxB_INDEX_MAX = 1 << 60
 
 
 class Matrix:
-    __slots__ = ("_matrix", "_keep", "_mask_alive", "__weakref__")
+    __slots__ = ("_matrix", "_keep", "_mask_alive", "_desc_alive", "__weakref__")
 
     def __init__(self, handle):
         """Wrap a raw GrB_Matrix* (ffi.new("GrB_Matrix*")); the type is read back from the
@@ -324,6 +324,7 @@ class Matrix:
         if desc is None:
             desc = current_desc.get(NULL)
         if desc is not NULL:
+            self._desc_alive = desc            # a temporary descriptor (desc & other) must outlive the call
             desc = desc.get_desc()
         return mask, accum, desc
 

@@ -14,7 +14,7 @@ GxB_INDEX_MAX = 1 << 60
 
 
 class Vector:
-    __slots__ = ("_vector", "_mask_alive", "_keep_scalar", "_owner", "__weakref__")
+    __slots__ = ("_vector", "_mask_alive", "_desc_alive", "_keep_scalar", "_owner", "__weakref__")
 
     def __init__(self, handle, owner=None):
         self._vector = handle
@@ -216,6 +216,7 @@ class Vector:
         if desc is None:
             desc = current_desc.get(NULL)
         if desc is not NULL:
+            self._desc_alive = desc            # a temporary descriptor (desc & other) must outlive the call
             desc = desc.get_desc()
         return mask, accum, desc
 

@@ -1,6 +1,7 @@
 """GrB_mxm under a complemented mask: the filtered route against the two steps the library used to take.
 
     python tools/msbfs_bench.py [--scales 20 22] [--ks 4 64] [--reps 3] [--out DIR]
+    python tools/msbfs_bench.py --pull [--alphas 2 4 8 14 32] [--scales 20 22] [--ks 4 64] [--reps 3] [--out DIR]
 
 new  C<!M, R> = A (+).(x) B in one call: the unmasked bins never form a blocked product.
 old  T = A (+).(x) B unmasked, then C<!M, R> = IDENTITY(T) (GrB_Matrix_apply): the product formed whole, then filtered.
@@ -9,6 +10,11 @@ Workloads: multi-source BFS (k = 4 and 64 sources, BOOL ANY_PAIR, F<!V, R> = F a
 of gap/bcmark.py (4 sources, FP32 PLUS_FIRST, a valued FP32 path-count mask), and C<!A, R> = A any.pair A at scale 16.  Old and
 new run alternately on the same inputs; their results must be equal, and the BFS levels must match scipy.  Times are host clocks
 around calls that end in a device synchronise, medians over --reps repetitions.
+
+--pull compares the directions of the multi-source BFS step instead (DESIGN.md section 3.2): push (GxB_AxB_SAXPY: the bins on
+every level), dot (GxB_AxB_DOT: every row pulls on every level) and auto (the default descriptor under B200GRB_MXM_PULL = alpha,
+for each --alphas value).  It reports the per-level times of each arm, the traversal medians and the alpha of the fastest auto
+arm; every arm's F must equal push's at every level and the levels must match scipy.
 """
 import argparse
 import json
@@ -89,6 +95,57 @@ def msbfs(A, S, n, k, reps):
     return {"old_ms": med["old"], "new_ms": med["new"], "levels": len(per_level["new"]), "per_level_ms": per_level, "matches_scipy": ok}
 
 
+def axb(method):
+    d = descriptor.Descriptor()
+    d[lib.GxB_AxB_METHOD] = getattr(lib, f"GxB_AxB_{method}")
+    return d
+
+
+def set_alpha(alpha):
+    os.environ["B200GRB_MXM_PULL"] = str(alpha)
+    lib.B200_reload_tunables()
+
+
+def msbfs_pull(A, S, n, k, reps, alphas):
+    """F<!V, R> = F any.pair A level by level under push, dot and auto(alpha); arms alternate within each repetition."""
+    sources = np.argsort(-np.diff(S.indptr), kind="stable")[:k]
+    arms = [("push", descriptor.RSC & axb("SAXPY"), 0), ("dot", descriptor.RSC & axb("DOT"), 0)]
+    arms += [(f"auto{a:g}", descriptor.RSC, a) for a in alphas]
+    res, fronts = {}, {}
+    for _ in range(reps):
+        for name, desc, alpha in arms:
+            set_alpha(alpha)
+            F = Matrix.from_lists(list(range(k)), list(sources), [True] * k, k, n, gb.BOOL)
+            V = F.dup()
+            lev = np.full((k, n), -1, np.int64)
+            lev[np.arange(k), sources] = 0
+            times, levels, d = [], [], 0
+            while True:
+                d += 1
+                dt, F = timed(lambda: F.mxm(A, semiring=gb.BOOL.ANY_PAIR, out=Matrix.sparse(gb.BOOL, k, n), mask=V, desc=desc))
+                times.append(dt)
+                I, J, _ = F.to_arrays()
+                levels.append(I.astype(np.int64) * n + J)
+                if F.nvals == 0:
+                    break
+                lev[I, J] = d
+                V.eadd(F, gb.BOOL.LOR, out=V)
+            res.setdefault(name, []).append((sum(times), times, lev))
+            fronts[name] = levels
+    set_alpha(0)
+    want = csgraph.shortest_path(S, unweighted=True, indices=sources)
+    want = np.where(np.isinf(want), -1, want).astype(np.int64)
+    ok = all(np.array_equal(r[2], want) for rs in res.values() for r in rs)
+    equal = all(len(fronts[a]) == len(fronts["push"]) and all(np.array_equal(x, y) for x, y in zip(fronts[a], fronts["push"]))
+                for a in fronts)
+    med = {a: round(statistics.median(x[0] for x in res[a]) * 1e3, 3) for a in res}
+    per_level = {a: [round(statistics.median(x[1][lv] for x in res[a]) * 1e3, 3) for lv in range(len(res[a][0][1]))] for a in res}
+    autos = [a for a in med if a.startswith("auto")]
+    best = min(autos, key=lambda a: med[a]) if autos else None
+    return {"traversal_ms": med, "per_level_ms": per_level, "best_auto": best, "levels": len(per_level["push"]),
+            "equal": equal, "matches_scipy": ok}
+
+
 def bc_forward(A, S, n, reps):
     """The forward sweep of gap/bcmark.py's bc() for 4 sources: frontier<!paths, R> = frontier plus.first A, paths += frontier."""
     deg = np.diff(S.indptr)
@@ -131,6 +188,8 @@ def main():
     ap.add_argument("--two-hop-scale", type=int, default=16)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--pull", action="store_true", help="push / dot / auto arms of the multi-source BFS step")
+    ap.add_argument("--alphas", type=float, nargs="+", default=[2, 4, 8, 14, 32])
     a = ap.parse_args()
     if not gb.have_device():
         raise SystemExit("msbfs_bench: no CUDA device")
@@ -142,17 +201,23 @@ def main():
         Ab = Matrix.from_csr(indptr, indices, np.ones(len(indices), bool), n, n, gb.BOOL)
         Af = Matrix.from_csr(indptr, indices, np.ones(len(indices), np.float32), n, n, gb.FP32)
         for k in a.ks:
-            r = {"workload": f"msbfs s{scale} k={k}", **msbfs(Ab, S, n, k, a.reps)}
+            if a.pull:
+                r = {"workload": f"msbfs pull s{scale} k={k}", **msbfs_pull(Ab, S, n, k, a.reps, a.alphas)}
+            else:
+                r = {"workload": f"msbfs s{scale} k={k}", **msbfs(Ab, S, n, k, a.reps)}
             print(json.dumps(r), flush=True)
             report["workloads"].append(r)
+        if a.pull:
+            continue
         r = {"workload": f"bc-forward s{scale} 4 sources", **bc_forward(Af, S, n, a.reps)}
         print(json.dumps(r), flush=True)
         report["workloads"].append(r)
-    n, indptr, indices = rmat_csr(a.two_hop_scale, 16, seed=1)
-    Ab = Matrix.from_csr(indptr, indices, np.ones(len(indices), bool), n, n, gb.BOOL)
-    r = {"workload": f"C<!A,R> = A any.pair A s{a.two_hop_scale}", **two_hop(Ab, a.reps)}
-    print(json.dumps(r), flush=True)
-    report["workloads"].append(r)
+    if not a.pull:
+        n, indptr, indices = rmat_csr(a.two_hop_scale, 16, seed=1)
+        Ab = Matrix.from_csr(indptr, indices, np.ones(len(indices), bool), n, n, gb.BOOL)
+        r = {"workload": f"C<!A,R> = A any.pair A s{a.two_hop_scale}", **two_hop(Ab, a.reps)}
+        print(json.dumps(r), flush=True)
+        report["workloads"].append(r)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "msbfs_bench.json"), "w") as f:

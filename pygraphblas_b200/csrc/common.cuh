@@ -358,6 +358,14 @@ GrB_Info dev_build_rowptr32(Csr &c, std::string *err);
 GrB_Info dev_exclusive_scan(int64_t *data, int64_t n, std::string *err);
 GrB_Info dev_transpose(const Csr &a, size_t vsize, Csr &t, std::string *err);
 GrB_Info dev_cast_values(DevBuf<void> &out, int to_code, const void *in, int from_code, int64_t n, std::string *err);
+// *out = the n values `in` (of type from_code) of an mxm operand as the multiply reads them: cast into `cast` to its x type xt
+// when it reads them (reads) and the types differ, else `in` itself.  The cast buffer belongs to the caller.
+static inline GrB_Info mxm_values(DevBuf<void> &cast, const void **out, bool reads, int xt, const void *in, int from_code, int64_t n,
+                                  std::string *err) {
+    *out = in;
+    if (reads && from_code != xt) { GB_TRY(dev_cast_values(cast, xt, in, from_code, n, err)); *out = cast; }
+    return GrB_SUCCESS;
+}
 GrB_Info dev_count_present(const uint8_t *pres, int64_t n, int64_t *count, std::string *err);
 GrB_Info upload_indices(const std::vector<uint64_t> &idx, DevBuf<uint64_t> &d, std::string *err);     // host list -> device (vector_ops.cu)
 // dense form <-> CSR (spmm.cu).  dense_to_csr compacts the present entries (pres NULL: all) into c, rowptr32 included;

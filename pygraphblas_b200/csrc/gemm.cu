@@ -216,9 +216,9 @@ GrB_Info gemm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     const int64_t n = (int64_t)(f.tran1 ? B->nrows : B->ncols);
     // operands cast to the multiply's input type where it reads them, as on the SpMM route
     DevBuf<void> a_cast, b_cast;
-    const void *aval = A->dn.val, *bval = B->dn.val;
-    if (mul_reads_x(mul) && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, aval, A->type->code, m * k, err)); aval = a_cast; }
-    if (mul_reads_y(mul) && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, bval, B->type->code, k * n, err)); bval = b_cast; }
+    const void *aval = nullptr, *bval = nullptr;
+    GB_TRY(mxm_values(a_cast, &aval, mul_reads_x(mul), xt, A->dn.val, A->type->code, m * k, err));
+    GB_TRY(mxm_values(b_cast, &bval, mul_reads_y(mul), xt, B->dn.val, B->type->code, k * n, err));
     // T in fresh buffers: C may alias A or B.  With k > 0 every position has a product and T needs no presence bytes; with
     // k = 0 none has one.
     DevBuf<void> tval; DevBuf<uint8_t> tpres;

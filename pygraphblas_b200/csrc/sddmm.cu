@@ -165,10 +165,10 @@ struct SddmmOperand {
 };
 static GrB_Info sddmm_operand(const GrB_Matrix A, bool reads, int xt, bool tr, const char *token, SddmmOperand &o, std::string *err) {
     const int64_t rows = (int64_t)A->nrows, cols = (int64_t)A->ncols, n = rows * cols;
-    o.val = A->dn.val; o.pres = A->dn.pres;
-    size_t b = tc_size(A->type->code);
-    o.bytes = (double)n * (b + (o.pres ? 1 : 0));
-    if (reads && A->type->code != xt) { GB_TRY(dev_cast_values(o.cast, xt, o.val, A->type->code, n, err)); o.val = o.cast; b = tc_size(xt); }
+    o.pres = A->dn.pres;
+    o.bytes = (double)n * (tc_size(A->type->code) + (o.pres ? 1 : 0));
+    GB_TRY(mxm_values(o.cast, &o.val, reads, xt, A->dn.val, A->type->code, n, err));
+    const size_t b = tc_size(reads ? xt : A->type->code);      // the bytes of one value of o.val
     if (tr && (reads || o.pres)) {              // an operand that is neither read nor has absent entries has no layout
         GB_TRY(o.tval.alloc((size_t)n * b + 16, err));
         if (o.pres) GB_TRY(o.tpres.alloc((size_t)n, err));

@@ -1038,13 +1038,13 @@ static GrB_Info split_numeric(const SplitPlan &sp, const SplitArgsT<BT> &base, s
     return GrB_SUCCESS;
 }
 
-// One row panel of an unmasked or complemented product: nrows rows of A and of M' (the entries of a complemented mask that
-// block, see mask_true_pattern), with 32-bit offsets relative to the panel's first entries (the narrow route: the whole
-// matrices, their rowptr32).  m_ptr is null when no entry blocks.
-struct UnmaskedPanel {
+// One row panel of a CSR x CSR product: nrows rows of A and of the mask -- M, or M' (the entries of a complemented mask that
+// block, see mask_true_pattern) -- with 32-bit offsets relative to the panel's first entries (the narrow route: the whole
+// matrices, their rowptr32).  m_ptr is null when no mask entry applies.  The unmasked bins leave m_val and mnnz unused.
+struct RowPanel {
     const uint32_t *a_ptr, *a_col; const void *a_val;
-    const uint32_t *m_ptr, *m_col;
-    int64_t nrows;
+    const uint32_t *m_ptr, *m_col; const void *m_val;
+    int64_t nrows, mnnz;
 };
 // the bins a call ran (esc-small, esc-medium, spa, spa-split, pull): reported once each, in this order, however many panels ran them
 struct UnmaskedUse { bool bin[5] = {false, false, false, false, false}; bool pull_dot = false; };
@@ -1066,7 +1066,7 @@ static const char *const WIDE_RESULT_REFUSAL = "GrB_mxm: results of >= 2^32 entr
 // dense-accumulator CTAs at that many bytes of accumulators and bitmaps (the wide route; the narrow one runs 2 per SM).  rc (the wide route, when the size rule counts):
 // the panel is refused, before its entries are allocated, when T would reach rc->limit entries.  G.last_flops grows by the panel's products.
 template <typename BT>
-static GrB_Info spgemm_unmasked(const UnmaskedPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
+static GrB_Info spgemm_unmasked(const RowPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
                                 bool need_a, bool need_b, int64_t spa_budget, UnmaskedUse &use, ResultCount *rc, PullSide *pull, Csr &T,
                                 std::string *err) {
     const int64_t nrows = P.nrows, ncols = B.ncols;
@@ -1219,20 +1219,13 @@ struct PhaseTrace {
     }
 };
 
-// One row panel of a masked product: nrows rows of A and M, with 32-bit offsets relative to the panel's first entries (the
-// narrow route: the whole matrices, their rowptr32)
-struct MaskedPanel {
-    const uint32_t *a_ptr, *a_col; const void *a_val;
-    const uint32_t *m_ptr, *m_col; const void *m_val;
-    int64_t nrows, mnnz;
-};
 // the methods a masked call ran: reported once each, in the same order, however many panels ran them
 struct MaskedUse { bool dot = false, warp = false, cls[3] = {false, false, false}, exact[3] = {false, false, false}; };
 
 // The masked methods on one panel: the accumulator word and the found flag of each of its mask entries, in the workspace
 // (*tval, *tfound; 1- and 2-byte types are narrowed into `typed`).  BT: the type of B's row offsets.
 template <typename BT>
-static GrB_Info masked_panel(const MaskedPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
+static GrB_Info masked_panel(const RowPanel &P, const Csr &B, const BT *b_ptr, const void *bval, int xt, int zt, int add, int mul,
                              bool need_a, bool need_b, int mtc, bool m_struct, bool dot, int64_t ncols, PhaseTrace &trace,
                              MaskedUse &use, void **tval, uint8_t **tfound, DevBuf<void> &typed, std::string *err) {
     const int64_t nrows = P.nrows;
@@ -1348,12 +1341,12 @@ template <typename OT>
 static GrB_Info masked_compact_t(int64_t nrows, int64_t ncols, int64_t mnnz, const OT *m_ptr, const uint32_t *m_col, const uint8_t *found,
                                  const void *tval, size_t vsize, Csr &T, std::string *err);
 
-// ------------------------------------------------------------------ the wide route of the masked methods
-// Rows of T<M> = A (+).(x) B depend on the same rows of A and M only, so the wide route walks A and M in row panels of at most
-// `bound` entries of each (a longer row is a panel of its own: every row has fewer than 2^31 entries), with their offsets rebased
-// to 32 bits: the kernels keep 32-bit positions in A and M, and the per-mask-entry scratch and the per-row arrays are those of one
-// panel.  B's rows are gathered by A's column ids and cannot be cut: the kernels read B's 64-bit offsets when B is wide.  Each
-// panel is compacted on its own; T is formed from the panels' row counts and entries.
+// ------------------------------------------------------------------ the row panels of the CSR x CSR products
+// Rows of T = A (+).(x) B, under a mask M or M' or none, depend on the same rows of A and of the mask only, so the wide route walks
+// A and the mask in row panels of at most `bound` entries of each (a longer row is a panel of its own: every row has fewer than
+// 2^31 entries), with their offsets rebased to 32 bits: the kernels keep 32-bit positions in A and the mask, and the per-mask-entry
+// scratch and the per-row arrays are those of one panel.  B's rows are gathered by A's column ids and cannot be cut: the kernels
+// read B's 64-bit offsets when B is wide.  Each panel is formed on its own; T is formed from the panels' row counts and entries.
 static constexpr int64_t WIDE_PANEL = (int64_t)1 << 30;
 static constexpr int64_t WIDE_PANEL_ROWS = (int64_t)1 << 26;       // and at most this many rows: the per-row arrays (40 B a row)
 
@@ -1403,147 +1396,39 @@ __global__ void gemm_bound_kernel(const int64_t *a_ptr, const uint32_t *a_col, c
     if (lane == 0 && l) atomicAdd(&total[1], l);
 }
 
-template <typename BT>
-static GrB_Info spgemm_masked_wide(const Csr &A, const Csr &B, const BT *b_ptr, const void *aval, const void *bval, int xt, int zt,
-                                   int add, int mul, bool need_a, bool need_b, const Csr &M, int mtc, bool m_struct, bool dot,
-                                   PhaseTrace &trace, MaskedUse &use, Csr &T, std::string *err) {
-    const int64_t nrows = A.nrows, ncols = dot ? B.nrows : B.ncols;
-    const size_t zsz = (size_t)tc_size(zt), asz = need_a ? (size_t)tc_size(xt) : 0, msz = M.val.get() ? (size_t)tc_size(mtc) : 0;
-    const int64_t bound = std::min(G.debug_wide > 0 ? wide_chunk() : WIDE_PANEL, WIDE_PANEL);
+// T (ncols columns, zsz bytes a value) = body(P, part) on the row panels P of A and of the mask M (null: no mask entry applies).
+// aval: A's values as the multiply reads them; asz, msz: the bytes of one value of A and of M in the panel (0: not read).  The
+// narrow route (!wide) is one panel, the whole of A and M through their rowptr32, formed straight into T; the wide route cuts
+// panels of at most `bound` entries of A and of M.
+template <typename Body>
+static GrB_Info spgemm_panels(const Csr &A, const void *aval, size_t asz, const Csr *M, size_t msz, bool wide, int64_t bound,
+                              int64_t ncols, size_t zsz, Csr &T, std::string *err, Body &&body) {
+    const int64_t nrows = A.nrows;
+    if (!wide)
+        return body(RowPanel{A.rowptr32, A.col, aval, M ? M->rowptr32.get() : nullptr, M ? M->col.get() : nullptr,
+                             M && msz ? M->val.get() : nullptr, nrows, M ? M->nnz : 0}, T);
     std::vector<Csr> parts;
     DevBuf<int64_t> ends;
     GB_TRY(ends.alloc(4, err));
-    // the panel that starts at row r0, compacted into `part`; *r1 = its end
+    // the panel that starts at row r0, formed into `part`; *r1 = its end.  Without M, A's offsets stand in for panel_end_kernel's M.
     auto panel = [&](int64_t r0, int64_t *r1, Csr &part) -> GrB_Info {
-        panel_end_kernel<<<1, 1, 0, G.stream>>>(A.rowptr, M.rowptr, r0, nrows, bound, WIDE_PANEL_ROWS, ends); GB_LAUNCHED();
+        panel_end_kernel<<<1, 1, 0, G.stream>>>(A.rowptr, M ? M->rowptr.get() : A.rowptr.get(), r0, nrows, bound, WIDE_PANEL_ROWS, ends);
+        GB_LAUNCHED();
         int64_t h[4];
         CU_TRY(cudaMemcpyAsync(h, ends, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
         CU_TRY(cudaStreamSynchronize(G.stream), err);
         *r1 = h[0];
-        const int64_t a0 = h[1], m0 = h[2], m1 = h[3];
-        const int64_t pn = *r1 - r0;
-        uint32_t *ap = nullptr, *mp = nullptr;
-        GB_TRY(ws_array(WS_PANEL_A, &ap, (size_t)pn + 1, err)); GB_TRY(ws_array(WS_PANEL_M, &mp, (size_t)pn + 1, err));
-        panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(A.rowptr, r0, pn, ap); GB_LAUNCHED();
-        panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(M.rowptr, r0, pn, mp); GB_LAUNCHED();
-        const MaskedPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr,
-                            mp, M.col + m0, msz ? static_cast<const uint8_t *>(M.val.get()) + m0 * msz : nullptr, pn, m1 - m0};
-        void *tval = nullptr; uint8_t *found = nullptr;
-        DevBuf<void> typed;
-        GB_TRY(masked_panel<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, mtc, m_struct, dot, ncols, trace, use,
-                                &tval, &found, typed, err));
-        return masked_compact_t<uint32_t>(pn, ncols, P.mnnz, mp, P.m_col, found, tval, zsz, part, err);
-    };
-    int64_t r1 = 0;
-    if (nrows > 0) {
-        parts.emplace_back();
-        GB_TRY(panel(0, &r1, parts[0]));
-        if (r1 == nrows) {                      // one panel: it is T
-            T = std::move(parts[0]);
-            G.last_nnz_out = (uint64_t)T.nnz;
-            return GrB_SUCCESS;
-        }
-    }
-    GB_TRY(csr_from_row_counts(nrows, ncols, zsz, T, err,
-        [&](int64_t *rowptr) {
-            CU_TRY(cudaMemsetAsync(rowptr + nrows, 0, 8, G.stream), err);
-            for (int64_t r0 = 0, q = 0; r0 < nrows; r0 = r1, ++q) {
-                if (q > 0) { parts.emplace_back(); GB_TRY(panel(r0, &r1, parts.back())); }
-                else r1 = parts[0].nrows;
-                row_len_kernel<<<grid_for(r1 - r0), 256, 0, G.stream>>>(parts.back().rowptr32, r1 - r0, rowptr + r0); GB_LAUNCHED();
-            }
-            return GrB_SUCCESS;
-        },
-        [&](Csr &t) {
-            int64_t at = 0;
-            for (Csr &part : parts) {
-                if (part.nnz) {
-                    CU_TRY(cudaMemcpyAsync(t.col.get() + at, part.col, (size_t)part.nnz * 4, cudaMemcpyDeviceToDevice, G.stream), err);
-                    CU_TRY(cudaMemcpyAsync(static_cast<uint8_t *>(t.val.get()) + at * zsz, part.val, (size_t)part.nnz * zsz,
-                                           cudaMemcpyDeviceToDevice, G.stream), err);
-                }
-                at += part.nnz;
-                part = Csr();
-            }
-            return GrB_SUCCESS;
-        }));
-    G.last_nnz_out = (uint64_t)T.nnz;
-    return GrB_SUCCESS;
-}
-
-static void masked_report(const MaskedUse &u, bool wide) {
-    bool first = true;
-    auto entry = [&](const char *k) { gb_kernel_used(k); if (first && wide) gb_kernel_used("offsets=64"); first = false; };
-    if (u.dot) entry("dot");
-    if (u.warp) entry("masked-warp");
-    for (int k = 0; k < 3; ++k) {
-        if (!u.cls[k]) continue;
-        entry(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
-        gb_kernel_used(u.exact[k] ? "filter=exact" : "filter=bloom");
-    }
-}
-
-// ------------------------------------------------------------------ the wide route of the unmasked and complemented-mask bins
-// The same row panels as the masked route's (of A and M', the entries of a complemented mask that block): each panel runs the
-// whole pipeline (flops, bins, symbolic, scan, numeric) into a CSR of its rows; T is the one panel, or is formed from the panels'
-// row counts and entries.  B is read through its 64-bit offsets when it is wide.  The route forms results of fewer than 2^32
-// entries: T would take 34 GB or more in FP32 (twice that while the panels are joined), which does not fit beside a wide operand
-// on an 80 GB card.  gemm_bound_kernel bounds nnz(T) before any panel runs: L >= the limit is refused at once; U < the limit
-// needs no further check; otherwise the panels' symbolic counts are added up and the call refused as soon as the scan of a
-// panel's counts reaches the limit, before that panel's entries are allocated or formed.  The dense accumulators of a panel are capped at WIDE_SPA_BUDGET bytes (one FP32 accumulator is
-// 1 GB at n = 2^28).
-static constexpr int64_t WIDE_RESULT = (int64_t)1 << 32;
-static constexpr int64_t WIDE_SPA_BUDGET = (int64_t)1 << 32;
-// the route of a CSR x CSR product without a (non-complemented) mask: a CSR without rowptr32, or any CSR under B200_debug_wide_gemm
-static inline bool gemm_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide_gemm > 0; }
-
-template <typename BT>
-static GrB_Info spgemm_unmasked_wide(const Csr &A, const Csr &B, const BT *b_ptr, const void *aval, const void *bval, int xt, int zt,
-                                     int add, int mul, bool need_a, bool need_b, const Csr *Mb, UnmaskedUse &use, Csr &T,
-                                     std::string *err) {
-    const int64_t nrows = A.nrows, ncols = B.ncols;
-    const bool comp = Mb && Mb->nnz > 0;
-    const size_t zsz = (size_t)tc_size(zt), asz = need_a ? (size_t)tc_size(xt) : 0;
-    const bool seam = G.debug_wide_gemm > 0;
-    const int64_t bound = std::min(seam ? G.debug_wide_gemm : WIDE_PANEL, WIDE_PANEL);
-    const int64_t budget = seam && G.debug_spa_budget > 0 ? G.debug_spa_budget : WIDE_SPA_BUDGET;
-    ResultCount rc;
-    rc.limit = seam && G.debug_gemm_limit > 0 ? G.debug_gemm_limit : WIDE_RESULT;
-    const int64_t *m_ptr = comp ? Mb->rowptr.get() : nullptr;
-    bool counting = false;
-    if (nrows > 0) {
-        DevBuf<unsigned long long> tot;
-        GB_TRY(tot.alloc(2, err));
-        CU_TRY(cudaMemsetAsync(tot, 0, 16, G.stream), err);
-        gemm_bound_kernel<BT><<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr, A.col, b_ptr, m_ptr, nrows, tot); GB_LAUNCHED();
-        unsigned long long h[2];
-        CU_TRY(cudaMemcpyAsync(h, tot, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
-        CU_TRY(cudaStreamSynchronize(G.stream), err);
-        if (h[1] >= (unsigned long long)rc.limit) return gb_fail(GrB_INVALID_VALUE, err, "%s", WIDE_RESULT_REFUSAL);
-        counting = h[0] >= (unsigned long long)rc.limit;
-    }
-    std::vector<Csr> parts;
-    DevBuf<int64_t> ends;
-    GB_TRY(ends.alloc(4, err));
-    // the panel that starts at row r0, formed into `part`; *r1 = its end.  Without M', A's offsets stand in for panel_end_kernel's M.
-    auto panel = [&](int64_t r0, int64_t *r1, Csr &part) -> GrB_Info {
-        panel_end_kernel<<<1, 1, 0, G.stream>>>(A.rowptr, comp ? m_ptr : A.rowptr.get(), r0, nrows, bound, WIDE_PANEL_ROWS, ends); GB_LAUNCHED();
-        int64_t h[4];
-        CU_TRY(cudaMemcpyAsync(h, ends, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
-        CU_TRY(cudaStreamSynchronize(G.stream), err);
-        *r1 = h[0];
-        const int64_t a0 = h[1], m0 = h[2], pn = *r1 - r0;
+        const int64_t a0 = h[1], m0 = h[2], m1 = h[3], pn = *r1 - r0;
         uint32_t *ap = nullptr, *mp = nullptr;
         GB_TRY(ws_array(WS_PANEL_A, &ap, (size_t)pn + 1, err));
         panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(A.rowptr, r0, pn, ap); GB_LAUNCHED();
-        if (comp) {
+        if (M) {
             GB_TRY(ws_array(WS_PANEL_M, &mp, (size_t)pn + 1, err));
-            panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(m_ptr, r0, pn, mp); GB_LAUNCHED();
+            panel_rowptr_kernel<<<grid_for(pn + 1), 256, 0, G.stream>>>(M->rowptr, r0, pn, mp); GB_LAUNCHED();
         }
-        const UnmaskedPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr,
-                              mp, comp ? Mb->col + m0 : nullptr, pn};
-        return spgemm_unmasked<BT>(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, budget, use, counting ? &rc : nullptr, nullptr, part,
-                                   err);
+        const RowPanel P{ap, A.col + a0, aval ? static_cast<const uint8_t *>(aval) + a0 * asz : nullptr, mp, M ? M->col + m0 : nullptr,
+                         M && msz ? static_cast<const uint8_t *>(M->val.get()) + m0 * msz : nullptr, pn, M ? m1 - m0 : 0};
+        return body(P, part);
     };
     int64_t r1 = 0;
     if (nrows > 0) {
@@ -1579,6 +1464,32 @@ static GrB_Info spgemm_unmasked_wide(const Csr &A, const Csr &B, const BT *b_ptr
         });
 }
 
+static void masked_report(const MaskedUse &u, bool wide) {
+    bool first = true;
+    auto entry = [&](const char *k) { gb_kernel_used(k); if (first && wide) gb_kernel_used("offsets=64"); first = false; };
+    if (u.dot) entry("dot");
+    if (u.warp) entry("masked-warp");
+    for (int k = 0; k < 3; ++k) {
+        if (!u.cls[k]) continue;
+        entry(k == 0 ? "stream-S" : (k == 1 ? "stream-M" : "stream-L"));
+        gb_kernel_used(u.exact[k] ? "filter=exact" : "filter=bloom");
+    }
+}
+
+// ------------------------------------------------------------------ the wide route of the unmasked and complemented-mask bins
+// The masked route's row panels (spgemm_panels, of A and M', the entries of a complemented mask that block): each panel runs the
+// whole pipeline (flops, bins, symbolic, scan, numeric) into a CSR of its rows; T is the one panel, or is formed from the panels'
+// row counts and entries.  B is read through its 64-bit offsets when it is wide.  The route forms results of fewer than 2^32
+// entries: T would take 34 GB or more in FP32 (twice that while the panels are joined), which does not fit beside a wide operand
+// on an 80 GB card.  gemm_bound_kernel bounds nnz(T) before any panel runs: L >= the limit is refused at once; U < the limit
+// needs no further check; otherwise the panels' symbolic counts are added up and the call refused as soon as the scan of a
+// panel's counts reaches the limit, before that panel's entries are allocated or formed.  The dense accumulators of a panel are capped at WIDE_SPA_BUDGET bytes (one FP32 accumulator is
+// 1 GB at n = 2^28).
+static constexpr int64_t WIDE_RESULT = (int64_t)1 << 32;
+static constexpr int64_t WIDE_SPA_BUDGET = (int64_t)1 << 32;
+// the route of a CSR x CSR product without a (non-complemented) mask: a CSR without rowptr32, or any CSR under B200_debug_wide_gemm
+static inline bool gemm_wide(const Csr &c) { return !c.rowptr32 || G.debug_wide_gemm > 0; }
+
 static void unmasked_report(const UnmaskedUse &u, bool wide) {
     static const char *const names[5] = {"esc-small", "esc-medium", "spa", "spa-split", "pull"};
     bool first = true;
@@ -1593,20 +1504,40 @@ static void unmasked_report(const UnmaskedUse &u, bool wide) {
 
 // T = A (+).(x) B, unmasked, or (A (+).(x) B)<!Mb> with Mb the entries of a complemented mask that block.  The narrow route runs
 // the bins once on the whole of A and Mb; the wide route (an operand or the mask of 2^32 or more entries, or B200_debug_wide_gemm)
-// on row panels, with B's 64-bit offsets when B is wide.  pull: the pull route of an eligible call (narrow only), or null.
+// on row panels, with B's 64-bit offsets when B is wide.  pull: the pull route of an eligible call, or null.
 static GrB_Info spgemm_unmasked_call(const Csr &A, const Csr &B, const void *aval, const void *bval, int xt, int zt, int add, int mul,
                                      bool need_a, bool need_b, const Csr *Mb, bool wide, PullSide *pull, Csr &T, std::string *err) {
-    const bool comp = Mb && Mb->nnz > 0;
+    const Csr *M = Mb && Mb->nnz > 0 ? Mb : nullptr;
+    const int64_t nrows = A.nrows;
+    const bool seam = G.debug_wide_gemm > 0;
+    const int64_t bound = std::min(seam ? G.debug_wide_gemm : WIDE_PANEL, WIDE_PANEL);
+    const int64_t budget = !wide ? 0 : seam && G.debug_spa_budget > 0 ? G.debug_spa_budget : WIDE_SPA_BUDGET;
+    ResultCount rc;
+    rc.limit = seam && G.debug_gemm_limit > 0 ? G.debug_gemm_limit : WIDE_RESULT;
     UnmaskedUse use;
     G.last_flops = 0;
-    if (!wide) {
-        const UnmaskedPanel P{A.rowptr32, A.col, aval, comp ? Mb->rowptr32.get() : nullptr, comp ? Mb->col.get() : nullptr, A.nrows};
-        GB_TRY(spgemm_unmasked<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, 0, use, nullptr, pull, T, err));
-    } else if (gemm_wide(B)) {
-        GB_TRY(spgemm_unmasked_wide<int64_t>(A, B, B.rowptr.get(), aval, bval, xt, zt, add, mul, need_a, need_b, Mb, use, T, err));
-    } else {
-        GB_TRY(spgemm_unmasked_wide<uint32_t>(A, B, B.rowptr32.get(), aval, bval, xt, zt, add, mul, need_a, need_b, Mb, use, T, err));
-    }
+    auto run = [&](auto b_ptr) -> GrB_Info {
+        bool counting = false;
+        if (wide && nrows > 0) {
+            DevBuf<unsigned long long> tot;
+            GB_TRY(tot.alloc(2, err));
+            CU_TRY(cudaMemsetAsync(tot, 0, 16, G.stream), err);
+            gemm_bound_kernel<<<grid_for(nrows * 32), 256, 0, G.stream>>>(A.rowptr, A.col, b_ptr, M ? M->rowptr.get() : nullptr, nrows, tot);
+            GB_LAUNCHED();
+            unsigned long long h[2];
+            CU_TRY(cudaMemcpyAsync(h, tot, sizeof(h), cudaMemcpyDeviceToHost, G.stream), err);
+            CU_TRY(cudaStreamSynchronize(G.stream), err);
+            if (h[1] >= (unsigned long long)rc.limit) return gb_fail(GrB_INVALID_VALUE, err, "%s", WIDE_RESULT_REFUSAL);
+            counting = h[0] >= (unsigned long long)rc.limit;
+        }
+        return spgemm_panels(A, aval, need_a ? tc_size(xt) : 0, M, 0, wide, bound, B.ncols, tc_size(zt), T, err,
+                             [&](const RowPanel &P, Csr &part) {
+                                 // the pull runs on the narrow route only
+                                 return spgemm_unmasked(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, budget, use,
+                                                        counting ? &rc : nullptr, wide ? nullptr : pull, part, err);
+                             });
+    };
+    GB_TRY(gemm_wide(B) ? run(B.rowptr.get()) : run(B.rowptr32.get()));
     G.last_nnz_out = (uint64_t)T.nnz;
     unmasked_report(use, wide);
     return GrB_SUCCESS;
@@ -1624,20 +1555,19 @@ static GrB_Info spgemm_masked(const Csr &A, const Csr &B, const void *aval, cons
     MaskedUse use;
     G.last_flops = 0;
     const bool wide = csr_wide(A) || csr_wide(B) || csr_wide(M);
-    if (!wide) {
-        DevBuf<void> typed;
-        void *words = nullptr; uint8_t *found = nullptr;
-        const MaskedPanel P{A.rowptr32, A.col, aval, M.rowptr32, M.col, M.val, nrows, M.nnz};
-        GB_TRY(masked_panel<uint32_t>(P, B, B.rowptr32.get(), bval, xt, zt, add, mul, need_a, need_b, mtc, m_struct, dot, ncols, trace,
-                                      use, &words, &found, typed, err));
-        GB_TRY(masked_compact(M, found, words, zsz, T, err));
-    } else if (csr_wide(B)) {
-        GB_TRY(spgemm_masked_wide<int64_t>(A, B, B.rowptr.get(), aval, bval, xt, zt, add, mul, need_a, need_b, M, mtc, m_struct, dot,
-                                           trace, use, T, err));
-    } else {
-        GB_TRY(spgemm_masked_wide<uint32_t>(A, B, B.rowptr32.get(), aval, bval, xt, zt, add, mul, need_a, need_b, M, mtc, m_struct, dot,
-                                            trace, use, T, err));
-    }
+    const int64_t bound = std::min(G.debug_wide > 0 ? wide_chunk() : WIDE_PANEL, WIDE_PANEL);
+    auto run = [&](auto b_ptr) {
+        return spgemm_panels(A, aval, need_a ? tc_size(xt) : 0, &M, M.val.get() ? tc_size(mtc) : 0, wide, bound, ncols, zsz, T, err,
+                             [&](const RowPanel &P, Csr &part) -> GrB_Info {
+                                 void *tval = nullptr; uint8_t *found = nullptr;
+                                 DevBuf<void> typed;
+                                 GB_TRY(masked_panel(P, B, b_ptr, bval, xt, zt, add, mul, need_a, need_b, mtc, m_struct, dot, ncols,
+                                                     trace, use, &tval, &found, typed, err));
+                                 return masked_compact_t<uint32_t>(P.nrows, ncols, P.mnnz, P.m_ptr, P.m_col, found, tval, zsz, part, err);
+                             });
+    };
+    GB_TRY(csr_wide(B) ? run(B.rowptr.get()) : run(B.rowptr32.get()));
+    G.last_nnz_out = (uint64_t)T.nnz;
     masked_report(use, wide);
     trace.mark("compaction");
     CU_TRY(cudaGetLastError(), err);
@@ -1733,6 +1663,16 @@ GrB_Info matrix_writeback(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryO
 // Values one operand gets in place of its own (the inner form of a positional multiply): side 1 = each entry of op(A) its column
 // index, side 2 = each entry of op(B) its row index; through ids (hypersparse operands) when given, plus off, of type tc
 struct MxmPos { int side = 0; int tc = 0; int64_t off = 0; const uint64_t *ids = nullptr; };
+// *out = the values of c (op(A) on side 1, op(B) or op(B)' on side 2; of type tc) as the multiply reads them: pos's index of each
+// entry, its column when by_col, else its row, when pos.side is this side; else mxm_values.  The buffer belongs to the caller.
+static GrB_Info mxm_csr_values(DevBuf<void> &cast, const void **out, const Csr &c, int tc, bool reads, int xt, const MxmPos &pos,
+                               int side, bool by_col, std::string *err) {
+    if (pos.side != side) return mxm_values(cast, out, reads, xt, c.val, tc, c.nnz, err);
+    GB_TRY(cast.alloc((size_t)c.nnz * tc_size(pos.tc) + 16, err));
+    GB_TRY(pos_csr_values(cast, pos.tc, nullptr, OP_ANY, c, by_col, pos.ids, pos.off, err));
+    *out = cast;
+    return GrB_SUCCESS;
+}
 
 // T = op(A) (+).(x) op(B) under Mask (*masked tells the write-back): a mask that is not complemented selects the masked
 // methods; a complemented one runs the unmasked bins with the filter of the entries that block (DESIGN.md section 3.2)
@@ -1758,18 +1698,10 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
                                               (double)(a.nrows + b.nrows + 2) * 8);
 
     DevBuf<void> a_cast, b_cast;
-    const void *aval = a.val, *bval = b.val;
-    if (pos.side == 1) {
-        GB_TRY(a_cast.alloc((size_t)a.nnz * tc_size(pos.tc) + 16, err));
-        GB_TRY(pos_csr_values(a_cast, pos.tc, nullptr, OP_ANY, a, /*by_col=*/true, pos.ids, pos.off, err));
-        aval = a_cast;
-    } else if (need_a && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
-    if (pos.side == 2) {
-        // op(B)'s row index: the row of b, or its column when b is B itself standing for B' (the dot method)
-        GB_TRY(b_cast.alloc((size_t)b.nnz * tc_size(pos.tc) + 16, err));
-        GB_TRY(pos_csr_values(b_cast, pos.tc, nullptr, OP_ANY, b, /*by_col=*/f.tran1 && dot, pos.ids, pos.off, err));
-        bval = b_cast;
-    } else if (need_b && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
+    const void *aval = nullptr, *bval = nullptr;
+    GB_TRY(mxm_csr_values(a_cast, &aval, a, A->type->code, need_a, xt, pos, 1, /*by_col=*/true, err));
+    // op(B)'s row index: the row of b, or its column when b is B itself standing for B' (the dot method)
+    GB_TRY(mxm_csr_values(b_cast, &bval, b, B->type->code, need_b, xt, pos, 2, /*by_col=*/f.tran1 && dot, err));
 
     GrB_Info r;
     if (use_mask) r = spgemm_masked(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, Mask->dev, Mask->type->code, f.mask_struct, dot, T, err);
@@ -1778,11 +1710,11 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
         const Csr *mb = nullptr;
         if (Mask && f.mask_struct) mb = &Mask->dev;
         else if (Mask) { GB_TRY(mask_true_pattern(Mask->dev, Mask->type->code, mtrue, err)); mb = &mtrue; }
-        // a complemented mask and a saturating monoid on the narrow route: GxB_AxB_DOT pulls every row with products, the
-        // default descriptor the rows the B200GRB_MXM_PULL rule picks (DESIGN.md section 3.2)
+        // a complemented mask and a saturating monoid (on the narrow route: spgemm_unmasked_call): GxB_AxB_DOT pulls every row
+        // with products, the default descriptor the rows the B200GRB_MXM_PULL rule picks (DESIGN.md section 3.2)
         PullSide ps;
         DevBuf<void> bt_cast;
-        const bool eligible = Mask && !wide && (add == OP_LOR || add == OP_LAND || add == OP_ANY);
+        const bool eligible = Mask && (add == OP_LOR || add == OP_LAND || add == OP_ANY);
         if (eligible) {
             ps.dot = f.axb == GxB_AxB_DOT;
             ps.alpha = f.axb == GxB_DEFAULT ? tunables().mxm_pull : 0.0;
@@ -1792,16 +1724,8 @@ static GrB_Info mxm_product(const GrB_Matrix Mask, const DescFlags &f, int xt, i
                 if (!f.tran1) GB_TRY(matrix_ensure_transpose(B));
                 const Csr &bt = f.tran1 ? B->dev : B->devT;
                 if (!bt.rowptr32) return gb_fail(GrB_PANIC, err, "GrB_mxm: the pull route needs 32-bit offsets of op(B)'");
-                o.bt_ptr = bt.rowptr32; o.bt_col = bt.col; o.bt_val = bt.val;
-                if (pos.side == 2) {
-                    GB_TRY(bt_cast.alloc((size_t)bt.nnz * tc_size(pos.tc) + 16, err));
-                    GB_TRY(pos_csr_values(bt_cast, pos.tc, nullptr, OP_ANY, bt, /*by_col=*/true, pos.ids, pos.off, err));
-                    o.bt_val = bt_cast;
-                } else if (need_b && B->type->code != xt) {
-                    GB_TRY(dev_cast_values(bt_cast, xt, bt.val, B->type->code, bt.nnz, err));
-                    o.bt_val = bt_cast;
-                }
-                return GrB_SUCCESS;
+                o.bt_ptr = bt.rowptr32; o.bt_col = bt.col;
+                return mxm_csr_values(bt_cast, &o.bt_val, bt, B->type->code, need_b, xt, pos, 2, /*by_col=*/true, err);
             };
         }
         r = spgemm_unmasked_call(a, b, aval, bval, xt, zt, add, mul, need_a, need_b, mb, wide, eligible ? &ps : nullptr, T, err);

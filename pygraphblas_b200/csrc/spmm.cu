@@ -376,9 +376,9 @@ GrB_Info spmm_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp accum,
     const int64_t m = a.nrows, n = a.ncols, k = (int64_t)B->ncols;
     // operands cast to the multiply's input types, as in the CSR path
     DevBuf<void> a_cast, x_cast;
-    const void *aval = a.val, *xval = B->dn.val;
-    if (mul_reads_x(mul) && A->type->code != xt) { GB_TRY(dev_cast_values(a_cast, xt, a.val, A->type->code, a.nnz, err)); aval = a_cast; }
-    if (mul_reads_y(mul) && B->type->code != xt) { GB_TRY(dev_cast_values(x_cast, xt, B->dn.val, B->type->code, n * k, err)); xval = x_cast; }
+    const void *aval = nullptr, *xval = nullptr;
+    GB_TRY(mxm_values(a_cast, &aval, mul_reads_x(mul), xt, a.val, A->type->code, a.nnz, err));
+    GB_TRY(mxm_values(x_cast, &xval, mul_reads_y(mul), xt, B->dn.val, B->type->code, n * k, err));
     // T in fresh buffers: C may alias A or X
     DevBuf<void> tval; DevBuf<uint8_t> tpres;
     GB_TRY(tval.alloc((size_t)(m * k) * tc_size(zt) + 16, err));
@@ -425,10 +425,10 @@ GrB_Info spmm_left_mxm(GrB_Matrix C, const GrB_Matrix Mask, const GrB_BinaryOp a
     const int64_t m = b.nrows, n = b.ncols, k = (int64_t)(f.tran0 ? A->ncols : A->nrows);
     // operands cast to the multiply's input types, as in the CSR path: op(B)' takes the swapped multiply's x, X its y
     DevBuf<void> b_cast, x_cast;
-    const void *bval = b.val, *xval = A->dn.val;
+    const void *bval = nullptr, *xval = nullptr;
     const uint8_t *xpres = A->dn.pres;
-    if (mul_reads_x(mul) && B->type->code != xt) { GB_TRY(dev_cast_values(b_cast, xt, b.val, B->type->code, b.nnz, err)); bval = b_cast; }
-    if (mul_reads_y(mul) && A->type->code != xt) { GB_TRY(dev_cast_values(x_cast, xt, A->dn.val, A->type->code, n * k, err)); xval = x_cast; }
+    GB_TRY(mxm_values(b_cast, &bval, mul_reads_x(mul), xt, b.val, B->type->code, b.nnz, err));
+    GB_TRY(mxm_values(x_cast, &xval, mul_reads_y(mul), xt, A->dn.val, A->type->code, n * k, err));
     // X' (n x k): the row-major k x n form transposed, unless A already is n x k (INP0 = TRAN) or k = 1
     const bool xtr = !f.tran0 && k > 1;
     const size_t bx = mul_reads_y(mul) ? tc_size(xt) : tc_size(A->type->code);
